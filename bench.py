@@ -22,14 +22,22 @@ One JSON line on stdout (rank 0):
              steps, D2H of the per-batch losses.  Two consecutive calls; `value`
              is the second, `first_call_value` the first (allocator cold).
   roofline   dominant kernel: algorithmic bytes / CUDA-event duration vs the
-             measured HBM copy bandwidth (MEASURED_PEAKS.json)
-  cpu_baseline  the unmodified reference (baseline/_ref, kind "reference"; the
+             measured HBM copy bandwidth (MEASURED_PEAKS.json; without it the
+             H100 SXM data-sheet 3350 GB/s, labelled as such)
+  cpu_baseline  the unmodified reference (oracle/_ref, kind "reference"; the
              torch-CPU restatement oracle/torch_port.py, kind "port", only if the
              install is absent) timed on this box's host cores on a bounded sample
              of the same workload
 
 ``--impl reference`` times only that CPU arm (all host threads) on the same
 config and prints the same line shape with "impl": "reference".
+
+``--dump-outputs DIR`` (single GPU) writes, right after the timed steps, what they
+computed: the epoch loss and the trained parameters (every row of a table that fits
+its share, else a fixed seeded sample of its rows, with the row ids) as
+DIR/<name>.npy, float32 / float64, under 64 MB at any shape.
+The inputs depend only on the arguments, so two builds can be compared output for
+output.
 """
 
 import argparse
@@ -65,6 +73,8 @@ def parse():
     ap.add_argument('--no-cpu-baseline', action='store_true')
     ap.add_argument('--no-e2e', action='store_true')
     ap.add_argument('--exchange', default='auto', choices=['auto', 'a2a', 'dense'])
+    ap.add_argument('--dump-outputs', default=None, metavar='DIR',
+                    help='write what the timed steps computed as DIR/<name>.npy')
     return ap.parse_args()
 
 
@@ -75,7 +85,7 @@ def workload_config(a, n_gpus):
             'batch': a.batch, 'optimizer': 'adagrad(lr=%g), row-wise fused' % a.lr,
             'negatives': 'device MT19937 masked rejection (numpy-bit-exact)',
             'parallelism': 'single GPU' if n_gpus == 1 else 'replicas x%d' % n_gpus,
-            'l2': 'inputs (embedding tables 282 MB + ids) exceed the 126 MB L2; no flush'}
+            'l2': 'inputs (embedding tables 282 MB + ids) exceed the 50 MB L2; no flush'}
 
 
 # --------------------------------------------------------------------------
@@ -200,13 +210,13 @@ class ClockSampler(object):
 # CPU port (cpu_baseline and the reference arm)
 # --------------------------------------------------------------------------
 
-REF_DIR = os.path.join(ROOT, 'baseline', '_ref')
+REF_DIR = os.path.join(ROOT, 'oracle', '_ref')
 
 
 def _reference_runner(a):
-    """fit_steps(lo, nsteps) on the UNMODIFIED reference (baseline/_ref, pip-installed from
-    /root/reference: `spotlight.factorization.implicit.ImplicitFactorizationModel.fit` on CPU
-    through its own public API), or None when the install is not on this box."""
+    """fit_steps(lo, nsteps) on the UNMODIFIED reference (oracle/_ref, placed there by
+    build() through oracle/build_ref.py: `spotlight.factorization.implicit.ImplicitFactorizationModel.fit`
+    on CPU through its own public API), or None when it is not installed."""
     if not os.path.isdir(os.path.join(REF_DIR, 'spotlight')):
         return None
     import torch
@@ -244,7 +254,7 @@ def _port_runner(a):
 def run_cpu_port(a, steps, warmup):
     """interactions/s of the reference's CPU fit() loop on this box's host cores.
 
-    kind "reference": the unmodified reference from baseline/_ref (stock code path, its own
+    kind "reference": the unmodified reference from oracle/_ref (stock code path, its own
     shuffle, sampler, autograd and the same Adagrad optimizer handed in through its
     `optimizer_func`); kind "port": oracle/torch_port.py, the same loop restated on stock
     torch CPU ops, when the install is absent.
@@ -279,7 +289,7 @@ def run_cpu_port(a, steps, warmup):
     t0 = time.perf_counter()
     fit_steps(users[lo:], items[lo:], steps)
     dt = time.perf_counter() - t0
-    what = ('unmodified reference (baseline/_ref: spotlight.factorization.implicit.'
+    what = ('unmodified reference (oracle/_ref: spotlight.factorization.implicit.'
             'ImplicitFactorizationModel.fit, use_cuda=False)' if kind == 'reference'
             else 'reference loop restated on torch CPU ops (oracle/torch_port.py)')
     return {'value': steps * B / dt, 'unit': UNIT, 'cores': best, 'kind': kind,
@@ -293,10 +303,10 @@ def main_reference(a):
     rank = int(os.environ.get('RANK', '0'))
     if rank != 0:
         return
-    # each reference step is O(table + batch) (about a second at the default batch on the box's
-    # host cores): K and W are honoured up to a bound that keeps the arm within a few minutes
-    steps = max(1, min(a.steps, 60))
-    warm = max(1, min(a.warmup, 5))
+    # each reference step is O(table + batch): about a second at the default batch on a
+    # many-core host, so large K make this arm take minutes
+    steps = max(1, a.steps)
+    warm = max(1, a.warmup)
     r = run_cpu_port(a, steps, warm)
     line = {'impl': 'reference', 'metric': METRIC, 'value': r['value'], 'unit': UNIT,
             'n_gpus': a.gpus, 'steps': steps, 'warmup': warm, 'ms_per_step': r['ms_per_step'],
@@ -541,10 +551,35 @@ def main_sharded(a, rank, world, local):
                            # the same window through the GPU's NVLink hardware counters (NVML field
                            # values NVLINK_THROUGHPUT_DATA_TX / RX of rank 0's GPU, all links)
                            'hw_counters': hw_nv,
-                           'peak_gbs_per_direction': 900.0},
+                           'peak_gbs_per_direction': 450.0},       # H100 SXM NVLink 4, 18 links
                 'roofline': None, 'cpu_baseline': None}
         print(json.dumps(line))
     dist.destroy_process_group()
+
+
+def dump_outputs(model, epoch_loss, out_dir):
+    """What the timed steps computed: the epoch loss and the parameters after the last step.
+    Each table keeps its rows whole when they fit 28 MiB (embedding + bias, fp32), else a fixed
+    seeded sample of that many rows; row ids are capped at 2^17 per table, so the files stay
+    under 64 MB at any shape."""
+    import torch
+    net = model._net
+    torch.cuda.synchronize()
+    os.makedirs(out_dir, exist_ok=True)
+    arrays = {'epoch_loss': np.array([epoch_loss], dtype=np.float64)}
+    for seed, side in enumerate(('user', 'item')):
+        emb = getattr(net, side + '_embeddings').weight
+        bias = getattr(net, side + '_biases').weight
+        n, dim = emb.shape
+        cap = min(1 << 17, (28 << 20) // (4 * (dim + 1)))
+        rows = np.arange(n) if n <= cap else np.sort(np.random.RandomState(seed).choice(n, cap, replace=False))
+        idx = torch.from_numpy(rows).to(emb.device)
+        with torch.no_grad():
+            arrays[side + '_rows'] = rows.astype(np.float64)
+            arrays[side + '_embeddings'] = emb[idx].cpu().numpy()
+            arrays[side + '_biases'] = bias[idx].cpu().numpy()
+    for name, v in arrays.items():
+        np.save(os.path.join(out_dir, name + '.npy'), np.ascontiguousarray(v, dtype=v.dtype))
 
 
 def main_ours(a):
@@ -554,6 +589,8 @@ def main_ours(a):
     world = int(os.environ.get('WORLD_SIZE', '1'))
     local = int(os.environ.get('LOCAL_RANK', '0'))
     if world > 1:
+        if a.dump_outputs:
+            raise SystemExit('--dump-outputs is a single-GPU option')
         return main_sharded(a, rank, world, local)
     sampler = ClockSampler(local).start() if rank == 0 else None      # long before the timed region
     model = build_model(a, local)
@@ -599,6 +636,8 @@ def main_ours(a):
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
     ms = float(t.item())
     value = world * K * B / (ms * 1e-3)
+    if a.dump_outputs and rank == 0:
+        dump_outputs(model, epoch_loss, a.dump_outputs)
 
     # ---- end to end through the public API (host ids) -------------------
     e2e = None
@@ -644,31 +683,23 @@ def main_ours(a):
         peaks = json.load(open(os.path.join(ROOT, 'MEASURED_PEAKS.json')))
     except (OSError, ValueError):
         pass
-    peak = float(peaks.get('hbm_gbs', 6650.0))
+    peak = float(peaks.get('hbm_gbs', 3350.0))
     R = 4 * a.dim
     if 'mf_user' in kb:     # planned step (DESIGN.md section 3): bytes / interaction, rows counted per use
         # mf_user: reads U, Q+, Q- rows + 3 biases + one 16-byte plan record; writes the updated U row + 2 g
         # mf_item: reads the 2 stashed user rows + 2 x (8-byte record + g); writes the 2 updated item rows
         alg = {'mf_user': 4 * R + 36, 'mf_item': 4 * R + 32}
-        traffic_file = 'traffic_r02.json'
     else:
         alg = {'mf_fwd': 3 * R + 60, 'mf_bwd': 7 * R + 84}
-        traffic_file = 'traffic_r01j.json'
     dom = max(alg, key=lambda k: kb[k])
     achieved = alg[dom] * B / (kb[dom] * 1e-3) / 1e9
     step_ms = sum(kb.values())
-    traffic = None
-    try:        # DRAM bytes of the dominant kernel from the committed ncu --set full capture
-        tr = json.load(open(os.path.join(ROOT, 'profiles', traffic_file)))
-        if tr['batch'] == B and tr['dim'] == a.dim:
-            traffic = tr['dram_bytes_per_launch'].get(dom)
-    except (OSError, ValueError, KeyError):
-        pass
     step_bytes = (6 * R + 40) * B
     roofline = {'bound': 'hbm', 'kernel': dom, 'achieved': achieved, 'peak': peak, 'unit': 'GB/s',
-                'frac': achieved / peak, 'traffic': traffic,
+                'frac': achieved / peak,
                 'algorithmic_bytes_per_launch': alg[dom] * B,
-                'peak_source': 'MEASURED_PEAKS.json hbm_gbs (measured copy)' if peaks else 'fallback 6650',
+                'peak_source': ('MEASURED_PEAKS.json hbm_gbs (measured copy)' if peaks
+                                else 'H100 SXM data sheet (3350 GB/s, not measured)'),
                 'algorithmic_bytes_per_interaction': alg[dom],
                 'kernel_ms': kb,
                 'per_kernel_frac': {k: alg[k] * B / (kb[k] * 1e-3) / 1e9 / peak for k in alg},

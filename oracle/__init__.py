@@ -25,6 +25,6 @@ restatements are NumPy, so there is no C build step for the oracle.
 
 Parity pinning: the restatements are checked (tests/test_oracle_*.py) against
 golden vectors produced by the *live* reference in the build container
-(``tests/golden/make_golden.py`` imports ``/root/reference``), against NumPy's
+(``tests/golden/make_golden.py`` imports a reference checkout), against NumPy's
 own ``RandomState`` and against ``sklearn.utils.murmurhash3_32``.
 """

@@ -1,8 +1,9 @@
 """The reference's fit() loop restated on stock torch CPU ops (oracle).
 
 TEST INFRASTRUCTURE / TIMED CPU BASELINE ONLY -- never imported by
-``spotlight_b200``.  The reference is pure Python over ATen; it cannot travel
-to the GPU box (no /root/reference there), so this module restates its hot
+``spotlight_b200``.  The reference is pure Python over ATen and is not part of
+this repository (bench.py uses it only when build() placed it in oracle/_ref),
+so this module restates its hot
 path with the *same* ATen ops in the same order, which gives the same
 arithmetic and the same performance characteristics on the host cores:
 

@@ -1,4 +1,4 @@
-"""Secondary measurement (not the driver's bench contract): sequence-model training
+"""Secondary measurement (not bench.py's headline metric): sequence-model training
 step, BASELINE.json configs[4] shape -- 1M items, dim 128, S = 200, pointwise loss,
 PoolNet and CNNNet(k=3, 1 layer).  Prints positions/s (CUDA events, K steps)."""
 import argparse, json, os, sys

@@ -23,7 +23,7 @@ for line in txt.splitlines():
         cur = None
 names = subprocess.run(['c++filt'], input='\n'.join(r[0] for r in rows), capture_output=True,
                        text=True).stdout.splitlines()
-print('# cuobjdump --dump-resource-usage spotlight_b200/libspotlight_b200.so  (sm_100a, -O3 -lineinfo)')
+print('# cuobjdump --dump-resource-usage spotlight_b200/libspotlight_b200.so  (sm_90a, -O3 -lineinfo)')
 print('# %d kernels; regs  stack  static_smem  local  kernel' % len(rows))
 out = []
 for (n, reg, stack, sh, loc), d in zip(rows, names):

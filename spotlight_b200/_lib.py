@@ -176,7 +176,7 @@ def load():
         if not os.path.exists(LIB_PATH):
             raise LibraryError(
                 'spotlight_b200: %s not found. Build it with '
-                '`python -c "import __graft_entry__ as g; g.build()"` (needs nvcc, sm_100a). '
+                '`python -c "import __graft_entry__ as g; g.build()"` (needs nvcc, sm_90a). '
                 'There is no CPU fallback.' % LIB_PATH)
         lib = ctypes.CDLL(LIB_PATH)
         missing = [n for n in EXPORTS if not hasattr(lib, n)]

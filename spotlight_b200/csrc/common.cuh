@@ -1,4 +1,4 @@
-// Shared device/host helpers for the spotlight_b200 kernels (sm_100a).
+// Shared device/host helpers for the spotlight_b200 kernels (sm_90a).
 #pragma once
 
 #include <cuda_runtime.h>

@@ -1,4 +1,4 @@
-// Embedding gathers and their deterministic backward for sm_100a.
+// Embedding gathers and their deterministic backward for sm_90a.
 //
 // Replaces ScaledEmbedding / ZeroEmbedding / BloomEmbedding forward
 // (spotlight/layers.py:23-56, 206-244: nn.Embedding lookup; Bloom = index_select

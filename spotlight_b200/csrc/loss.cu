@@ -6,7 +6,7 @@
 namespace {
 
 constexpr int L_THREADS = 256;
-constexpr int L_MAX_GRID = 148 * 8;
+constexpr int L_MAX_GRID = 132 * 8;
 
 __device__ __forceinline__ void elem_loss(int loss, float p, float n, float& per, float& gp, float& gn) {
     if (loss == SLB_LOSS_BPR) {

@@ -1,4 +1,4 @@
-// Fused implicit-feedback matrix-factorisation training step for sm_100a.
+// Fused implicit-feedback matrix-factorisation training step for sm_90a.
 //
 // Replaces the loop body of ImplicitFactorizationModel.fit
 // (spotlight/factorization/implicit.py:229-242): two BilinearNet forwards
@@ -201,7 +201,7 @@ __global__ void __launch_bounds__(MF_TILE_THREADS) mf_fwd_tile_kernel(MfDev a) {
     const int gl = lane & (LPR - 1);
     const int grp = lane / LPR;
     // EX: the row is exactly one 128-bit load per lane (D == 4 * LPR), so D is a compile-time
-    // constant: no column loop, shifts for the row offsets (B200, D = 64: step 476 -> 431 us)
+    // constant: no column loop, shifts for the row offsets
     const int D = EX ? LPR * 4 : a.D;
     const float invB = 1.0f / static_cast<float>(a.NB);
     const int64_t ntiles = (a.B + TI - 1) / TI;
@@ -305,9 +305,6 @@ __device__ __forceinline__ void cswap(int& x, int& y) {
 // Sorted (5..CAP-term) segments: once the partner row ids are known (lane-parallel, after
 // the shared-memory sort) each lane asks L2 for its partners' rows, so the row walk that
 // follows -- GEN_CHUNK rows in flight per lane -- runs at L2 rather than HBM latency.
-// Measured at B = 524 288 (item rows average 10.5 terms): backward 301 -> 266 us.  The same
-// prefetch for a segment's own weight / state rows, and for short segments' partners, was
-// slower (+12 us), as were 16-row chunks and walking two user segments at once (spills).
 #ifndef GEN_CHUNK
 #define GEN_CHUNK 8
 #endif
@@ -316,11 +313,11 @@ __device__ __forceinline__ void pf_row_l2(const float* row, int D) {
     for (int o = 0; o < D * 4; o += 128) asm volatile("prefetch.global.L2 [%0];" ::"l"(p + o));
 }
 
-// BWD_BULK (default 0; round-2 experiment, built only through profiles/run_variants.sh):
+// BWD_BULK (default 0; experiment, built only through profiles/build_variant.sh):
 // the user-side kernel (MODE 2, exact row width) stages the weight / optimizer-state rows of a
 // whole 32-segment tile in shared memory with one cp.async.bulk per row, completion on one
-// mbarrier per warp -- 16 KB in flight per warp without holding a register.  NOT yet run on
-// hardware: it compiles for sm_100a (SASS: UBLKCP) and is off in the shipped library.
+// mbarrier per warp -- 16 KB in flight per warp without holding a register.  Not run on
+// hardware: it compiles for sm_90a (SASS: UBLKCP) and is off in the shipped library.
 #ifndef BWD_BULK
 #define BWD_BULK 0
 #endif
@@ -375,7 +372,7 @@ __global__ void __launch_bounds__(MF_TILE_THREADS, MODE == 1 ? BWD_MINB1 : BWD_M
     const unsigned gmask = group_mask(LPR);
     int32_t* sh = sh_all + ((threadIdx.x >> 5) * GPW + grp) * 4 * CAP;
     // EX: the row is exactly one 128-bit load per lane (D == 4 * LPR), so D is a compile-time
-    // constant: no column loop, shifts for the row offsets (B200, D = 64: step 476 -> 431 us)
+    // constant: no column loop, shifts for the row offsets
     const int D = EX ? LPR * 4 : a.D;
 #if defined(BWD_OPT_CT)
     // round-2 experiment (off unless -DBWD_OPT_CT=<SLB_OPT_* value>): the optimizer kind is a
@@ -793,7 +790,7 @@ __global__ void __launch_bounds__(MF_THREADS) mf_apply_kernel(MfDev a) {
     }
 }
 
-constexpr int MF_MAX_GRID = 148 * 16;
+constexpr int MF_MAX_GRID = 132 * 16;
 
 #include "mf_v2.cuh"
 #include "mf_adam.cuh"

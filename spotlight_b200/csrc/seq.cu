@@ -1,4 +1,4 @@
-// Sequence-model training step for sm_100a: PoolNet and CNNNet.
+// Sequence-model training step for sm_90a: PoolNet and CNNNet.
 //
 // Replaces the loop body of ImplicitSequenceModel.fit
 // (spotlight/sequence/implicit.py:230-255): user_representation
@@ -16,7 +16,8 @@
 //                        the time axis (two-level scan through shared memory)
 //   conv_gemm_kernel     causal dilated conv as a shifted-row GEMM on the tensor cores
 //                        (mma.sync TF32, 3xTF32 split for fp32-level accuracy, 64x64x16
-//                        tiles): forward (+bias, act, residual) and input-gradient modes
+//                        tiles): forward (+bias, act, residual) and input-gradient modes;
+//                        at D = 128 tc_conv_gemm_kernel / tc_conv_dw_kernel (wgmma, seq_tc.cuh)
 //   conv_dw_kernel       weight gradient, split over positions + fixed-order reduce
 //   seq_score_kernel     one lane group per position: dots, loss, d loss/d r,
 //                        target-role contribution rows, row counts
@@ -29,7 +30,7 @@
 namespace {
 
 constexpr int SQ_THREADS = 256;
-constexpr int SQ_MAX_GRID = 148 * 8;
+constexpr int SQ_MAX_GRID = 132 * 8;
 constexpr int MAX_LAYERS = 8;
 
 struct SeqDev {
@@ -710,9 +711,12 @@ struct SeqLayout {
     size_t bytes;
 };
 
+// The weight-gradient split counts follow the device's SM count: the fixed-order reduction
+// over splits is deterministic on one GPU model, but its summation order (and so the last
+// bits of dW) can differ between models with different SM counts.
 int dw_splits(int64_t M, int D, int k) {
     const int tiles = ((D + GM - 1) / GM) * ((D + GN - 1) / GN) * k;
-    int s = (2 * 148 + tiles - 1) / tiles;
+    int s = (2 * slb_sms() + tiles - 1) / tiles;
     if (s < 1) s = 1;
     if (s > 128) s = 128;
     const int64_t maxs = (M + GK - 1) / GK;
@@ -720,14 +724,14 @@ int dw_splits(int64_t M, int D, int k) {
     return s;
 }
 
-// tcgen05 path: D == 128 exactly (one 128 x 128 tile spans all channels)
+// wgmma path: D == 128 exactly (one 128 x 128 tile spans all channels)
 bool use_tc(int D) {
-    static const bool disabled = getenv("SLB_NO_TCGEN05") != nullptr;
+    static const bool disabled = getenv("SLB_NO_WGMMA") != nullptr;
     return !disabled && D == 128;
 }
 
 int dw_splits_tc(int64_t M, int k) {
-    int s = (2 * 148 + k - 1) / k;
+    int s = (2 * slb_sms() + k - 1) / k;
     const int64_t maxs = (M + tc::KC - 1) / tc::KC;
     if (s > maxs) s = static_cast<int>(maxs);
     return s < 1 ? 1 : s;
@@ -884,9 +888,9 @@ int run_representation(const slb_seq_step_args* x, const SeqLayout& l, float* re
         }
         if (!x->residual && !(last && rep_dst)) g.Out = l.A[i];
         if (use_tc(D)) {
-            SLB_REQUIRE(l.Wb[i] != nullptr, "seq: tcgen05 forward needs the [k][out][in] weight copy");
+            SLB_REQUIRE(l.Wb[i] != nullptr, "seq: wgmma forward needs the [k][out][in] weight copy");
             g.Wm = l.Wb[i];                                  // [j][n = out][c = in]
-            if (tc_configure(tc::tc_conv_gemm_kernel) != 0) { slb_set_error("seq: cannot configure tcgen05 kernel"); return SLB_ECUDA; }
+            if (tc_configure(tc::tc_conv_gemm_kernel) != 0) { slb_set_error("seq: cannot configure wgmma kernel"); return SLB_ECUDA; }
             tc::tc_conv_gemm_kernel<<<static_cast<unsigned>((B * T + tc::TM - 1) / tc::TM), 128, tc::SMEM_BYTES, st>>>(g);
             SLB_LAUNCH_CHECK("tc_conv_gemm_kernel(fwd)");
         } else {
@@ -977,7 +981,7 @@ int slb_seq_train_step(const slb_seq_step_args* x, slb_stream_t stream) {
             w.slab = ((B * T + splits - 1) / splits + slab_q - 1) / slab_q * slab_q;
             w.part = l.part; w.bpart = l.bpart;
             if (tcp) {
-                if (tc_configure(tc::tc_conv_dw_kernel) != 0) { slb_set_error("seq: cannot configure tcgen05 kernel"); return SLB_ECUDA; }
+                if (tc_configure(tc::tc_conv_dw_kernel) != 0) { slb_set_error("seq: cannot configure wgmma kernel"); return SLB_ECUDA; }
                 dim3 wg(static_cast<unsigned>(k), static_cast<unsigned>(splits));
                 tc::tc_conv_dw_kernel<<<wg, 128, tc::SMEM_BYTES, st>>>(w);
                 SLB_LAUNCH_CHECK("tc_conv_dw_kernel");

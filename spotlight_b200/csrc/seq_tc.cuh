@@ -1,25 +1,25 @@
-// tcgen05 (5th-generation tensor core) path of the CNNNet causal convolution for
+// Warpgroup tensor-core (wgmma, sm_90a) path of the CNNNet causal convolution for
 // D = 128 -- BASELINE configs[4].  Included by seq.cu after ConvGemm / ConvDw.
 //
 // The conv is a dense contraction (SURVEY §8a row Q2): per layer
 //   forward / input-gradient : Out[(b,t), n] = sum_{j<k} sum_c In[b, t + shift_j, c] * W_j[n][c]
 //   weight gradient          : dW_j[i][o]    = sum_{(b,t)} In[b, t + shift_j, i] * dZ[(b,t), o]
-// Both run as 128 x 128 output tiles with the accumulator in TMEM (128 lanes x
-// 128 fp32 columns) and tcgen05.mma.kind::tf32 issued by one thread.  fp32-level
-// accuracy (the 1e-5 parity budget) comes from the 3xTF32 split: every operand
-// chunk is staged twice in shared memory (hi = tf32(x), lo = tf32(x - hi)) and
-// each K step issues lo*hi + hi*lo + hi*hi into the same accumulator.
+// Both run as 128 x 128 output tiles computed by one warpgroup (128 threads): two
+// wgmma.mma_async m64n128k8 tf32 per K step (rows 0..63 and 64..127), fp32
+// accumulators in registers (2 x 64 per thread).  fp32-level accuracy (the 1e-5
+// parity budget) comes from the 3xTF32 split: every operand chunk is staged twice
+// in shared memory (hi = tf32(x), lo = tf32(x - hi)) and each K step issues
+// lo*hi + hi*lo + hi*hi into the same accumulator.
 //
 // Operands are staged by the CUDA cores (the split has to touch every element
-// anyway) straight into the no-swizzle canonical UMMA layouts:
-//   K-major  (forward/dX): 8 rows x 16 B core matrices, element (r, k) at
-//            (r/8)*SBO + (k/4)*LBO + (r%8)*16 + (k%4)*4,  LBO = 128, SBO = 1024
-// The weight gradient contracts over positions, which are the *outer* index of its
-// operands in memory; its staging transposes 4 x 4 register blocks so it can use the
-// same K-major layout.
-// One mbarrier tracks MMA completion (tcgen05.commit); the pipeline is single
-// stage (stage -> fence -> MMA -> wait), which already moves the math off the
-// CUDA cores; multi-stage TMA feeding is the next step.
+// anyway) straight into the no-swizzle canonical K-major layout of the shared
+// memory matrix descriptors: 8 rows x 16 B core matrices, element (r, k) at
+//   (r/8)*SBO + (k/4)*LBO + (r%8)*16 + (k%4)*4,  LBO = 128, SBO = 1024
+// (tf32 wgmma takes K-major operands only).  The weight gradient contracts over
+// positions, which are the *outer* index of its operands in memory; its staging
+// transposes 4 x 4 register blocks so it can use the same K-major layout.
+// The pipeline is single stage (stage -> fence -> wgmma -> wait); the weight
+// gradient's bias column sums run while the MMAs of a chunk are in flight.
 #pragma once
 
 namespace tc {
@@ -28,96 +28,84 @@ constexpr int TM = 128;          // tile rows (positions / in-channels)
 constexpr int TN = 128;          // tile cols (= D)
 constexpr int KC = 32;           // K elements staged per chunk (4 MMA k-steps of 8)
 constexpr int TILE_BYTES = TM * KC * 4;          // 16 KB per staged operand copy
-constexpr int SMEM_BYTES = 4 * TILE_BYTES + 64;  // A_hi, A_lo, B_hi, B_lo + barrier + tmem ptr
+constexpr int SMEM_BYTES = 4 * TILE_BYTES;       // A_hi, A_lo, B_hi, B_lo
+constexpr uint32_t LBO = 128;                    // next core matrix along K
+constexpr uint32_t SBO = 1024;                   // next 8-row group
+constexpr uint32_t HALF_BYTES = 8 * SBO;         // rows 64..127 of a staged operand
+constexpr uint32_t KSTEP_BYTES = 2 * LBO;        // 8 tf32 of K = two core matrices
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
     return static_cast<uint32_t>(__cvta_generic_to_shared(p));
 }
-__device__ __forceinline__ void mbar_init(uint64_t* bar, int count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
-}
-__device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
-    uint32_t ok;
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(ok) : "r"(smem_u32(bar)), "r"(parity) : "memory");
-    return ok != 0;
-}
-// Bounded wait: a wrong descriptor must fail loudly (trap), never hang the GPU.
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-    for (int spin = 0; spin < (1 << 24); ++spin)
-        if (mbar_try_wait(bar, parity)) return;
-    __trap();
-}
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem, int ncols) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)), "r"(ncols));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::);
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, int ncols) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols));
-}
-__device__ __forceinline__ void fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
+// generic-proxy stores to shared memory become visible to the wgmma (async proxy) reads
 __device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
 
-__device__ __forceinline__ void umma_tf32(uint32_t tmem_c, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                          uint32_t accumulate) {
+// shared-memory matrix descriptor (sm_90): start address, LBO and SBO in 16-byte
+// units, base offset 0, no swizzle
+__device__ __forceinline__ uint64_t make_desc(uint32_t smem_addr) {
+    return static_cast<uint64_t>((smem_addr >> 4) & 0x3fffu) |
+           (static_cast<uint64_t>((LBO >> 4) & 0x3fffu) << 16) |
+           (static_cast<uint64_t>((SBO >> 4) & 0x3fffu) << 32);
+}
+
+// d (64 x 128 fp32, wgmma accumulator fragment) += A (64 x 8 tf32) * B (8 x 128 tf32)
+__device__ __forceinline__ void wgmma_tf32(float (&d)[64], uint64_t adesc, uint64_t bdesc) {
     asm volatile(
         "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(tmem_c), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-// 32 consecutive fp32 columns of this thread's TMEM lane
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, float (&v)[32]) {
-    uint32_t r[32];
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
+        "setp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 "
         "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-          "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-          "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-          "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr));
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-    for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(r[i]);
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+        "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+        "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+        "%64, %65, p, 1, 1;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+          "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+          "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+          "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+          "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(adesc), "l"(bdesc), "r"(1)
+        : "memory");
 }
-
-// shared-memory matrix descriptor, SWIZZLE_NONE, version 1 (sm_100)
-__device__ __forceinline__ uint64_t make_desc(uint32_t smem_addr, uint32_t lbo, uint32_t sbo) {
-    return static_cast<uint64_t>((smem_addr >> 4) & 0x3fffu) |
-           (static_cast<uint64_t>((lbo >> 4) & 0x3fffu) << 16) |
-           (static_cast<uint64_t>((sbo >> 4) & 0x3fffu) << 32) |
-           (1ull << 46);
-}
-// instruction descriptor: D = f32, A = B = tf32, M = 128, N = 128
-constexpr uint32_t IDESC_KK = (1u << 4) | (2u << 7) | (2u << 10) | ((TN >> 3) << 17) | ((TM >> 4) << 24);
 
 __device__ __forceinline__ void split4(float4 x, uint4& hi, uint4& lo) {
     split_tf32(x.x, hi.x, lo.x); split_tf32(x.y, hi.y, lo.y);
     split_tf32(x.z, hi.z, lo.z); split_tf32(x.w, hi.w, lo.w);
 }
 
-// 3 x (KC / 8) MMAs for one staged chunk; `first` clears the accumulator on the first one
-__device__ __forceinline__ void issue_chunk(uint32_t tmem, uint32_t sA_hi, uint32_t sA_lo, uint32_t sB_hi,
-                                            uint32_t sB_lo, uint32_t step_bytes, uint32_t lbo, uint32_t sbo,
-                                            uint32_t idesc, bool first) {
+// 2 halves x 3 x (KC / 8) MMAs for one staged chunk, committed as one group and waited for
+__device__ __forceinline__ void mma_chunk(float (&acc)[2][64], const uint8_t* A_hi, const uint8_t* A_lo,
+                                          const uint8_t* B_hi, const uint8_t* B_lo) {
+    const uint32_t ah0 = smem_u32(A_hi), al0 = smem_u32(A_lo), bh0 = smem_u32(B_hi), bl0 = smem_u32(B_lo);
+    wgmma_fence();
 #pragma unroll
     for (int s = 0; s < KC / 8; ++s) {
-        const uint64_t ah = make_desc(sA_hi + s * step_bytes, lbo, sbo), al = make_desc(sA_lo + s * step_bytes, lbo, sbo);
-        const uint64_t bh = make_desc(sB_hi + s * step_bytes, lbo, sbo), bl = make_desc(sB_lo + s * step_bytes, lbo, sbo);
-        umma_tf32(tmem, al, bh, idesc, (first && s == 0) ? 0u : 1u);
-        umma_tf32(tmem, ah, bl, idesc, 1u);
-        umma_tf32(tmem, ah, bh, idesc, 1u);
+        const uint32_t o = s * KSTEP_BYTES;
+        const uint64_t bh = make_desc(bh0 + o), bl = make_desc(bl0 + o);
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const uint64_t ah = make_desc(ah0 + h * HALF_BYTES + o), al = make_desc(al0 + h * HALF_BYTES + o);
+            wgmma_tf32(acc[h], al, bh);
+            wgmma_tf32(acc[h], ah, bl);
+            wgmma_tf32(acc[h], ah, bh);
+        }
     }
+    wgmma_commit();
 }
+
+// Accumulator fragment of m64nNk8: warp w of the warpgroup holds rows 16w .. 16w+15 of
+// each 64-row half; acc[h][4i + 2r + c] is row 64h + 16w + 8r + lane/4, column
+// 8i + 2(lane%4) + c.
+__device__ __forceinline__ int frag_row(int h, int r) {
+    return h * 64 + (threadIdx.x >> 5) * 16 + r * 8 + ((threadIdx.x & 31) >> 2);
+}
+__device__ __forceinline__ int frag_col(int i) { return i * 8 + 2 * (threadIdx.x & 3); }
 
 // ---------------------------------------------------------------------------
 // forward / input-gradient:  K-major operands.  g.Wm is [k][n][c] (row n holds the
@@ -129,29 +117,25 @@ __global__ void __launch_bounds__(128) tc_conv_gemm_kernel(ConvGemm g) {
     uint8_t* A_lo = tc_smem + TILE_BYTES;
     uint8_t* B_hi = tc_smem + 2 * TILE_BYTES;
     uint8_t* B_lo = tc_smem + 3 * TILE_BYTES;
-    uint64_t* bar = reinterpret_cast<uint64_t*>(tc_smem + 4 * TILE_BYTES);
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tc_smem + 4 * TILE_BYTES + 16);
-    const int tid = threadIdx.x, warp = tid >> 5;
+    const int tid = threadIdx.x;
     const int D = g.D;                                   // == 128
     const int64_t M = g.B * g.Tout;
-    const int64_t m = static_cast<int64_t>(blockIdx.x) * TM + tid;     // this thread's output row
-    const int64_t b = m < M ? m / g.Tout : 0;
-    const int t = m < M ? static_cast<int>(m - b * g.Tout) : 0;
+    const int64_t m0 = static_cast<int64_t>(blockIdx.x) * TM;
+    const int64_t ms = m0 + tid;                         // the A row this thread stages
+    const int64_t bs = ms < M ? ms / g.Tout : 0;
+    const int ts = ms < M ? static_cast<int>(ms - bs * g.Tout) : 0;
 
-    if (tid == 0) mbar_init(bar, 1);
-    if (warp == 0) tmem_alloc(tmem_slot, TN);
-    fence_before();
-    __syncthreads();
-    fence_after();
-    const uint32_t tmem = *tmem_slot;
+    float acc[2][64];
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int i = 0; i < 64; ++i) acc[h][i] = 0.f;
 
-    const uint32_t off = (tid >> 3) * 1024 + (tid & 7) * 16;          // (r/8)*SBO + (r%8)*16
-    uint32_t phase = 0;
-    bool first = true;
+    const uint32_t off = (tid >> 3) * SBO + (tid & 7) * 16;          // (r/8)*SBO + (r%8)*16
     for (int j = 0; j < g.k; ++j) {
-        const int q = t + g.shift[j];
-        const bool rowok = m < M && q >= 0 && q < g.Tin;
-        const float* arow = g.In + (b * g.Tin + (rowok ? q : 0)) * D;
+        const int q = ts + g.shift[j];
+        const bool rowok = ms < M && q >= 0 && q < g.Tin;
+        const float* arow = g.In + (bs * g.Tin + (rowok ? q : 0)) * D;
         const float* brow = g.Wm + (static_cast<int64_t>(j) * D + tid) * D;     // row n = tid
         for (int c0 = 0; c0 < D; c0 += KC) {
 #pragma unroll
@@ -161,60 +145,53 @@ __global__ void __launch_bounds__(128) tc_conv_gemm_kernel(ConvGemm g) {
                 const float4 bv = ldg4(brow + c0 + 4 * c);
                 uint4 h, l;
                 split4(av, h, l);
-                *reinterpret_cast<uint4*>(A_hi + off + c * 128) = h;
-                *reinterpret_cast<uint4*>(A_lo + off + c * 128) = l;
+                *reinterpret_cast<uint4*>(A_hi + off + c * LBO) = h;
+                *reinterpret_cast<uint4*>(A_lo + off + c * LBO) = l;
                 split4(bv, h, l);
-                *reinterpret_cast<uint4*>(B_hi + off + c * 128) = h;
-                *reinterpret_cast<uint4*>(B_lo + off + c * 128) = l;
+                *reinterpret_cast<uint4*>(B_hi + off + c * LBO) = h;
+                *reinterpret_cast<uint4*>(B_lo + off + c * LBO) = l;
             }
             fence_async_smem();
             __syncthreads();
-            if (tid == 0) {
-                fence_after();
-                issue_chunk(tmem, smem_u32(A_hi), smem_u32(A_lo), smem_u32(B_hi), smem_u32(B_lo),
-                            256, 128, 1024, IDESC_KK, first);
-                umma_commit(bar);
-            }
-            first = false;
-            mbar_wait(bar, phase);           // MMAs done: operands may be overwritten
-            phase ^= 1;
+            mma_chunk(acc, A_hi, A_lo, B_hi, B_lo);
+            wgmma_wait_all();
+            __syncthreads();                 // every warp's MMAs done: operands may be overwritten
         }
     }
-    fence_after();
 
-    // epilogue: thread = output row `m`, 4 x 32 columns out of TMEM lane 32*warp + lane
-    const uint32_t lane_base = tmem + (static_cast<uint32_t>(warp * 32) << 16);
-    const int rt = t + g.res_shift;
-    const bool resok = g.Res && m < M && rt >= 0 && rt < g.res_T;
-    for (int cb = 0; cb < TN; cb += 32) {
-        float v[32];
-        tmem_ld32(lane_base + cb, v);
-        if (m < M) {
+    // epilogue: 4 output rows per thread, 16 column pairs each
 #pragma unroll
-            for (int c4 = 0; c4 < 32; c4 += 4) {
-                const int n = cb + c4;
-                float x[4] = {v[c4], v[c4 + 1], v[c4 + 2], v[c4 + 3]};
-                float4 res = make_float4(0, 0, 0, 0);
-                if (resok) res = ld4(g.Res + (b * g.res_T + rt) * D + n);
+    for (int h = 0; h < 2; ++h) {
+#pragma unroll
+        for (int r = 0; r < 2; ++r) {
+            const int64_t m = m0 + frag_row(h, r);
+            if (m >= M) continue;
+            const int64_t b = m / g.Tout;
+            const int t = static_cast<int>(m - b * g.Tout);
+            const int rt = t + g.res_shift;
+            const bool resok = g.Res && rt >= 0 && rt < g.res_T;
+#pragma unroll
+            for (int i = 0; i < TN / 8; ++i) {
+                const int n = frag_col(i);
+                float v0 = acc[h][4 * i + 2 * r], v1 = acc[h][4 * i + 2 * r + 1];
+                float2 res = make_float2(0.f, 0.f);
+                if (resok) res = *reinterpret_cast<const float2*>(g.Res + (b * g.res_T + rt) * D + n);
                 if (g.mode == 0) {
-                    const float4 bb = ldg4(g.bias + n);
-                    x[0] += bb.x; x[1] += bb.y; x[2] += bb.z; x[3] += bb.w;
-#pragma unroll
-                    for (int y = 0; y < 4; ++y) x[y] = g.nonlin == 0 ? tanhf(x[y]) : fmaxf(x[y], 0.f);
-                    st4(g.Aout + m * D + n, make_float4(x[0], x[1], x[2], x[3]));
+                    const float2 bb = *reinterpret_cast<const float2*>(g.bias + n);
+                    v0 += bb.x; v1 += bb.y;
+                    v0 = g.nonlin == 0 ? tanhf(v0) : fmaxf(v0, 0.f);
+                    v1 = g.nonlin == 0 ? tanhf(v1) : fmaxf(v1, 0.f);
+                    *reinterpret_cast<float2*>(g.Aout + m * D + n) = make_float2(v0, v1);
                 }
-                float4 o = make_float4(x[0] + res.x, x[1] + res.y, x[2] + res.z, x[3] + res.w);
+                float2 o = make_float2(v0 + res.x, v1 + res.y);
                 if (g.accumulate) {
-                    const float4 old = ld4(g.Out + m * D + n);
-                    o.x += old.x; o.y += old.y; o.z += old.z; o.w += old.w;
+                    const float2 old = *reinterpret_cast<const float2*>(g.Out + m * D + n);
+                    o.x += old.x; o.y += old.y;
                 }
-                st4(g.Out + m * D + n, o);
+                *reinterpret_cast<float2*>(g.Out + m * D + n) = o;
             }
         }
     }
-    fence_before();
-    __syncthreads();
-    if (warp == 0) tmem_dealloc(tmem, TN);
 }
 
 // ---------------------------------------------------------------------------
@@ -228,27 +205,22 @@ __global__ void __launch_bounds__(128) tc_conv_dw_kernel(ConvDw g) {
     uint8_t* A_lo = tc_smem + TILE_BYTES;
     uint8_t* B_hi = tc_smem + 2 * TILE_BYTES;
     uint8_t* B_lo = tc_smem + 3 * TILE_BYTES;
-    uint64_t* bar = reinterpret_cast<uint64_t*>(tc_smem + 4 * TILE_BYTES);
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tc_smem + 4 * TILE_BYTES + 16);
-    const int tid = threadIdx.x, warp = tid >> 5;
+    const int tid = threadIdx.x;
     const int D = g.D;                                   // == 128
     const int j = blockIdx.x;
     const int64_t split = blockIdx.y;
     const int64_t M = g.B * g.Tout;
     const int64_t mlo = split * g.slab, mhi = mlo + g.slab < M ? mlo + g.slab : M;
 
-    if (tid == 0) mbar_init(bar, 1);
-    if (warp == 0) tmem_alloc(tmem_slot, TN);
-    fence_before();
-    __syncthreads();
-    fence_after();
-    const uint32_t tmem = *tmem_slot;
+    float acc[2][64];
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int i = 0; i < 64; ++i) acc[h][i] = 0.f;
 
     // staging: both operands are brought into the K-major canonical layout (rows =
     // channel, k = position) by a 4 x 4 register transpose: a unit is 4 positions x 4
     // channels; thread handles units (pg = u / 32, cg = u % 32) for u = tid, tid + 128.
-    uint32_t phase = 0;
-    bool first = true;
     float bacc = 0.f;                                    // bias gradient: column sums of dZ (tap 0 only)
     for (int64_t mb = mlo; mb < mhi; mb += KC) {
 #pragma unroll
@@ -276,7 +248,7 @@ __global__ void __launch_bounds__(128) tc_conv_dw_kernel(ConvDw g) {
 #pragma unroll
             for (int qd = 0; qd < 4; ++qd) {
                 const int row = cg * 4 + qd;
-                const uint32_t o = (row >> 3) * 1024 + pg * 128 + (row & 7) * 16;
+                const uint32_t o = (row >> 3) * SBO + pg * LBO + (row & 7) * 16;
                 uint4 h, l;
                 split4(make_float4(ar[qd][0], ar[qd][1], ar[qd][2], ar[qd][3]), h, l);
                 *reinterpret_cast<uint4*>(A_hi + o) = h;
@@ -288,40 +260,28 @@ __global__ void __launch_bounds__(128) tc_conv_dw_kernel(ConvDw g) {
         }
         fence_async_smem();
         __syncthreads();
-        if (tid == 0) {
-            fence_after();
-            issue_chunk(tmem, smem_u32(A_hi), smem_u32(A_lo), smem_u32(B_hi), smem_u32(B_lo),
-                        256, 128, 1024, IDESC_KK, first);
-            umma_commit(bar);
-        }
-        first = false;
+        mma_chunk(acc, A_hi, A_lo, B_hi, B_lo);
         if (j == 0) {                                     // db[o = tid]: fixed order over the chunk
             for (int pp = 0; pp < KC; ++pp) {
                 const int64_t m2 = mb + pp;
                 if (m2 < mhi) bacc += g.dZ[m2 * D + tid];
             }
         }
-        mbar_wait(bar, phase);
-        phase ^= 1;
+        wgmma_wait_all();
+        __syncthreads();
     }
-    fence_after();
     float* out = g.part + ((split * g.k + j) * D) * D;   // [i][o]
-    const uint32_t lane_base = tmem + (static_cast<uint32_t>(warp * 32) << 16);
-    for (int cb = 0; cb < TN; cb += 32) {
-        float v[32];
-        if (mlo < mhi) tmem_ld32(lane_base + cb, v);
-        else {
 #pragma unroll
-            for (int i = 0; i < 32; ++i) v[i] = 0.f;
+    for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int r = 0; r < 2; ++r) {
+            const int64_t i = frag_row(h, r);
+#pragma unroll
+            for (int c = 0; c < TN / 8; ++c)
+                *reinterpret_cast<float2*>(out + i * D + frag_col(c)) =
+                    make_float2(acc[h][4 * c + 2 * r], acc[h][4 * c + 2 * r + 1]);
         }
-#pragma unroll
-        for (int c4 = 0; c4 < 32; c4 += 4)
-            st4(out + static_cast<int64_t>(tid) * D + cb + c4, make_float4(v[c4], v[c4 + 1], v[c4 + 2], v[c4 + 3]));
-    }
     if (j == 0) g.bpart[split * D + tid] = bacc;
-    fence_before();
-    __syncthreads();
-    if (warp == 0) tmem_dealloc(tmem, TN);
 }
 
 }  // namespace tc

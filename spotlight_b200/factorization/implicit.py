@@ -84,7 +84,7 @@ PLANNED_STEP = True
 # both paths are bit-exact with numpy, so the threshold is a speed knob only
 DEVICE_SHUFFLE_MIN = 1 << 17
 
-_NO_CPU = ('spotlight_b200 runs the fit() hot path in sm_100a CUDA kernels and has no CPU '
+_NO_CPU = ('spotlight_b200 runs the fit() hot path in sm_90a CUDA kernels and has no CPU '
            'route; construct the model with use_cuda=True.')
 
 

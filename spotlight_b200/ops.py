@@ -7,7 +7,7 @@ include/spotlight_b200.h) and is registered with ``torch.library`` so that
 spotlight/factorization/implicit.py:237-243).
 
 PyTorch is plumbing here: it owns device memory and streams; all arithmetic
-happens in the hand-written sm_100a kernels.  CPU tensors are rejected -- there
+happens in the hand-written sm_90a kernels.  CPU tensors are rejected -- there
 is no CPU path.
 """
 
@@ -37,7 +37,7 @@ def require_cuda(*tensors):
     for t in tensors:
         if t is not None and not t.is_cuda:
             raise RuntimeError(
-                'spotlight_b200 ops need CUDA tensors (sm_100a); there is no CPU path. '
+                'spotlight_b200 ops need CUDA tensors (sm_90a); there is no CPU path. '
                 'Construct the model with use_cuda=True.')
         if t is not None and t.device.index != torch.cuda.current_device():
             # the library launches on the current device and never calls cudaSetDevice

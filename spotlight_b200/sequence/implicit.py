@@ -27,7 +27,7 @@ from spotlight_b200.torch_utils import cpu, gpu, minibatch, set_seed, shuffled_o
 
 DEVICE_SHUFFLE_MIN = 1 << 17        # as factorization/implicit.py: a speed knob, both paths are bit-exact
 
-_NO_CPU = ('spotlight_b200 runs the fit() hot path in sm_100a CUDA kernels and has no CPU '
+_NO_CPU = ('spotlight_b200 runs the fit() hot path in sm_90a CUDA kernels and has no CPU '
            'route; construct the model with use_cuda=True.')
 
 

@@ -475,8 +475,8 @@ class ShardedMF(object):
         flag the caller reads once per epoch -- the step's result is then invalid and the epoch
         must be rerun with more slots or the synchronising ``step_a2a``).
 
-        CPU-verified against the float64 oracle (tests/test_sharded_cpu.py, gloo); NOT yet run or
-        measured on the B200s -- the round's GPU budget was spent (DESIGN.md section 6)."""
+        CPU-verified against the float64 oracle (tests/test_sharded_cpu.py, gloo); not yet run or
+        measured on GPUs (DESIGN.md section 8)."""
         plan, st, P, be = self.plan, self.st, self.plan.world, self.backend
         dev = users.device
         B = users.numel()

@@ -1,11 +1,11 @@
 """Generate golden vectors from the LIVE reference (build container only).
 
-Run:  PYTHONDONTWRITEBYTECODE=1 python tests/golden/make_golden.py
+Run:  SPOTLIGHT_REFERENCE=<reference checkout> PYTHONDONTWRITEBYTECODE=1 python tests/golden/make_golden.py
 
-Imports the unmodified reference from /root/reference (read-only), drives its
-own modules / methods with fixed seeds, and stores inputs + outputs as small
-``.npz`` fixtures next to this script.  The GPU box has no /root/reference; the
-tests there read only the committed fixtures.
+Imports the unmodified reference from the checkout SPOTLIGHT_REFERENCE names
+(read-only), drives its own modules / methods with fixed seeds, and stores
+inputs + outputs as small ``.npz`` fixtures next to this script.  The tests read
+only the committed fixtures.
 
 What is recorded (per case): the model ``state_dict``, the minibatch ids, the
 RandomState key/pos before sampling, the negatives the reference drew, its
@@ -21,7 +21,7 @@ import sys
 import numpy as np
 
 sys.dont_write_bytecode = True
-sys.path.insert(0, '/root/reference')
+sys.path.insert(0, os.environ['SPOTLIGHT_REFERENCE'])
 
 import torch  # noqa: E402
 
@@ -286,7 +286,7 @@ if __name__ == '__main__':
              cnn_kwargs=dict(kernel_width=3, dilation=1, num_layers=1))
     seq_case('cnn_bpr_l2_relu', 'bpr', 'cnn', num_items=61, dim=16, batch=10, S=11,
              cnn_kwargs=dict(kernel_width=3, dilation=(1, 2), num_layers=2, nonlinearity='relu'))
-    # D = 128: the tcgen05 conv path of the product (csrc/seq_tc.cuh) against the live reference
+    # D = 128: the wgmma conv path of the product (csrc/seq_tc.cuh) against the live reference
     seq_case('cnn_pointwise_d128', 'pointwise', 'cnn', num_items=61, dim=128, batch=10, S=25,
              cnn_kwargs=dict(kernel_width=3, dilation=1, num_layers=1))
     seq_case('cnn_adaptive_k5_nores', 'adaptive_hinge', 'cnn', num_items=61, dim=16, batch=6,

@@ -212,8 +212,8 @@ def test_fused_adam_schedule_and_dense_fallback():
 
 
 def test_reference_arm_prints_the_contract_line():
-    """`bench.py --impl reference` (the arm the driver times beside ours): runs the
-    reference's own fit loop (baseline/_ref when installed, else the oracle port) on the
+    """`bench.py --impl reference` (the CPU arm timed beside ours): runs the
+    reference's own fit loop (oracle/_ref when installed, else the oracle port) on the
     host cores and prints one JSON line with the contract's keys.  Tiny workload here."""
     import json
     import subprocess

@@ -50,7 +50,7 @@ def test_pool_step_golden(name):
                                        ('cnn_adaptive_k5_nores', 'adaptive_hinge'),
                                        ('cnn_pointwise_d128', 'pointwise')])
 def test_cnn_step_golden(name, loss):
-    # cnn_pointwise_d128 runs the tcgen05 conv (D == 128) against the live reference's
+    # cnn_pointwise_d128 runs the wgmma conv (D == 128) against the live reference's
     # scores and gradients at the north star's 1e-5; the D = 16 cases run the mma.sync path
     from spotlight_b200 import ops
     g = load_golden(name)
