@@ -287,3 +287,200 @@ int slb_rank_pairs(const float* scores, int64_t n_rows, int64_t n_items, const i
 }
 
 }  // extern "C"
+
+// f3 evaluation ranking in one pass per row: for every target of a row, the average rank
+// (rank_pairs_kernel's, bit for bit) and the stable position (where the target lands in
+// argsort(-row, kind='stable')), from #(row > s), #(row == s) and #(row == s, item < target).
+// One CTA per row.  The row's targets are staged in shared memory sorted by (score desc, id asc);
+// each row element is binary-searched against them once and drops +1/-1 boundaries into integer
+// histograms whose prefix sums are every target's three counts.  Integer counts only, so the
+// result does not depend on the order the elements are visited in.  A row with more than
+// RT_CAP targets is handled in chunks of RT_CAP and re-read once per chunk.  NaN compares as
+// neither greater nor equal, as in rank_pairs_kernel.
+namespace {
+
+constexpr int RT_THREADS = 256;
+constexpr int RT_CAP = 1024;
+constexpr int RT_WARPS = RT_THREADS / 32;
+
+// f(v, i) for every element of row[0, n): scalar head up to 16-byte alignment, float4 body,
+// scalar tail (a row of a [rows, n] block is 16-byte aligned only when n % 4 == 0)
+template <class F>
+__device__ __forceinline__ void rt_stream_row(const float* __restrict__ row, int64_t n, F&& f) {
+    const int64_t mis = static_cast<int64_t>((reinterpret_cast<uintptr_t>(row) >> 2) & 3);
+    const int64_t head = min(n, (4 - mis) & 3);
+    for (int64_t i = threadIdx.x; i < head; i += RT_THREADS) f(__ldg(row + i), i);
+    const int64_t nv = (n - head) >> 2;
+    const float4* row4 = reinterpret_cast<const float4*>(row + head);
+    for (int64_t q = threadIdx.x; q < nv; q += RT_THREADS) {
+        const float4 v = __ldg(row4 + q);
+        const int64_t i = head + 4 * q;
+        f(v.x, i); f(v.y, i + 1); f(v.z, i + 2); f(v.w, i + 3);
+    }
+    for (int64_t i = head + 4 * nv + threadIdx.x; i < n; i += RT_THREADS) f(__ldg(row + i), i);
+}
+
+// (score desc, id asc), NaN scores last
+__device__ __forceinline__ bool rt_before(float ka, int32_t ia, float kb, int32_t ib) {
+    const bool na = isnan(ka), nb = isnan(kb);
+    if (na != nb) return nb;
+    if (!na && ka != kb) return ka > kb;
+    return ia < ib;
+}
+
+// block-wide exclusive prefix sum of three ints (all threads must call)
+__device__ __forceinline__ void rt_exclusive_scan3(int v[3], int (*warp_tot)[RT_WARPS]) {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    int inc[3] = {v[0], v[1], v[2]};
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1)
+#pragma unroll
+        for (int k = 0; k < 3; ++k) {
+            const int u = __shfl_up_sync(0xffffffffu, inc[k], o);
+            if (lane >= o) inc[k] += u;
+        }
+    if (lane == 31)
+        for (int k = 0; k < 3; ++k) warp_tot[k][warp] = inc[k];
+    __syncthreads();
+    for (int k = 0; k < 3; ++k) {
+        int before = inc[k] - v[k];
+        for (int w = 0; w < warp; ++w) before += warp_tot[k][w];
+        v[k] = before;
+    }
+    __syncthreads();
+}
+
+__device__ __forceinline__ void rt_write(int64_t p, int gt, int eq, int eq_before, float* __restrict__ avg_rank,
+                                         int64_t* __restrict__ position) {
+    if (avg_rank) avg_rank[p] = 1.0f + static_cast<float>(gt) + 0.5f * static_cast<float>(eq - 1);
+    if (position) position[p] = static_cast<int64_t>(gt) + eq_before;
+}
+
+__global__ void __launch_bounds__(RT_THREADS)
+rank_targets_kernel(const float* __restrict__ scores, int64_t n_rows, int64_t n_items,
+                    const int64_t* __restrict__ row_ptr, const int64_t* __restrict__ targets,
+                    float* __restrict__ avg_rank, int64_t* __restrict__ position) {
+    __shared__ float key[RT_CAP];
+    __shared__ int32_t id[RT_CAP];
+    __shared__ int16_t slot[RT_CAP];              // index of the sorted entry within its chunk
+    __shared__ int32_t hist[3][RT_CAP + 1];       // boundaries of the greater / equal / equal-before ranges
+    __shared__ int warp_tot[3][RT_WARPS];
+
+    for (int64_t r = blockIdx.x; r < n_rows; r += gridDim.x) {
+        const float* row = scores + r * n_items;
+        const int64_t t0 = row_ptr[r], t1 = row_ptr[r + 1];
+        if (t1 - t0 == 1) {
+            // one target (sequence_mrr_score): plain compares and a block reduction
+            const int64_t t = targets[t0];
+            const float s = row[t];
+            int c[3] = {0, 0, 0};
+            rt_stream_row(row, n_items, [&](float v, int64_t i) {
+                c[0] += v > s;
+                c[1] += v == s;
+                c[2] += (v == s) & (i < t);
+            });
+            int tot[3] = {c[0], c[1], c[2]};
+            rt_exclusive_scan3(c, warp_tot);
+            if (threadIdx.x == RT_THREADS - 1)
+                rt_write(t0, c[0] + tot[0], c[1] + tot[1], c[2] + tot[2], avg_rank, position);
+            continue;
+        }
+        for (int64_t c0 = t0; c0 < t1; c0 += RT_CAP) {
+            const int m = static_cast<int>(min(static_cast<int64_t>(RT_CAP), t1 - c0));
+            int P = 1;
+            while (P < m) P <<= 1;
+            for (int j = threadIdx.x; j < P; j += RT_THREADS) {
+                if (j < m) {
+                    const int64_t t = targets[c0 + j];
+                    id[j] = static_cast<int32_t>(t);
+                    key[j] = row[t];
+                } else {
+                    id[j] = INT32_MAX;
+                    key[j] = __int_as_float(0x7fffffff);
+                }
+                slot[j] = static_cast<int16_t>(j);
+            }
+            for (int j = threadIdx.x; j <= m; j += RT_THREADS) hist[0][j] = hist[1][j] = hist[2][j] = 0;
+            __syncthreads();
+            // bitonic sort of the P staged entries
+            for (int k = 2; k <= P; k <<= 1)
+                for (int h = k >> 1; h > 0; h >>= 1) {
+                    for (int i = threadIdx.x; i < P; i += RT_THREADS) {
+                        const int l = i ^ h;
+                        if (l <= i) continue;
+                        const bool swap = (i & k) == 0 ? rt_before(key[l], id[l], key[i], id[i])
+                                                       : rt_before(key[i], id[i], key[l], id[l]);
+                        if (swap) {
+                            const float tk = key[i]; key[i] = key[l]; key[l] = tk;
+                            const int32_t ti = id[i]; id[i] = id[l]; id[l] = ti;
+                            const int16_t ts = slot[i]; slot[i] = slot[l]; slot[l] = ts;
+                        }
+                    }
+                    __syncthreads();
+                }
+            int nv = 0;                                   // non-NaN targets, sorted first
+            for (int j0 = 0; j0 < P; j0 += RT_THREADS) {
+                const int j = j0 + threadIdx.x;
+                nv += __syncthreads_count(j < P && !isnan(key[j]));
+            }
+            if (nv > 0)
+                rt_stream_row(row, n_items, [&](float v, int64_t i) {
+                    if (isnan(v)) return;
+                    // a = #(targets with key >= v): v is greater than the targets [a, nv)
+                    int lo = 0, hi = nv;
+                    while (lo < hi) { const int mid = (lo + hi) >> 1; if (key[mid] >= v) lo = mid + 1; else hi = mid; }
+                    const int a = lo;
+                    if (a < nv) atomicAdd(&hist[0][a], 1);
+                    if (a == 0 || key[a - 1] != v) return;
+                    // b = #(targets with key > v): v equals the targets [b, a)
+                    lo = 0; hi = a - 1;
+                    while (lo < hi) { const int mid = (lo + hi) >> 1; if (key[mid] > v) lo = mid + 1; else hi = mid; }
+                    const int b = lo;
+                    atomicAdd(&hist[1][b], 1);
+                    atomicSub(&hist[1][a], 1);
+                    // within [b, a) the ids ascend: v precedes the targets with id > i
+                    hi = a;
+                    while (lo < hi) { const int mid = (lo + hi) >> 1; if (id[mid] <= i) lo = mid + 1; else hi = mid; }
+                    if (lo < a) {
+                        atomicAdd(&hist[2][lo], 1);
+                        atomicSub(&hist[2][a], 1);
+                    }
+                });
+            __syncthreads();
+            // inclusive prefix sums over [0, nv): thread x owns a contiguous run of entries
+            const int L = (nv + RT_THREADS - 1) / RT_THREADS;
+            const int beg = min(nv, static_cast<int>(threadIdx.x) * L), end = min(nv, beg + L);
+            int run[3] = {0, 0, 0};
+            for (int x = beg; x < end; ++x)
+                for (int k = 0; k < 3; ++k) run[k] += hist[k][x];
+            rt_exclusive_scan3(run, warp_tot);
+            for (int x = beg; x < end; ++x) {
+                for (int k = 0; k < 3; ++k) run[k] += hist[k][x];
+                rt_write(c0 + slot[x], run[0], run[1], run[2], avg_rank, position);
+            }
+            for (int x = nv + threadIdx.x; x < m; x += RT_THREADS) rt_write(c0 + slot[x], 0, 0, 0, avg_rank, position);
+            __syncthreads();
+        }
+    }
+}
+
+}  // namespace
+
+extern "C" {
+
+int slb_rank_targets(const float* scores, int64_t n_rows, int64_t n_items, const int64_t* row_ptr,
+                     const int64_t* targets, int64_t n_targets, float* avg_rank, int64_t* position,
+                     slb_stream_t stream) {
+    if (n_targets <= 0 || n_rows <= 0) return SLB_OK;
+    SLB_REQUIRE(scores && row_ptr && targets && n_items > 0 && n_items <= INT32_MAX,
+                "rank_targets: bad arguments");
+    if (!avg_rank && !position) return SLB_OK;
+    const int64_t cap = static_cast<int64_t>(slb_sms()) * 8;
+    const int grid = static_cast<int>(n_rows < cap ? n_rows : cap);
+    rank_targets_kernel<<<grid, RT_THREADS, 0, static_cast<cudaStream_t>(stream)>>>(
+        scores, n_rows, n_items, row_ptr, targets, avg_rank, position);
+    SLB_LAUNCH_CHECK("rank_targets_kernel");
+    return SLB_OK;
+}
+
+}  // extern "C"
