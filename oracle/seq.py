@@ -13,6 +13,15 @@ and the gradients autograd produces for them (padding rows of the item
 embedding and item bias receive zero gradient: ``padding_idx=PADDING_IDX`` at
 representations.py:68-72, 349-353).  Pinned against golden vectors from the
 live reference in tests/test_oracle_seq.py.
+
+``mutate`` (a tuple of names, empty by default) restates plausible kernel
+mistakes for tests/test_seq_oracle_cpu.py, which shows that the GPU
+tolerances catch each of them:
+
+* ``'count_per_row'``  PoolNet divides by a per-row count of non-padding items
+  instead of the per-element count of non-zero entries;
+* ``'pad0_rf_minus_1'`` CNNNet pads layer 0 by rf - 1 instead of rf;
+* ``'residual_shift'``  CNNNet adds e_t instead of e_{t-1} on layer 0's residual.
 """
 
 import numpy as np
@@ -22,7 +31,7 @@ from oracle.mf import loss_and_score_grads
 PADDING_IDX = 0
 
 
-def pool_representation(E, seq, dtype=np.float32):
+def pool_representation(E, seq, dtype=np.float32, mutate=()):
     """All S+1 prefix representations, shape (B, S+1, D).
 
     r_t = sum_{s<t} e_s / (sum_{s<t} [e_s != 0] + 1), element-wise count
@@ -33,7 +42,10 @@ def pool_representation(E, seq, dtype=np.float32):
     P = np.zeros((B, S + 1, D), dtype=dtype)
     C = np.zeros((B, S + 1, D), dtype=dtype)
     P[:, 1:] = np.cumsum(e, axis=1, dtype=dtype)
-    C[:, 1:] = np.cumsum((e != 0.0).astype(dtype), axis=1, dtype=dtype)
+    nz = e != 0.0
+    if 'count_per_row' in mutate:
+        nz = np.broadcast_to((seq != PADDING_IDX)[..., None], e.shape)
+    C[:, 1:] = np.cumsum(nz.astype(dtype), axis=1, dtype=dtype)
     return P / (C + 1.0), C
 
 
@@ -62,11 +74,14 @@ def _prep_negs(negs, B, S, loss, n_neg):
     return negs.reshape(1, B, S)
 
 
-def pool_step(E, bias, seq, negs, loss='pointwise', n_neg=1, dtype=np.float32):
-    """One PoolNet minibatch.  negs: (B,S), or (n*B,S) for adaptive_hinge."""
+def pool_step(E, bias, seq, negs, loss='pointwise', n_neg=1, dtype=np.float32, mutate=()):
+    """One PoolNet minibatch.  negs: (B,S), or (n*B,S) for adaptive_hinge.
+
+    Also returns the score gradients gp (B,S) and gn ((n,B,S) for adaptive_hinge, else (B,S)).
+    """
     B, S = seq.shape
     D = E.shape[1]
-    rall, C = pool_representation(E, seq, dtype)
+    rall, C = pool_representation(E, seq, dtype, mutate)
     r = rall[:, :S]
     negs3 = _prep_negs(negs, B, S, loss, n_neg)
     pos = _scores(r, E, bias, seq, dtype)
@@ -89,7 +104,7 @@ def pool_step(E, bias, seq, negs, loss='pointwise', n_neg=1, dtype=np.float32):
     dE[PADDING_IDX] = 0
     dbias[PADDING_IDX] = 0
     return dict(pos=pos, neg=neg if loss == 'adaptive_hinge' else neg[0], loss=lval,
-                dE=dE, dbias=dbias, final=rall[:, S])
+                dE=dE, dbias=dbias, final=rall[:, S], gp=gp, gn=gn if loss == 'adaptive_hinge' else gn[0])
 
 
 def _act(x, kind):
@@ -101,7 +116,7 @@ def _dact(a, kind):
 
 
 def cnn_representation(E, convs, seq, kernel_width, dilation, nonlinearity='tanh',
-                       residual=True, dtype=np.float32):
+                       residual=True, dtype=np.float32, mutate=()):
     """CNNNet.user_representation.  convs: list of (W (D,D,k,1), b (D,)).
 
     Returns (y (B,S+1,D), saved) where y[:, t] only sees items < t.
@@ -115,7 +130,8 @@ def cnn_representation(E, convs, seq, kernel_width, dilation, nonlinearity='tanh
         rf = k + (k - 1) * (d - 1)
         if l == 0:
             xin = np.zeros((B, S + rf, D), dtype=dtype)      # left pad rf (not rf-1)
-            xin[:, rf:] = e
+            pad0 = rf - 1 if 'pad0_rf_minus_1' in mutate else rf
+            xin[:, pad0:pad0 + S] = e
         else:
             xin = np.zeros((B, S + 1 + rf - 1, D), dtype=dtype)
             xin[:, rf - 1:] = x
@@ -127,7 +143,10 @@ def cnn_representation(E, convs, seq, kernel_width, dilation, nonlinearity='tanh
         if residual:
             if l == 0:
                 res = np.zeros((B, S + 1, D), dtype=dtype)
-                res[:, 1:] = e
+                if 'residual_shift' in mutate:
+                    res[:, :S] = e
+                else:
+                    res[:, 1:] = e
             else:
                 res = x
             y = a + res
@@ -139,12 +158,13 @@ def cnn_representation(E, convs, seq, kernel_width, dilation, nonlinearity='tanh
 
 
 def cnn_step(E, bias, convs, seq, negs, kernel_width, dilation, loss='pointwise',
-             n_neg=1, nonlinearity='tanh', residual=True, dtype=np.float32):
-    """One CNNNet minibatch: loss and grads for E, bias and every conv."""
+             n_neg=1, nonlinearity='tanh', residual=True, dtype=np.float32, mutate=()):
+    """One CNNNet minibatch: loss and grads for E, bias and every conv (and gp / gn as in
+    pool_step)."""
     B, S = seq.shape
     D = E.shape[1]
     y, saved = cnn_representation(E, convs, seq, kernel_width, dilation,
-                                  nonlinearity, residual, dtype)
+                                  nonlinearity, residual, dtype, mutate)
     r = y[:, :S]
     negs3 = _prep_negs(negs, B, S, loss, n_neg)
     pos = _scores(r, E, bias, seq, dtype)
@@ -177,9 +197,10 @@ def cnn_step(E, bias, convs, seq, negs, kernel_width, dilation, loss='pointwise'
         db = dz.sum(axis=(0, 1), dtype=dtype)
         dconvs.append((dW, db))
         if l == 0:
-            de += dxin[:, rf:]
+            pad0 = rf - 1 if 'pad0_rf_minus_1' in mutate else rf
+            de += dxin[:, pad0:pad0 + S]
             if residual:
-                de += dy[:, 1:]
+                de += dy[:, :S] if 'residual_shift' in mutate else dy[:, 1:]
         else:
             dprev = dxin[:, rf - 1:]
             if residual:
@@ -190,4 +211,5 @@ def cnn_step(E, bias, convs, seq, negs, kernel_width, dilation, loss='pointwise'
     dE[PADDING_IDX] = 0
     dbias[PADDING_IDX] = 0
     return dict(pos=pos, neg=neg if loss == 'adaptive_hinge' else neg[0], loss=lval,
-                dE=dE, dbias=dbias, dconvs=dconvs, final=y[:, S])
+                dE=dE, dbias=dbias, dconvs=dconvs, final=y[:, S],
+                gp=gp, gn=gn if loss == 'adaptive_hinge' else gn[0])

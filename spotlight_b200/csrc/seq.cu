@@ -367,10 +367,18 @@ __global__ void __launch_bounds__(256) seq_fill_kernel(SeqDev a) {
     }
 }
 
+// One lane group per touched row: sums the row's contribution rows C[t] and score gradients
+// gs[t] in ascending term order, then writes dE / dbias, or applies the fused optimizer.
+// The fused optimizer updates a row (embedding and bias together) when any of its terms has
+// a non-zero score gradient or its summed embedding gradient is non-zero -- the MF rule
+// (mf_v2.cuh user_member / user_finish) extended by the input role, whose gradient reaches a
+// row through later positions' scores.  With weight decay an updated row is decayed in every
+// element, including those whose gradient is zero.
 template <int LPR>
 __global__ void __launch_bounds__(SQ_THREADS) seq_reduce_kernel(SeqDev a) {
     constexpr int GROUPS = SQ_THREADS / LPR;
     constexpr int CAP = seg_sort_cap(LPR);
+    constexpr int NCH = LPR == 32 ? 4 : 1;   // float4 chunks per lane: D <= LPR * 4 below 128, <= 512
     __shared__ int32_t sh_sort[GROUPS * 2 * CAP];
     const int gl = threadIdx.x & (LPR - 1);
     const int gib = threadIdx.x / LPR;
@@ -383,44 +391,56 @@ __global__ void __launch_bounds__(SQ_THREADS) seq_reduce_kernel(SeqDev a) {
         const int start = a.seg.seg_start[s];
         const int len = a.seg.seg_start[s + 1] - start;
         const int64_t row = a.seg.seg_row[s];
+        float4 acc[NCH];
+#pragma unroll
+        for (int q = 0; q < NCH; ++q) acc[q] = make_float4(0, 0, 0, 0);
         float bacc = 0.f;
-        for (int c0 = 0; c0 < D; c0 += LPR * 4) {
-            const int c = c0 + gl * 4;
-            float4 acc = make_float4(0, 0, 0, 0);
-            float b2 = 0.f;
-            seg_visit_sorted<LPR>(a.seg.members, start, len, gl, gmask, sh, [&](int32_t t) {
+        bool nz = false;                     // a term with a non-zero score gradient (group-uniform)
+        seg_visit_sorted<LPR>(a.seg.members, start, len, gl, gmask, sh, [&](int32_t t) {
+            const float* src = a.C + static_cast<int64_t>(t) * D;
+#pragma unroll
+            for (int q = 0; q < NCH; ++q) {
+                const int c = gl * 4 + q * LPR * 4;
                 if (c < D) {
-                    const float4 v = ld4(a.C + static_cast<int64_t>(t) * D + c);
-                    acc.x += v.x; acc.y += v.y; acc.z += v.z; acc.w += v.w;
+                    const float4 v = ld4(src + c);
+                    acc[q].x += v.x; acc[q].y += v.y; acc[q].z += v.z; acc[q].w += v.w;
                 }
-                b2 += a.gs[t];
-            });
+            }
+            const float g = a.gs[t];
+            bacc += g;
+            nz = nz || g != 0.f;
+        });
+        if (a.opt == SLB_OPT_NONE) {
+#pragma unroll
+            for (int q = 0; q < NCH; ++q) {
+                const int c = gl * 4 + q * LPR * 4;
+                if (c < D) st4(a.dE + row * D + c, acc[q]);
+            }
+            if (gl == 0) a.dbias[row] = bacc;
+            continue;
+        }
+#pragma unroll
+        for (int q = 0; q < NCH; ++q)
+            nz = nz || acc[q].x != 0.f || acc[q].y != 0.f || acc[q].z != 0.f || acc[q].w != 0.f;
+        if (!__any_sync(gmask, nz)) continue;   // group-uniform
+        // row-wise optimizer applied in place: this is the last kernel of the step, every
+        // gradient that reads E has been formed
+        const OptV2 o = {a.opt, a.lr, a.wd, a.eps};
+#pragma unroll
+        for (int q = 0; q < NCH; ++q) {
+            const int c = gl * 4 + q * LPR * 4;
             if (c < D) {
-                if (a.opt == SLB_OPT_NONE) {
-                    st4(a.dE + row * D + c, acc);
-                } else if (acc.x != 0.f || acc.y != 0.f || acc.z != 0.f || acc.w != 0.f) {
-                    // row-wise optimizer applied in place: this is the last kernel of the step, every
-                    // gradient that reads E has been formed (SGD / Adagrad change an element only when
-                    // its gradient is non-zero, so this equals the dense update)
-                    const OptV2 o = {a.opt, a.lr, a.wd, a.eps};
-                    float* wrow = const_cast<float*>(a.E) + row * D + c;
-                    float* srow = a.opt == SLB_OPT_ADAGRAD ? a.sE + row * D + c : nullptr;
-                    float4 w4 = ld4(wrow), s4 = make_float4(0.f, 0.f, 0.f, 0.f);
-                    if (srow) s4 = ld4(srow);
-                    row_update(o, w4, s4, acc);
-                    st4(wrow, w4);
-                    if (srow) st4(srow, s4);
-                }
-            }
-            bacc = b2;
-        }
-        if (gl == 0) {
-            if (a.opt == SLB_OPT_NONE) a.dbias[row] = bacc;
-            else if (bacc != 0.f) {
-                const OptV2 o = {a.opt, a.lr, a.wd, a.eps};
-                bias_update(o, const_cast<float*>(a.bias) + row, a.opt == SLB_OPT_ADAGRAD ? a.sbias + row : nullptr, bacc);
+                float* wrow = const_cast<float*>(a.E) + row * D + c;
+                float* srow = a.opt == SLB_OPT_ADAGRAD ? a.sE + row * D + c : nullptr;
+                float4 w4 = ld4(wrow), s4 = make_float4(0.f, 0.f, 0.f, 0.f);
+                if (srow) s4 = ld4(srow);
+                row_update(o, w4, s4, acc[q]);
+                st4(wrow, w4);
+                if (srow) st4(srow, s4);
             }
         }
+        if (gl == 0)
+            bias_update(o, const_cast<float*>(a.bias) + row, a.opt == SLB_OPT_ADAGRAD ? a.sbias + row : nullptr, bacc);
     }
 }
 

@@ -24,7 +24,8 @@ from spotlight_b200 import _lib
 
 
 class FusedSGD(torch.optim.SGD):
-    """Plain SGD (no momentum).  ``weight_decay`` is applied to touched rows only."""
+    """Plain SGD (no momentum).  ``weight_decay``: on the fused pipelines it is applied to the
+    rows a minibatch updates only (see ``FusedAdagrad``)."""
 
     fused_kind = _lib.OPT_SGD
 
@@ -44,10 +45,13 @@ class FusedAdagrad(torch.optim.Adagrad):
     (torch defaults).  State lives in ``self.state[p]['sum']`` exactly as in
     ``torch.optim.Adagrad`` so training can continue with either.
 
-    ``weight_decay``: on the fused epoch pipeline it is added (as ``wd * w``) to the gradient
-    of the rows a minibatch touches with a non-zero gradient only; torch's dense Adagrad decays
-    every row on every step.  With ``weight_decay = 0`` (the default, and what the parity tests
-    use) the two are the same update; with ``weight_decay > 0`` they differ."""
+    ``weight_decay``: on the fused pipelines it is added (as ``wd * w``) to the gradient of the
+    rows a minibatch updates only, in every element of such a row; torch's dense Adagrad decays
+    every row on every step.  A row is updated when one of its terms has a non-zero score
+    gradient (in a sequence step also when its embedding gradient is non-zero, through the
+    item's input role), even if its own embedding gradient is exactly zero.  With
+    ``weight_decay = 0`` (the default) this is the dense update; with ``weight_decay > 0`` rows
+    outside the minibatch are not decayed."""
 
     fused_kind = _lib.OPT_ADAGRAD
 
