@@ -33,3 +33,15 @@ for (n, reg, stack, sh, loc), d in zip(rows, names):
     out.append((d, reg, stack, sh, loc))
 for d, reg, stack, sh, loc in sorted(out):
     print('%5d %6d %12d %6d  %s' % (reg, stack, sh, loc, d[:140]))
+
+# Dynamic shared memory of the LSTM recurrence kernels per CTA: csrc/seq.cu lstm_cluster_size /
+# lstm_dev and csrc/seq_lstm.cuh fwd_smem_floats / bwd_smem_floats restated.
+print('# lstm_fwd_kernel / lstm_bwd_kernel dynamic shared memory per CTA')
+print('#   D  cluster  units  seqs/tile   fwd_bytes   bwd_bytes')
+for D in (4, 32, 64, 100, 128, 132, 256):
+    c = 1 if D <= 64 else (4 if D <= 128 else 8)
+    U = -(-D // c)
+    NB = min(max(256 // U, 1), 32)
+    fwd = 4 * U * D + 4 * U + 2 * NB * (D + 4)
+    bwd = 4 * U * D + 4 * NB * U + 2 * NB * D
+    print('%5d %8d %6d %10d %11d %11d' % (D, c, U, NB, 4 * fwd, 4 * bwd))

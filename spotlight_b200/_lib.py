@@ -92,6 +92,8 @@ class SeqStepArgs(ctypes.Structure):
         ('workspace', c_vp), ('workspace_bytes', c_sz),
         ('opt', c_i32), ('lr', c_f32), ('weight_decay', c_f32), ('eps', c_f32),
         ('state_E', c_vp), ('state_bias', c_vp),
+        ('lstm_w_ih', c_vp), ('lstm_w_hh', c_vp), ('lstm_b_ih', c_vp), ('lstm_b_hh', c_vp),
+        ('dlstm_w_ih', c_vp), ('dlstm_w_hh', c_vp), ('dlstm_b_ih', c_vp), ('dlstm_b_hh', c_vp),
     ]
 
 

@@ -23,6 +23,8 @@
 //                        target-role contribution rows, row counts
 //   pool_bwd_kernel      exclusive suffix sums of d r / (count + 1)
 //   seq_fill / seq_reduce  deterministic segmented scatter into dE, dbias
+//   lstm_fwd / lstm_bwd  LSTMNet recurrence and its BPTT on thread-block clusters (seq_lstm.cuh);
+//                        the LSTM's projections and weight gradients are k = 1 conv GEMMs
 #include <stdlib.h>
 
 #include "segindex.cuh"
@@ -612,6 +614,7 @@ struct ConvDw {
 
 }  // namespace
 #include "seq_tc.cuh"
+#include "seq_lstm.cuh"
 namespace {
 
 __global__ void __launch_bounds__(256) conv_dw_kernel(ConvDw g) {
@@ -728,6 +731,7 @@ struct SeqLayout {
     float* dR; float* dZ; float* dYa; float* dYb;
     float* C; int32_t* keys; float* gs;
     float* part; float* bpart; int splits; int64_t slab;
+    float* G; float* Cs; float* WT;      // LSTM: (4,B,T,D) gates, (B,T,D) cells, 4 x (D,D) W_ih^T blocks
     size_t bytes;
 };
 
@@ -771,7 +775,18 @@ SeqLayout seq_layout(void* base, const slb_seq_step_args* x, bool training) {
     l.hdr = ws.take<int32_t>(16);
     l.seg = seg_index_carve(ws, x->num_items, training ? 2 * B * S : 1);
     l.partial = ws.take<float>(SQ_MAX_GRID);
-    if (L == 0) {
+    if (x->lstm_w_ih) {
+        l.rep_pool = ws.take<float>(B * T * D);          // h_t
+        l.X0 = ws.take<float>(B * S * D);
+        l.G = ws.take<float>(4 * B * T * D);
+        l.Cs = ws.take<float>(B * T * D);
+        l.WT = ws.take<float>(4 * D * D);
+        if (training) {
+            l.splits = use_tc(static_cast<int>(D)) ? dw_splits_tc(B * T, 1) : dw_splits(B * T, static_cast<int>(D), 1);
+            l.part = ws.take<float>(static_cast<size_t>(l.splits) * D * D);
+            l.bpart = ws.take<float>(static_cast<size_t>(l.splits) * D);
+        }
+    } else if (L == 0) {
         l.rep_pool = ws.take<float>(B * T * D);
     } else {
         l.X0 = ws.take<float>(B * S * D);
@@ -825,6 +840,13 @@ int seq_validate(const slb_seq_step_args* x, bool training) {
                         "seq: kernel_width must be in [1,16], dilation >= 1");
         SLB_REQUIRE(x->nonlinearity == 0 || x->nonlinearity == 1, "seq: nonlinearity must be tanh(0) or relu(1)");
     }
+    if (x->lstm_w_ih) {
+        SLB_REQUIRE(x->n_layers == 0, "seq: the LSTM representation takes no conv layers");
+        SLB_REQUIRE(x->dim <= 256, "seq: the fused LSTM supports dim <= 256 (got %d)", x->dim);
+        SLB_REQUIRE(x->lstm_w_hh && x->lstm_b_ih && x->lstm_b_hh, "seq: LSTM parameters missing");
+        if (training)
+            SLB_REQUIRE(x->dlstm_w_ih && x->dlstm_w_hh && x->dlstm_b_ih && x->dlstm_b_hh, "seq: LSTM grads missing");
+    }
     if (training) {
         SLB_REQUIRE(x->negs && x->bias && x->loss_out, "seq: null pointer");
         SLB_REQUIRE(x->opt != SLB_OPT_NONE || (x->dE && x->dbias), "seq: dE / dbias needed without a fused optimizer");
@@ -874,11 +896,166 @@ void conv_shifts(const slb_seq_step_args* x, int layer, int* shift, int* Tin) {
     *Tin = layer == 0 ? x->seq_len : x->seq_len + 1;
 }
 
+// One shifted-row conv GEMM (forward or input gradient): wgmma at D = 128 with W_nc ([j][n][c],
+// the contraction index contiguous), mma.sync otherwise with W_cn ([j][c][n]).
+int launch_conv_gemm(ConvGemm g, const float* W_nc, const float* W_cn, cudaStream_t st, const char* name) {
+    const int64_t rows = g.B * g.Tout;
+    if (use_tc(g.D)) {
+        g.Wm = W_nc;
+        if (tc_configure(tc::tc_conv_gemm_kernel) != 0) { slb_set_error("seq: cannot configure wgmma kernel"); return SLB_ECUDA; }
+        tc::tc_conv_gemm_kernel<<<static_cast<unsigned>((rows + tc::TM - 1) / tc::TM), 128, tc::SMEM_BYTES, st>>>(g);
+    } else {
+        g.Wm = W_cn;
+        dim3 grid(static_cast<unsigned>((rows + GM - 1) / GM), static_cast<unsigned>((g.D + GN - 1) / GN));
+        conv_gemm_kernel<<<grid, 256, 0, st>>>(g);
+    }
+    SLB_LAUNCH_CHECK(name);
+    return SLB_OK;
+}
+
+// One conv weight gradient: split over position slabs into w.part / w.bpart, then the
+// fixed-order reduce into dW (D, D, k) and db (D).
+int launch_conv_dw(ConvDw w, float* dW, float* db, cudaStream_t st) {
+    const int64_t M = w.B * w.Tout;
+    const bool tcp = use_tc(w.D);
+    const int splits = tcp ? dw_splits_tc(M, w.k) : dw_splits(M, w.D, w.k);
+    const int slab_q = tcp ? tc::KC : GK;
+    w.slab = ((M + splits - 1) / splits + slab_q - 1) / slab_q * slab_q;
+    if (tcp) {
+        if (tc_configure(tc::tc_conv_dw_kernel) != 0) { slb_set_error("seq: cannot configure wgmma kernel"); return SLB_ECUDA; }
+        dim3 wg(static_cast<unsigned>(w.k), static_cast<unsigned>(splits));
+        tc::tc_conv_dw_kernel<<<wg, 128, tc::SMEM_BYTES, st>>>(w);
+        SLB_LAUNCH_CHECK("tc_conv_dw_kernel");
+    } else {
+        dim3 wg(static_cast<unsigned>(((w.D + GM - 1) / GM) * ((w.D + GN - 1) / GN)), static_cast<unsigned>(w.k),
+                static_cast<unsigned>(splits));
+        conv_dw_kernel<<<wg, 256, 0, st>>>(w);
+        SLB_LAUNCH_CHECK("conv_dw_kernel");
+    }
+    conv_dw_reduce_kernel<<<sq_grid((static_cast<int64_t>(w.k) * w.D * w.D + w.D + 255) / 256), 256, 0, st>>>(
+        w.part, w.bpart, splits, w.k, w.D, dW, db);
+    SLB_LAUNCH_CHECK("conv_dw_reduce_kernel");
+    return SLB_OK;
+}
+
+// ------------------------------------------------------------------ LSTMNet host side
+// Cluster size c of the recurrence kernels: W_hh (16 D^2 bytes) is split over c CTAs' shared memory.
+int lstm_cluster_size(int D) { return D <= 64 ? 1 : (D <= 128 ? 4 : 8); }
+
+lstm::LstmDev lstm_dev(const slb_seq_step_args* x, const SeqLayout& l, float* H) {
+    lstm::LstmDev a = {};
+    const int D = x->dim, c = lstm_cluster_size(D);
+    a.B = x->batch; a.T = x->seq_len + 1; a.D = D;
+    a.U = (D + c - 1) / c;
+    const int nb = lstm::THREADS / a.U;              // one (sequence, unit) item per thread
+    a.NB = nb > 32 ? 32 : nb;                        // U <= 64, so NB >= 4
+    a.ntiles = static_cast<int>((a.B + a.NB - 1) / a.NB);
+    a.w_hh = x->lstm_w_hh; a.b_ih = x->lstm_b_ih; a.b_hh = x->lstm_b_hh;
+    a.G = l.G; a.Cs = l.Cs; a.H = H; a.dR = l.dR;
+    return a;
+}
+
+// Launches a recurrence kernel on clusters of lstm_cluster_size(D) CTAs: as many clusters as
+// can be resident at once, each walking the sequence tiles.  Refuses to launch when not even
+// one cluster can be scheduled.
+int lstm_launch(void (*kernel)(lstm::LstmDev), const lstm::LstmDev& a, size_t smem_floats, cudaStream_t st,
+                const char* name) {
+    const int c = lstm_cluster_size(a.D);
+    const size_t smem = smem_floats * sizeof(float);
+    SLB_REQUIRE(a.NB >= 1 && a.U * a.NB <= lstm::THREADS, "%s: a tile needs one thread per item", name);
+    if (cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)) != cudaSuccess) {
+        cudaGetLastError();
+        slb_set_error("%s: cannot configure %zu B of shared memory", name, smem);
+        return SLB_ECUDA;
+    }
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeClusterDimension;
+    attr[0].val.clusterDim.x = c;
+    attr[0].val.clusterDim.y = 1;
+    attr[0].val.clusterDim.z = 1;
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3(static_cast<unsigned>(c * a.ntiles));
+    cfg.blockDim = dim3(lstm::THREADS);
+    cfg.dynamicSmemBytes = smem;
+    cfg.stream = st;
+    cfg.attrs = attr;
+    cfg.numAttrs = 1;
+    int active = 0;
+    if (cudaOccupancyMaxActiveClusters(&active, kernel, &cfg) != cudaSuccess || active < 1) {
+        cudaGetLastError();
+        slb_set_error("%s: a cluster of %d CTAs with %zu B of shared memory each cannot be scheduled", name, c, smem);
+        return SLB_ECUDA;
+    }
+    cfg.gridDim = dim3(static_cast<unsigned>(c * (active < a.ntiles ? active : a.ntiles)));
+    if (cudaLaunchKernelEx(&cfg, kernel, a) != cudaSuccess) {
+        slb_set_error("%s: launch failed: %s", name, cudaGetErrorString(cudaGetLastError()));
+        return SLB_ECUDA;
+    }
+    return SLB_OK;
+}
+
+// h_t for t = 0..S into H: gather, four projection GEMMs into G, the recurrence
+int run_lstm_forward(const slb_seq_step_args* x, const SeqLayout& l, float* H, cudaStream_t st) {
+    const int64_t B = x->batch;
+    const int S = x->seq_len, T = S + 1, D = x->dim;
+    const int64_t BTD = B * T * D, DD = static_cast<int64_t>(D) * D;
+    const int lpr = lpr_of(D);
+    SQ_DISPATCH_LPR(lpr, seq_gather_kernel, sq_grid((B * S + SQ_THREADS / lpr - 1) / (SQ_THREADS / lpr)), st,
+                    x->E, x->seqs, B * S, D, x->num_items, l.X0);
+    SLB_LAUNCH_CHECK("seq_gather_kernel");
+    for (int g = 0; g < 4; ++g) {
+        conv_wt_kernel<<<sq_grid((DD + 255) / 256), 256, 0, st>>>(x->lstm_w_ih + g * DD, 1, D, l.WT + g * DD, nullptr);
+        SLB_LAUNCH_CHECK("conv_wt_kernel(lstm)");
+        // x_t = E[seq_{t-1}], x_0 = 0: the layer-0 shift of -1 (representations.py:213-224)
+        ConvGemm p = {};
+        p.In = l.X0; p.Tin = S; p.Out = l.G + g * BTD; p.Tout = T; p.k = 1; p.shift[0] = -1;
+        p.B = B; p.D = D; p.mode = 1;                     // pure GEMM: no bias, no activation
+        const int rc = launch_conv_gemm(p, x->lstm_w_ih + g * DD, l.WT + g * DD, st, "conv_gemm(lstm projection)");
+        if (rc != SLB_OK) return rc;
+    }
+    const lstm::LstmDev a = lstm_dev(x, l, H);
+    return lstm_launch(lstm::lstm_fwd_kernel, a, lstm::fwd_smem_floats(D, a.U, a.NB), st, "lstm_fwd_kernel");
+}
+
+// BPTT from dR, then per gate block: dW_ih, dW_hh (+ both bias gradients) and the input
+// gradient accumulated into the seq-role contribution rows C[b, s] (x_{s+1} = e_s).
+int run_lstm_backward(const slb_seq_step_args* x, const SeqLayout& l, cudaStream_t st) {
+    const int64_t B = x->batch;
+    const int S = x->seq_len, T = S + 1, D = x->dim;
+    const int64_t BTD = B * T * D, DD = static_cast<int64_t>(D) * D;
+    const lstm::LstmDev a = lstm_dev(x, l, l.rep_pool);
+    int rc = lstm_launch(lstm::lstm_bwd_kernel, a, lstm::bwd_smem_floats(D, a.U, a.NB), st, "lstm_bwd_kernel");
+    if (rc != SLB_OK) return rc;
+    for (int g = 0; g < 4; ++g) {
+        ConvDw w = {};                                    // a_t reads x_t = X0[t - 1] and h_{t-1}
+        w.dZ = l.G + g * BTD; w.Tout = T; w.k = 1; w.shift[0] = -1; w.B = B; w.D = D;
+        w.part = l.part; w.bpart = l.bpart;
+        w.In = l.X0; w.Tin = S;
+        rc = launch_conv_dw(w, x->dlstm_w_ih + g * DD, x->dlstm_b_ih + g * D, st);
+        if (rc != SLB_OK) return rc;
+        w.In = l.rep_pool; w.Tin = T;
+        rc = launch_conv_dw(w, x->dlstm_w_hh + g * DD, x->dlstm_b_hh + g * D, st);
+        if (rc != SLB_OK) return rc;
+        ConvGemm d = {};                                  // d e_s = d x_{s+1}
+        d.In = l.G + g * BTD; d.Tin = T; d.Out = l.C; d.Tout = S; d.k = 1; d.shift[0] = 1;
+        d.B = B; d.D = D; d.mode = 1; d.accumulate = 1;
+        rc = launch_conv_gemm(d, l.WT + g * DD, x->lstm_w_ih + g * DD, st, "conv_gemm(lstm dx)");
+        if (rc != SLB_OK) return rc;
+    }
+    return SLB_OK;
+}
+
 // representation forward; returns pointer to the (B,T,D) result inside the workspace
 int run_representation(const slb_seq_step_args* x, const SeqLayout& l, float* rep_dst, cudaStream_t st,
                        float** rep_out) {
     const int64_t B = x->batch;
     const int S = x->seq_len, T = S + 1, D = x->dim;
+    if (x->lstm_w_ih) {
+        float* H = rep_dst ? rep_dst : l.rep_pool;
+        const int rc = run_lstm_forward(x, l, H, st);
+        *rep_out = H;
+        return rc;
+    }
     if (x->n_layers == 0) {
         float* rep = rep_dst ? rep_dst : l.rep_pool;
         const size_t smem = static_cast<size_t>(16) * D * sizeof(float);
@@ -907,17 +1084,10 @@ int run_representation(const slb_seq_step_args* x, const SeqLayout& l, float* re
             g.Res = g.In; g.res_T = g.Tin; g.res_shift = i == 0 ? -1 : 0;   // representations.py:404-407, 419-420
         }
         if (!x->residual && !(last && rep_dst)) g.Out = l.A[i];
-        if (use_tc(D)) {
-            SLB_REQUIRE(l.Wb[i] != nullptr, "seq: wgmma forward needs the [k][out][in] weight copy");
-            g.Wm = l.Wb[i];                                  // [j][n = out][c = in]
-            if (tc_configure(tc::tc_conv_gemm_kernel) != 0) { slb_set_error("seq: cannot configure wgmma kernel"); return SLB_ECUDA; }
-            tc::tc_conv_gemm_kernel<<<static_cast<unsigned>((B * T + tc::TM - 1) / tc::TM), 128, tc::SMEM_BYTES, st>>>(g);
-            SLB_LAUNCH_CHECK("tc_conv_gemm_kernel(fwd)");
-        } else {
-            dim3 grid(static_cast<unsigned>((B * T + GM - 1) / GM), static_cast<unsigned>((D + GN - 1) / GN));
-            conv_gemm_kernel<<<grid, 256, 0, st>>>(g);
-            SLB_LAUNCH_CHECK("conv_gemm_kernel(fwd)");
-        }
+        if (use_tc(D)) SLB_REQUIRE(l.Wb[i] != nullptr, "seq: wgmma forward needs the [k][out][in] weight copy");
+        // Wb = [j][n = out][c = in], Wf = [j][c = in][n = out]
+        const int rc = launch_conv_gemm(g, l.Wb[i], l.Wf[i], st, "conv_gemm(fwd)");
+        if (rc != SLB_OK) return rc;
         *rep_out = g.Out;
     }
     return SLB_OK;
@@ -978,7 +1148,10 @@ int slb_seq_train_step(const slb_seq_step_args* x, slb_stream_t stream) {
     SQ_DISPATCH_LPR(lpr, seq_score_kernel, sq_grid((B * T + groups - 1) / groups), st, a);
     SLB_LAUNCH_CHECK("seq_score_kernel");
 
-    if (x->n_layers == 0) {
+    if (x->lstm_w_ih) {
+        rc = run_lstm_backward(x, l, st);
+        if (rc != SLB_OK) return rc;
+    } else if (x->n_layers == 0) {
         const size_t smem = static_cast<size_t>(16) * D * sizeof(float);
         SQ_DISPATCH_NCH(D, pool_bwd_kernel, static_cast<unsigned>(B), smem, st, x->E, x->seqs, S, D, x->num_items, l.dR, l.C);
         SLB_LAUNCH_CHECK("pool_bwd_kernel");
@@ -995,43 +1168,21 @@ int slb_seq_train_step(const slb_seq_step_args* x, slb_stream_t stream) {
             conv_shifts(x, i, w.shift, &w.Tin);
             w.In = i == 0 ? l.X0 : l.Y[i - 1];
             w.dZ = l.dZ; w.Tout = T; w.k = k; w.B = B; w.D = D;
-            const bool tcp = use_tc(D);
-            const int splits = tcp ? dw_splits_tc(B * T, k) : dw_splits(B * T, D, k);
-            const int slab_q = tcp ? tc::KC : GK;
-            w.slab = ((B * T + splits - 1) / splits + slab_q - 1) / slab_q * slab_q;
             w.part = l.part; w.bpart = l.bpart;
-            if (tcp) {
-                if (tc_configure(tc::tc_conv_dw_kernel) != 0) { slb_set_error("seq: cannot configure wgmma kernel"); return SLB_ECUDA; }
-                dim3 wg(static_cast<unsigned>(k), static_cast<unsigned>(splits));
-                tc::tc_conv_dw_kernel<<<wg, 128, tc::SMEM_BYTES, st>>>(w);
-                SLB_LAUNCH_CHECK("tc_conv_dw_kernel");
-            } else {
-                dim3 wg(static_cast<unsigned>(((D + GM - 1) / GM) * ((D + GN - 1) / GN)), static_cast<unsigned>(k),
-                        static_cast<unsigned>(splits));
-                conv_dw_kernel<<<wg, 256, 0, st>>>(w);
-                SLB_LAUNCH_CHECK("conv_dw_kernel");
-            }
-            conv_dw_reduce_kernel<<<sq_grid((static_cast<int64_t>(k) * D * D + D + 255) / 256), 256, 0, st>>>(
-                l.part, l.bpart, splits, k, D, x->dconv_w[i], x->dconv_b[i]);
-            SLB_LAUNCH_CHECK("conv_dw_reduce_kernel");
+            rc = launch_conv_dw(w, x->dconv_w[i], x->dconv_b[i], st);
+            if (rc != SLB_OK) return rc;
             // input gradient: shifted GEMM over dZ with the transposed weights
             ConvGemm g = {};
             int fshift[16], Tin;
             conv_shifts(x, i, fshift, &Tin);
             for (int j = 0; j < k; ++j) g.shift[j] = -fshift[j];
-            g.In = l.dZ; g.Tin = T; g.Tout = Tin; g.Wm = l.Wb[i]; g.k = k; g.B = B; g.D = D; g.mode = 1;
+            g.In = l.dZ; g.Tin = T; g.Tout = Tin; g.k = k; g.B = B; g.D = D; g.mode = 1;
             if (x->residual) { g.Res = dY; g.res_T = T; g.res_shift = i == 0 ? 1 : 0; }
             if (i == 0) { g.Out = l.C; g.accumulate = 1; }      // seq-role rows C[b, s] += d e_s
             else { g.Out = ping; }
-            if (tcp) {
-                g.Wm = l.Wf[i];                              // [j][n = in][c = out]
-                tc::tc_conv_gemm_kernel<<<static_cast<unsigned>((B * Tin + tc::TM - 1) / tc::TM), 128, tc::SMEM_BYTES, st>>>(g);
-                SLB_LAUNCH_CHECK("tc_conv_gemm_kernel(dx)");
-            } else {
-                dim3 grid(static_cast<unsigned>((B * Tin + GM - 1) / GM), static_cast<unsigned>((D + GN - 1) / GN));
-                conv_gemm_kernel<<<grid, 256, 0, st>>>(g);
-                SLB_LAUNCH_CHECK("conv_gemm_kernel(dx)");
-            }
+            // Wf = [j][n = in][c = out], Wb = [j][c = out][n = in]
+            rc = launch_conv_gemm(g, l.Wf[i], l.Wb[i], st, "conv_gemm(dx)");
+            if (rc != SLB_OK) return rc;
             if (i > 0) { dY = ping; float* tmp = ping; ping = pong; pong = tmp; }
         }
     }

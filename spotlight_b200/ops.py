@@ -617,8 +617,9 @@ class _HostPtrArray(object):
         return ctypes.cast(arr, ctypes.c_void_p)
 
 
-def seq_step_args(E, bias, seqs, negs, loss, n_neg, cnn=None, keep=None):
-    """cnn: None (PoolNet) or dict(kernel_width, dilation, nonlinearity, residual, weights, biases)."""
+def seq_step_args(E, bias, seqs, negs, loss, n_neg, cnn=None, keep=None, lstm=None):
+    """cnn: None (PoolNet) or dict(kernel_width, dilation, nonlinearity, residual, weights, biases);
+    lstm: None or dict(w_ih, w_hh, b_ih, b_hh) (LSTMNet, nn.LSTM shapes)."""
     keep = keep if keep is not None else _HostPtrArray()
     a = SeqStepArgs()
     a.batch, a.seq_len = int(seqs.shape[0]), int(seqs.shape[1])
@@ -636,15 +637,31 @@ def seq_step_args(E, bias, seqs, negs, loss, n_neg, cnn=None, keep=None):
         a.residual = 1 if cnn['residual'] else 0
         a.conv_w = keep.ptrs(cnn['weights'])
         a.conv_b = keep.ptrs(cnn['biases'])
+    if lstm is not None:
+        a.lstm_w_ih, a.lstm_w_hh = lstm['w_ih'].data_ptr(), lstm['w_hh'].data_ptr()
+        a.lstm_b_ih, a.lstm_b_hh = lstm['b_ih'].data_ptr(), lstm['b_hh'].data_ptr()
     return a, keep
 
 
-def seq_train_step(E, bias, seqs, negs, loss, n_neg, cnn=None, want_scores=False, norm_count=None, fused=None):
+_LSTM_KEYS = ('w_ih', 'w_hh', 'b_ih', 'b_hh')
+
+
+def _lstm_params(lstm):
+    if lstm is None:
+        return None
+    require_cuda(*[lstm[k] for k in _LSTM_KEYS])
+    return {k: _f32c(lstm[k]) for k in _LSTM_KEYS}
+
+
+def seq_train_step(E, bias, seqs, negs, loss, n_neg, cnn=None, want_scores=False, norm_count=None, fused=None,
+                   lstm=None):
     """Fused forward + backward of one sequence minibatch, dense gradients.
 
-    Returns dict(loss, pos, neg, dE, dbias, dconv_w, dconv_b).  ``fused`` = dict(kind, lr,
+    Returns dict(loss, pos, neg, dE, dbias, dconv_w, dconv_b, dlstm).  ``fused`` = dict(kind, lr,
     weight_decay, eps, state_E, state_bias): the row-wise optimizer is applied to ``E`` / ``bias`` in
     place inside the step (no dense item-table gradient exists; ``dE`` / ``dbias`` are None).
+    ``lstm`` = dict(w_ih, w_hh, b_ih, b_hh) selects the LSTMNet representation; ``dlstm`` then holds
+    the gradients under the same keys.
     """
     require_cuda(E, bias, seqs, negs)
     lib = _lib.load()
@@ -656,8 +673,10 @@ def seq_train_step(E, bias, seqs, negs, loss, n_neg, cnn=None, want_scores=False
         cnn = dict(cnn)
         cnn['weights'] = [_f32c(w) for w in cnn['weights']]
         cnn['biases'] = [_f32c(b) for b in cnn['biases']]
-    a, keep = seq_step_args(E, bias, seqs, negs, loss, n_neg, cnn)
-    out = dict(loss=torch.empty(1, dtype=torch.float32, device=dev), dE=None, dbias=None, dconv_w=[], dconv_b=[])
+    lstm = _lstm_params(lstm)
+    a, keep = seq_step_args(E, bias, seqs, negs, loss, n_neg, cnn, lstm=lstm)
+    out = dict(loss=torch.empty(1, dtype=torch.float32, device=dev), dE=None, dbias=None, dconv_w=[], dconv_b=[],
+               dlstm=None)
     if fused is None:
         out['dE'], out['dbias'] = torch.zeros_like(E), torch.zeros_like(bias)
     a.loss_out = out['loss'].data_ptr()
@@ -678,6 +697,10 @@ def seq_train_step(E, bias, seqs, negs, loss, n_neg, cnn=None, want_scores=False
         out['dconv_b'] = [torch.zeros_like(b) for b in cnn['biases']]
         a.dconv_w = keep.ptrs(out['dconv_w'])
         a.dconv_b = keep.ptrs(out['dconv_b'])
+    if lstm is not None:
+        out['dlstm'] = {k: torch.zeros_like(lstm[k]) for k in _LSTM_KEYS}
+        a.dlstm_w_ih, a.dlstm_w_hh = out['dlstm']['w_ih'].data_ptr(), out['dlstm']['w_hh'].data_ptr()
+        a.dlstm_b_ih, a.dlstm_b_hh = out['dlstm']['b_ih'].data_ptr(), out['dlstm']['b_hh'].data_ptr()
     need = lib.slb_seq_step_workspace_bytes(ctypes.byref(a))
     ws = workspace('seq%d' % a.num_items, need, dev)
     a.workspace, a.workspace_bytes = ws.data_ptr(), ws.numel()
@@ -686,7 +709,7 @@ def seq_train_step(E, bias, seqs, negs, loss, n_neg, cnn=None, want_scores=False
     return out
 
 
-def seq_representation(E, seqs, cnn=None):
+def seq_representation(E, seqs, cnn=None, lstm=None):
     """(B, S+1, D) causal representations: entry t has seen items < t."""
     require_cuda(E, seqs)
     lib = _lib.load()
@@ -697,8 +720,9 @@ def seq_representation(E, seqs, cnn=None):
         cnn = dict(cnn)
         cnn['weights'] = [_f32c(w) for w in cnn['weights']]
         cnn['biases'] = [_f32c(b) for b in cnn['biases']]
+    lstm = _lstm_params(lstm)
     dummy_bias = torch.zeros(1, dtype=torch.float32, device=E.device)
-    a, keep = seq_step_args(E, dummy_bias, seqs, None, 0, 1, cnn)
+    a, keep = seq_step_args(E, dummy_bias, seqs, None, 0, 1, cnn, lstm=lstm)
     rep = torch.empty((B, S + 1, E.shape[1]), dtype=torch.float32, device=E.device)
     need = lib.slb_seq_step_workspace_bytes(ctypes.byref(a))
     ws = workspace('seq%d' % a.num_items, need, E.device)

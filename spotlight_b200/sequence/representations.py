@@ -1,14 +1,13 @@
 """Sequence representations with the reference's classes, constructor
 arguments and parameter names (spotlight/sequence/representations.py:27-596).
 
-``PoolNet`` and ``CNNNet`` run on the kernels of csrc/seq.cu; both keep the
-reference's module protocol -- ``user_representation(item_sequences) ->
+``PoolNet``, ``CNNNet`` and ``LSTMNet`` run on the kernels of csrc/seq.cu; all
+keep the reference's module protocol -- ``user_representation(item_sequences) ->
 (all_steps (B, D, S), final (B, D))`` and ``forward(user_representations,
 targets) -> (B, S)`` -- so they also work with external training loops and the
-reference's evaluation code.  ``LSTMNet`` / ``MixtureLSTMNet`` are outside the
-accelerated path (SURVEY §2) and are provided as stock ``torch.nn`` modules on
-top of this package's embedding layers so ``representation='lstm'|'mixture'``
-still constructs.
+reference's evaluation code.  ``MixtureLSTMNet`` is outside the accelerated path
+and is provided as stock ``torch.nn`` modules on top of this package's embedding
+layers so ``representation='mixture'`` still constructs.
 """
 
 import torch
@@ -36,6 +35,12 @@ class _SeqNetBase(nn.Module):
     def _cnn_spec(self):
         return None
 
+    def _lstm_spec(self):
+        return None
+
+    def _autograd_params(self):
+        return (self.item_embeddings.weight,)
+
     def fusable(self):
         emb = self.item_embeddings
         return (type(emb) is ScaledEmbedding and emb.padding_idx == PADDING_IDX and not emb.sparse
@@ -45,13 +50,14 @@ class _SeqNetBase(nn.Module):
     def user_representation(self, item_sequences):
         """``(all, final)``: ``all[:, :, t]`` has seen items before ``t``
         (t = 0..S-1), ``final`` has seen the whole sequence."""
-        if not self.fusable() or (torch.is_grad_enabled() and self.item_embeddings.weight.requires_grad):
+        if not self.fusable() or (torch.is_grad_enabled()
+                                  and any(p.requires_grad for p in self._autograd_params())):
             # custom / Bloom item layers, or an external training loop that needs
             # autograd through the representation: differentiable composition over
             # this package's embedding op (not the measured path)
             return self._user_representation_autograd(item_sequences)
         rep = ops.seq_representation(self.item_embeddings.weight.detach(),
-                                     item_sequences, self._cnn_spec())
+                                     item_sequences, self._cnn_spec(), lstm=self._lstm_spec())
         rep = rep.permute(0, 2, 1)                      # (B, D, S+1) like the reference
         return rep[:, :, :-1], rep[:, :, -1]
 
@@ -146,9 +152,18 @@ class CNNNet(_SeqNetBase):
                     biases=[layer.bias for layer in self.cnn_layers])
 
 
-class LSTMNet(nn.Module):
-    """LSTM over the item sequence (representations.py:147-258).  Stock
-    ``nn.LSTM``; not on the accelerated path."""
+class LSTMNet(_SeqNetBase):
+    """Single-layer LSTM over the left zero-padded item sequence (representations.py:147-258).
+
+    Parameters: embeddings/biases as ``PoolNet`` plus ``lstm.weight_ih_l0``, ``lstm.weight_hh_l0``
+    ``(4D, D)`` and ``lstm.bias_ih_l0``, ``lstm.bias_hh_l0`` ``(4D,)`` -- the reference's
+    ``nn.LSTM``, which stays the parameter holder, so ``state_dict``s interchange.  On a plain
+    item table with ``D <= 256`` the representation runs on the recurrence kernels of
+    csrc/seq_lstm.cuh; otherwise (Bloom items, larger ``D``) and whenever autograd needs the
+    representation, ``nn.LSTM`` computes it.
+    """
+
+    LSTM_MAX_DIM = 256
 
     def __init__(self, num_items, embedding_dim=32, item_embedding_layer=None, sparse=False):
         super(LSTMNet, self).__init__()
@@ -160,17 +175,23 @@ class LSTMNet(nn.Module):
         self.lstm = nn.LSTM(batch_first=True, input_size=embedding_dim, hidden_size=embedding_dim)
 
     def fusable(self):
-        return False
+        return (super(LSTMNet, self).fusable()
+                and self.item_embeddings.embedding_dim <= self.LSTM_MAX_DIM
+                and self.lstm.num_layers == 1 and self.lstm.bias and not self.lstm.bidirectional)
 
-    def user_representation(self, item_sequences):
+    def _autograd_params(self):
+        return (self.item_embeddings.weight,) + tuple(self.lstm.parameters())
+
+    def _user_representation_autograd(self, item_sequences):
         emb = self.item_embeddings(item_sequences).permute(0, 2, 1).unsqueeze(3)
         emb = F.pad(emb, (0, 0, 1, 0)).squeeze(3).permute(0, 2, 1)
         out, _ = self.lstm(emb)
         out = out.permute(0, 2, 1)
         return out[:, :, :-1], out[:, :, -1]
 
-    def forward(self, user_representations, targets):
-        return _SeqNetBase.forward(self, user_representations, targets)
+    def _lstm_spec(self):
+        return dict(w_ih=self.lstm.weight_ih_l0.detach(), w_hh=self.lstm.weight_hh_l0.detach(),
+                    b_ih=self.lstm.bias_ih_l0.detach(), b_hh=self.lstm.bias_hh_l0.detach())
 
 
 class MixtureLSTMNet(nn.Module):
