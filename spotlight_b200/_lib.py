@@ -17,7 +17,9 @@ LIB_PATH = os.environ.get('SLB_LIBRARY') or os.path.join(_HERE, 'libspotlight_b2
 c_i32, c_i64, c_f32 = ctypes.c_int32, ctypes.c_int64, ctypes.c_float
 c_vp, c_sz = ctypes.c_void_p, ctypes.c_size_t
 
-LOSS_KIND = {'pointwise': 0, 'bpr': 1, 'hinge': 2, 'adaptive_hinge': 3}
+LOSS_KIND = {'pointwise': 0, 'bpr': 1, 'hinge': 2, 'adaptive_hinge': 3,
+             'regression': 4, 'poisson': 5, 'logistic': 6}
+RATING_LOSSES = ('regression', 'poisson', 'logistic')
 GRAD_DENSE, GRAD_COMPACT = 0, 1
 OPT_NONE, OPT_SGD, OPT_ADAGRAD, OPT_ADAM = 0, 1, 2, 3
 
@@ -35,7 +37,7 @@ EXPORTS = (
     'slb_mf_bloom_workspace_bytes', 'slb_mf_bloom_train_step',
     'slb_bias_sparse_workspace_bytes', 'slb_bias_sparse_apply',
     'slb_unique_workspace_bytes', 'slb_unique_bucket', 'slb_shard_gather_batch', 'slb_adagrad_dense',
-    'slb_loss_workspace_bytes', 'slb_pairwise_loss',
+    'slb_loss_workspace_bytes', 'slb_pairwise_loss', 'slb_rating_loss',
     'slb_seq_step_workspace_bytes', 'slb_seq_train_step', 'slb_seq_representation',
 )
 
@@ -61,6 +63,7 @@ class MfStepArgs(ctypes.Structure):
         ('beta1', c_f32), ('beta2', c_f32), ('one_minus_beta1', c_f32), ('one_minus_beta2', c_f32),
         ('state2_Wu', c_vp), ('state2_Wi', c_vp), ('state2_bu', c_vp), ('state2_bi', c_vp),
         ('last_u', c_vp), ('last_i', c_vp), ('adam_sched', c_vp), ('adam_step', c_i64),
+        ('ratings', c_vp),
     ]
 
 
@@ -162,6 +165,7 @@ def _declare(lib):
     lib.slb_loss_workspace_bytes.restype = c_sz
     lib.slb_pairwise_loss.argtypes = [c_i32, c_vp, c_vp, c_vp, c_i64, c_i32, c_vp, c_vp, c_vp,
                                       c_vp, c_sz, c_vp]
+    lib.slb_rating_loss.argtypes = [c_i32, c_vp, c_vp, c_i64, c_vp, c_vp, c_vp, c_sz, c_vp]
     lib.slb_seq_step_workspace_bytes.argtypes = [P(SeqStepArgs)]
     lib.slb_seq_step_workspace_bytes.restype = c_sz
     lib.slb_seq_train_step.argtypes = [P(SeqStepArgs), c_vp]

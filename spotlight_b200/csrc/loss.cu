@@ -100,6 +100,55 @@ loss_grad_kernel(int loss, const float* __restrict__ pos, const float* __restric
     }
 }
 
+// Rating losses on the prediction the caller hands in (poisson: already exp(score)),
+// spotlight/losses.py:188-244.  d = d per / d pred.
+__device__ __forceinline__ void rating_elem(int loss, float p, float r, float& per, float& d) {
+    if (loss == SLB_LOSS_REGRESSION) {
+        const float e = r - p;
+        per = e * e; d = -2.0f * e;
+    } else if (loss == SLB_LOSS_POISSON) {
+        per = p - r * logf(p); d = 1.0f - r / p;
+    } else {
+        const float t = fminf(fmaxf(r, 0.0f), 1.0f);       // (-1, 1) targets -> (0, 1), losses.py:240
+        per = fmaxf(p, 0.0f) - p * t + log1pf(expf(-fabsf(p)));
+        d = sigmoidf_(p) - t;
+    }
+}
+
+// One pass: per-element gradients (the divisor n is known up front) and the block partials;
+// the last block folds the partials in a fixed order.
+__global__ void __launch_bounds__(L_THREADS)
+rating_loss_kernel(int loss, const float* __restrict__ pred, const float* __restrict__ ratings, int64_t n,
+                   float* partial, int32_t* done, float* loss_out, float* __restrict__ grad) {
+    __shared__ float red[L_THREADS / 32];
+    __shared__ bool is_last;
+    const float inv = 1.0f / static_cast<float>(n);
+    float ls = 0.f;
+    for (int64_t i = static_cast<int64_t>(blockIdx.x) * L_THREADS + threadIdx.x; i < n;
+         i += static_cast<int64_t>(gridDim.x) * L_THREADS) {
+        float per, d;
+        rating_elem(loss, pred[i], ratings[i], per, d);
+        ls += per;
+        if (grad) grad[i] = d * inv;
+    }
+    const float bl = block_sum<L_THREADS>(ls, red);
+    if (threadIdx.x == 0) {
+        partial[blockIdx.x] = bl;
+        __threadfence();
+        is_last = atomicAdd(done, 1) == static_cast<int>(gridDim.x) - 1;
+    }
+    __syncthreads();
+    if (is_last && threadIdx.x < 32) {
+        __threadfence();
+        float a = 0.f;
+        for (int k = threadIdx.x; k < static_cast<int>(gridDim.x); k += 32)
+            a += *reinterpret_cast<volatile float*>(partial + k);
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) a += __shfl_down_sync(0xffffffffu, a, o);
+        if (threadIdx.x == 0) { *loss_out = a * inv; *done = 0; }
+    }
+}
+
 }  // namespace
 
 extern "C" {
@@ -138,6 +187,29 @@ int slb_pairwise_loss(int32_t loss, const float* pos, const float* neg, const ui
         loss_grad_kernel<<<grid, L_THREADS, 0, st>>>(loss, pos, neg, mask, n, n_neg, sums, gpos, gneg);
         SLB_LAUNCH_CHECK("loss_grad_kernel");
     }
+    return SLB_OK;
+}
+
+int slb_rating_loss(int32_t loss, const float* pred, const float* ratings, int64_t n,
+                    float* loss_out, float* grad, void* workspace, size_t workspace_bytes,
+                    slb_stream_t stream) {
+    SLB_REQUIRE(loss >= SLB_LOSS_REGRESSION && loss <= SLB_LOSS_LOGISTIC, "rating_loss: bad loss kind %d", loss);
+    SLB_REQUIRE(pred && ratings && loss_out && workspace, "rating_loss: null pointer");
+    SLB_REQUIRE(n > 0, "rating_loss: n must be > 0");
+    if (workspace_bytes < slb_loss_workspace_bytes(n)) {
+        slb_set_error("rating_loss: workspace too small");
+        return SLB_ENOSPC;
+    }
+    WsCarver ws(workspace);
+    int32_t* done = ws.take<int32_t>(8);
+    ws.take<float>(8);
+    float* partial = ws.take<float>(2 * L_MAX_GRID);
+    const int64_t want = (n + L_THREADS - 1) / L_THREADS;
+    const int64_t cap = static_cast<int64_t>(slb_sms()) * 8 < L_MAX_GRID ? static_cast<int64_t>(slb_sms()) * 8 : L_MAX_GRID;
+    const int grid = static_cast<int>(want < cap ? want : cap);
+    rating_loss_kernel<<<grid, L_THREADS, 0, static_cast<cudaStream_t>(stream)>>>(loss, pred, ratings, n, partial,
+                                                                                  done, loss_out, grad);
+    SLB_LAUNCH_CHECK("rating_loss_kernel");
     return SLB_OK;
 }
 

@@ -55,7 +55,12 @@ struct MfDev {
     // hashed-table mode: bias grads are handled outside the segments; frozen rows get no grad
     int32_t no_bias;
     int64_t frozen_a, frozen_b;     // table rows that receive no gradient (-1 = none)
+    const float* ratings;           // [B], rating losses only
 };
+
+__host__ __device__ __forceinline__ bool is_rating_loss(int loss) {
+    return loss >= SLB_LOSS_REGRESSION && loss <= SLB_LOSS_LOGISTIC;
+}
 
 template <int LPR>
 __device__ __forceinline__ float row_dot(const float* __restrict__ a, const float* __restrict__ b,
@@ -83,6 +88,25 @@ __device__ __forceinline__ void pair_loss(int loss, float p, float n, float& per
         const float act = z >= 0.0f ? 1.0f : 0.0f;  // clamp backward passes at the boundary
         gp = -act;
         gn = act;
+    }
+}
+
+// Rating losses on the raw score s of one interaction with observed rating r: the loss term
+// and d loss_b / d s (unscaled by 1/B).  spotlight/losses.py:169-244 with fit's exp for poisson
+// (spotlight/factorization/explicit.py:225-226): d/ds of exp(s) - r log(exp(s)) is exp(s) - r.
+__device__ __forceinline__ void rating_loss(int loss, float s, float r, float& per, float& g) {
+    if (loss == SLB_LOSS_REGRESSION) {
+        const float d = s - r;
+        per = d * d;
+        g = 2.0f * d;
+    } else if (loss == SLB_LOSS_POISSON) {
+        const float p = expf(s);
+        per = p - r * logf(p);
+        g = p - r;
+    } else {                                  // logistic: BCE with logits against clamp(r, 0, 1)
+        const float t = fminf(fmaxf(r, 0.0f), 1.0f);
+        per = fmaxf(s, 0.0f) - s * t + log1pf(expf(-fabsf(s)));
+        g = sigmoidf_(s) - t;
     }
 }
 
@@ -197,6 +221,8 @@ __global__ void __launch_bounds__(MF_TILE_THREADS) mf_fwd_tile_kernel(MfDev a) {
     __shared__ bool is_last;
     constexpr int GPW = 32 / LPR;            // groups per warp
     constexpr int ITERS = TI / GPW > 0 ? TI / GPW : 1;
+    // rating losses: one row pair and one gradient term per interaction, term id b (not 2b, 2b+1)
+    constexpr bool RATING = LOSS >= SLB_LOSS_REGRESSION;
     const int lane = threadIdx.x & 31;
     const int gl = lane & (LPR - 1);
     const int grp = lane / LPR;
@@ -214,34 +240,58 @@ __global__ void __launch_bounds__(MF_TILE_THREADS) mf_fwd_tile_kernel(MfDev a) {
         const int64_t b = tile * TI + lane;
         const bool valid = lane < TI && b < a.B;
         int64_t u64 = 0, i64 = 0, j64 = 0;
-        if (valid) { u64 = a.users[b]; i64 = a.items[b]; j64 = a.negs[b]; }
+        float r = 0.f;
+        if (valid) {
+            u64 = a.users[b]; i64 = a.items[b];
+            if (RATING) r = a.ratings[b]; else j64 = a.negs[b];
+        }
         const bool bad = u64 < 0 || u64 >= a.U || i64 < 0 || i64 >= a.I || j64 < 0 || j64 >= a.I;
         if (bad) { u64 = 0; i64 = 0; j64 = 0; }
         const int u = static_cast<int>(u64), i = static_cast<int>(i64), j = static_cast<int>(j64);
-        const float ub = __ldg(a.bu + u), ib = __ldg(a.bi + i), jb = __ldg(a.bi + j);
+        const float ub = __ldg(a.bu + u), ib = __ldg(a.bi + i), jb = RATING ? 0.f : __ldg(a.bi + j);
         float dpm = 0.f, dnm = 0.f;
 #pragma unroll 4
         for (int s = 0; s < ITERS; ++s) {
             const int src = (s * GPW + grp) % TI;       // TI < GPW: surplus groups recompute
             const int uu = __shfl_sync(0xffffffffu, u, src);
             const int ii = __shfl_sync(0xffffffffu, i, src);
-            const int jj = __shfl_sync(0xffffffffu, j, src);
             const float* ur = a.Wu + static_cast<int64_t>(uu) * D;
             const float* qi = a.Wi + static_cast<int64_t>(ii) * D;
-            const float* qj = a.Wi + static_cast<int64_t>(jj) * D;
             float dp = 0.f, dn = 0.f;
-            for (int c = gl * 4; c < D; c += LPR * 4) {
-                const float4 u4 = ldg4(ur + c), i4 = ldg4(qi + c), j4 = ldg4(qj + c);
-                dp += dot4(u4, i4);
-                dn += dot4(u4, j4);
+            if constexpr (RATING) {
+                for (int c = gl * 4; c < D; c += LPR * 4) dp += dot4(ldg4(ur + c), ldg4(qi + c));
+            } else {
+                const int jj = __shfl_sync(0xffffffffu, j, src);
+                const float* qj = a.Wi + static_cast<int64_t>(jj) * D;
+                for (int c = gl * 4; c < D; c += LPR * 4) {
+                    const float4 u4 = ldg4(ur + c), i4 = ldg4(qi + c), j4 = ldg4(qj + c);
+                    dp += dot4(u4, i4);
+                    dn += dot4(u4, j4);
+                }
             }
-            dp = group_sum<LPR>(dp, 0xffffffffu);
-            dn = group_sum<LPR>(dn, 0xffffffffu);
-            const float tp = __shfl_sync(0xffffffffu, dp, (lane % GPW) * LPR);
-            const float tn = __shfl_sync(0xffffffffu, dn, (lane % GPW) * LPR);
-            if (lane / GPW == s) { dpm = tp; dnm = tn; }
+            if constexpr (RATING) {
+                dp = group_sum<LPR>(dp, 0xffffffffu);
+                const float tp = __shfl_sync(0xffffffffu, dp, (lane % GPW) * LPR);
+                if (lane / GPW == s) dpm = tp;
+            } else {
+                dp = group_sum<LPR>(dp, 0xffffffffu);
+                dn = group_sum<LPR>(dn, 0xffffffffu);
+                const float tp = __shfl_sync(0xffffffffu, dp, (lane % GPW) * LPR);
+                const float tn = __shfl_sync(0xffffffffu, dn, (lane % GPW) * LPR);
+                if (lane / GPW == s) { dpm = tp; dnm = tn; }
+            }
         }
-        if (valid) {
+        if (RATING && valid) {
+            const float p = dpm + ub + ib;
+            float per, g;
+            rating_loss(LOSS, p, r, per, g);
+            lsum += per;
+            g *= invB;
+            if (bad) { atomicExch(a.err, 1); g = 0.f; }
+            if (a.pos_out) a.pos_out[b] = p;
+            a.t_a[b] = u; a.t_b[b] = i; a.t_g[b] = g;
+            if (g != 0.f) { atomicAdd(a.seg.cnt + u, 1); atomicAdd(a.seg.cnt + a.U + i, 1); }
+        } else if (valid) {
             const float p = dpm + ub + ib, n = dnm + ub + jb;
             float per, gp, gn;
             pair_loss(LOSS, p, n, per, gp, gn);
@@ -969,16 +1019,18 @@ struct MfLayout {
     size_t bytes;
 };
 
-MfLayout mf_layout(void* base, int64_t B, int64_t U, int64_t I) {
+// terms_per: gradient terms per interaction (2: positive + negative, 1: rating losses)
+MfLayout mf_layout(void* base, int64_t B, int64_t U, int64_t I, int terms_per = 2) {
     WsCarver ws(base);
     MfLayout l;
-    // persistent (zero-at-rest) part first
+    const int64_t T = terms_per * B;
+    // persistent (zero-at-rest) part first, at offsets that depend on U + I only
     l.done = ws.take<int32_t>(8);
     l.err = l.done + 4;
-    l.seg = seg_index_carve(ws, U + I, 4 * B);
-    l.t_a = ws.take<int32_t>(2 * B);
-    l.t_b = ws.take<int32_t>(2 * B);
-    l.t_g = ws.take<float>(2 * B);
+    l.seg = seg_index_carve(ws, U + I, 2 * T);
+    l.t_a = ws.take<int32_t>(T);
+    l.t_b = ws.take<int32_t>(T);
+    l.t_g = ws.take<float>(T);
     l.partial = ws.take<float>(MF_MAX_GRID);
     l.bytes = ws.bytes();
     return l;
@@ -1044,14 +1096,20 @@ int validate(const slb_mf_step_args* x) {
     SLB_REQUIRE(x != nullptr, "mf_train_step: null args");
     SLB_REQUIRE(x->batch > 0, "mf_train_step: batch must be > 0");
     SLB_REQUIRE(x->dim >= 4 && x->dim % 4 == 0, "mf_train_step: dim must be a positive multiple of 4 (got %d)", x->dim);
-    SLB_REQUIRE(x->loss >= 0 && x->loss <= 3, "mf_train_step: bad loss kind %d", x->loss);
+    SLB_REQUIRE(x->loss >= 0 && x->loss <= SLB_LOSS_LOGISTIC, "mf_train_step: bad loss kind %d", x->loss);
     SLB_REQUIRE(x->n_neg >= 1, "mf_train_step: n_neg must be >= 1");
     SLB_REQUIRE(x->loss == SLB_LOSS_ADAPTIVE_HINGE || x->n_neg == 1, "mf_train_step: n_neg > 1 only for adaptive hinge");
     SLB_REQUIRE(x->num_users > 0 && x->num_items > 0, "mf_train_step: empty tables");
     SLB_REQUIRE(x->num_users + x->num_items < (1ll << 31) - SEG_SCAN_TILE, "mf_train_step: num_users + num_items must be < 2^31");
     SLB_REQUIRE(x->batch * 4 < (1ll << 31), "mf_train_step: batch too large");
-    SLB_REQUIRE(x->users && x->items && x->negs && x->Wu && x->Wi && x->bu && x->bi && x->loss_out,
+    SLB_REQUIRE(x->users && x->items && x->Wu && x->Wi && x->bu && x->bi && x->loss_out,
                 "mf_train_step: null pointer");
+    if (is_rating_loss(x->loss)) {
+        SLB_REQUIRE(x->ratings != nullptr && x->negs == nullptr && x->neg_out == nullptr,
+                    "mf_train_step: rating losses need ratings and take no negatives");
+    } else {
+        SLB_REQUIRE(x->negs != nullptr, "mf_train_step: null negs");
+    }
     SLB_REQUIRE(x->workspace != nullptr, "mf_train_step: null workspace");
     if (x->grad_mode == SLB_GRAD_DENSE) {
         if (x->opt != SLB_OPT_NONE) {
@@ -1091,12 +1149,13 @@ int validate(const slb_mf_step_args* x) {
 }
 
 int launch_step(const slb_mf_step_args* x, const int64_t* users, const int64_t* items,
-                const int64_t* negs, int64_t B, float* loss_out, cudaStream_t st,
+                const int64_t* negs, const float* ratings, int64_t B, float* loss_out, cudaStream_t st,
                 int phases = 0x1f, int64_t step_idx = 0) {
     // layout is sized for x->batch so that short last batches reuse the same carve
-    MfLayout l = mf_layout(x->workspace, x->batch, x->num_users, x->num_items);
+    MfLayout l = mf_layout(x->workspace, x->batch, x->num_users, x->num_items, is_rating_loss(x->loss) ? 1 : 2);
     MfDev a;
-    a.B = B; a.NB = x->norm_batch > 0 ? x->norm_batch : B; a.T = 2 * B; a.users = users; a.items = items; a.negs = negs;
+    a.B = B; a.NB = x->norm_batch > 0 ? x->norm_batch : B; a.T = is_rating_loss(x->loss) ? B : 2 * B;
+    a.users = users; a.items = items; a.negs = negs; a.ratings = ratings;
     a.loss = x->loss; a.n_neg = x->n_neg;
     a.U = x->num_users; a.I = x->num_items; a.D = x->dim;
     a.Wu = x->Wu; a.Wi = x->Wi; a.bu = x->bu; a.bi = x->bi;
@@ -1146,6 +1205,9 @@ int launch_step(const slb_mf_step_args* x, const int64_t* users, const int64_t* 
             switch (x->loss) {
                 case SLB_LOSS_POINTWISE: FWD_TILE(SLB_LOSS_POINTWISE); break;
                 case SLB_LOSS_BPR: FWD_TILE(SLB_LOSS_BPR); break;
+                case SLB_LOSS_REGRESSION: FWD_TILE(SLB_LOSS_REGRESSION); break;
+                case SLB_LOSS_POISSON: FWD_TILE(SLB_LOSS_POISSON); break;
+                case SLB_LOSS_LOGISTIC: FWD_TILE(SLB_LOSS_LOGISTIC); break;
                 default: FWD_TILE(SLB_LOSS_HINGE); break;
             }
         }
@@ -1266,7 +1328,7 @@ V2Layout v2_layout(void* base, int64_t B, int64_t U, int64_t I, int D) {
         p.words = (2 * B + 31) / 32;
         p.bits = ws.take<uint32_t>(static_cast<size_t>(SEG_LONG_CTAS) * 2 * p.words);
         p.B = B; p.U = U; p.I = I;
-        p.err = nullptr; p.users = nullptr; p.items = nullptr; p.negs = nullptr;
+        p.err = nullptr; p.users = nullptr; p.items = nullptr; p.negs = nullptr; p.ratings = nullptr;
     }
     l.st.t_g = ws.take<float>(2 * B);
     l.st.stash = ws.take<float>(static_cast<size_t>(B) * D);
@@ -1290,8 +1352,8 @@ bool v2_eligible(const slb_mf_step_args* x) {
 }
 
 int v2_launch_plan(const slb_mf_step_args* x, PlanDev p, int32_t* err, const int64_t* users, const int64_t* items,
-                   const int64_t* negs, int64_t B, cudaStream_t st) {
-    p.B = B; p.users = users; p.items = items; p.negs = negs; p.err = err;
+                   const int64_t* negs, const float* ratings, int64_t B, cudaStream_t st) {
+    p.B = B; p.users = users; p.items = items; p.negs = negs; p.ratings = ratings; p.err = err;
     p.seg.long_cap = seg_sort_cap(lpr_for_dim(x->dim));
     const int sms = slb_sms();
     int g = static_cast<int>((B + 255) / 256);
@@ -1341,6 +1403,9 @@ void v2_user_dispatch(const MfDev& a, const PlanDev& p, const StepV2& v, bool sm
     switch (a.loss) {
         case SLB_LOSS_POINTWISE: v2_user_launch<LPR, SLB_LOSS_POINTWISE>(a, p, v, small, grid, st); break;
         case SLB_LOSS_BPR: v2_user_launch<LPR, SLB_LOSS_BPR>(a, p, v, small, grid, st); break;
+        case SLB_LOSS_REGRESSION: v2_user_launch<LPR, SLB_LOSS_REGRESSION>(a, p, v, small, grid, st); break;
+        case SLB_LOSS_POISSON: v2_user_launch<LPR, SLB_LOSS_POISSON>(a, p, v, small, grid, st); break;
+        case SLB_LOSS_LOGISTIC: v2_user_launch<LPR, SLB_LOSS_LOGISTIC>(a, p, v, small, grid, st); break;
         default: v2_user_launch<LPR, SLB_LOSS_HINGE>(a, p, v, small, grid, st); break;
     }
 }
@@ -1355,14 +1420,14 @@ void v2_item_launch(const MfDev& a, const PlanDev& p, const StepV2& v, bool smal
 
 // phases: 1 plan, 2 user kernels (forward + user update), 4 item kernels
 int v2_launch_step(const slb_mf_step_args* x, const V2Layout& l, int slot, int32_t* err, const int64_t* users,
-                   const int64_t* items, const int64_t* negs, int64_t B, float* loss_out, cudaStream_t st,
-                   int phases) {
+                   const int64_t* items, const int64_t* negs, const float* ratings, int64_t B, float* loss_out,
+                   cudaStream_t st, int phases) {
     if (phases & 1) {
-        const int rc = v2_launch_plan(x, l.plan[slot], err, users, items, negs, B, st);
+        const int rc = v2_launch_plan(x, l.plan[slot], err, users, items, negs, ratings, B, st);
         if (rc != SLB_OK) return rc;
     }
     PlanDev p = l.plan[slot];
-    p.B = B; p.users = users; p.items = items; p.negs = negs; p.err = err;
+    p.B = B; p.users = users; p.items = items; p.negs = negs; p.ratings = ratings; p.err = err;
     p.seg.long_cap = seg_sort_cap(lpr_for_dim(x->dim));
     const MfDev a = v2_dev(x, B, loss_out);
     const int sms = slb_sms();
@@ -1411,13 +1476,14 @@ extern "C" {
 
 size_t slb_mf_step_workspace_bytes(int64_t batch, int32_t n_neg, int32_t loss,
                                    int64_t num_users, int64_t num_items) {
-    (void)n_neg; (void)loss;
-    return mf_layout(nullptr, batch, num_users, num_items).bytes;
+    (void)n_neg;
+    return mf_layout(nullptr, batch, num_users, num_items, is_rating_loss(loss) ? 1 : 2).bytes;
 }
 
 int64_t slb_mf_compact_rows(int64_t batch, int32_t n_neg, int32_t loss, int32_t which) {
-    (void)n_neg; (void)loss; (void)which;
-    return 2 * batch;  // positive + selected negative term per interaction
+    (void)n_neg; (void)which;
+    // rating losses: one term per interaction; otherwise positive + selected negative
+    return is_rating_loss(loss) ? batch : 2 * batch;
 }
 
 size_t slb_mf_fused_workspace_bytes(int64_t batch, int64_t num_users, int64_t num_items, int32_t dim) {
@@ -1433,10 +1499,10 @@ int slb_mf_train_step(const slb_mf_step_args* x, slb_stream_t stream) {
         if (r2 != SLB_OK) return r2;
         const V2Layout l = v2_layout(x->fused_workspace, x->batch, x->num_users, x->num_items, x->dim);
         MfLayout old = mf_layout(x->workspace, x->batch, x->num_users, x->num_items);
-        return v2_launch_step(x, l, 0, old.err, x->users, x->items, x->negs, x->batch, x->loss_out,
+        return v2_launch_step(x, l, 0, old.err, x->users, x->items, x->negs, x->ratings, x->batch, x->loss_out,
                               static_cast<cudaStream_t>(stream), 7);
     }
-    return launch_step(x, x->users, x->items, x->negs, x->batch, x->loss_out,
+    return launch_step(x, x->users, x->items, x->negs, x->ratings, x->batch, x->loss_out,
                        static_cast<cudaStream_t>(stream));
 }
 
@@ -1448,10 +1514,10 @@ int slb_mf_train_step_phases(const slb_mf_step_args* x, int32_t phases, slb_stre
         if (r2 != SLB_OK) return r2;
         const V2Layout l = v2_layout(x->fused_workspace, x->batch, x->num_users, x->num_items, x->dim);
         MfLayout old = mf_layout(x->workspace, x->batch, x->num_users, x->num_items);
-        return v2_launch_step(x, l, (phases >> 8) & 1, old.err, x->users, x->items, x->negs, x->batch, x->loss_out,
-                              static_cast<cudaStream_t>(stream), phases & 7);
+        return v2_launch_step(x, l, (phases >> 8) & 1, old.err, x->users, x->items, x->negs, x->ratings, x->batch,
+                              x->loss_out, static_cast<cudaStream_t>(stream), phases & 7);
     }
-    return launch_step(x, x->users, x->items, x->negs, x->batch, x->loss_out,
+    return launch_step(x, x->users, x->items, x->negs, x->ratings, x->batch, x->loss_out,
                        static_cast<cudaStream_t>(stream), phases);
 }
 
@@ -1501,7 +1567,8 @@ static int fit_epoch_impl(const slb_mf_step_args* x, const int64_t* users, const
                 ++next_wait;
             }
             if (two && k >= 2) cudaStreamWaitEvent(plan_st, ev_done[slot], 0);      // slot free again
-            const int r = v2_launch_plan(&tmp, l.plan[slot], old.err, users + lo, items + lo, negs + lo, B, plan_st);
+            const int r = v2_launch_plan(&tmp, l.plan[slot], old.err, users + lo, items + lo, negs ? negs + lo : nullptr,
+                                         x->ratings ? x->ratings + lo : nullptr, B, plan_st);
             if (two) cudaEventRecord(ev_plan[slot], plan_st);
             return r;
         };
@@ -1513,8 +1580,8 @@ static int fit_epoch_impl(const slb_mf_step_args* x, const int64_t* users, const
             if (k + 1 < nsteps) rc2 = plan_of(k + 1);
             if (rc2 != SLB_OK) break;
             if (two) cudaStreamWaitEvent(main_st, ev_plan[slot], 0);
-            rc2 = v2_launch_step(&tmp, l, slot, old.err, users + lo, items + lo, negs + lo, B, losses_out + k,
-                                 main_st, 6);
+            rc2 = v2_launch_step(&tmp, l, slot, old.err, users + lo, items + lo, negs ? negs + lo : nullptr,
+                                 x->ratings ? x->ratings + lo : nullptr, B, losses_out + k, main_st, 6);
             if (two) cudaEventRecord(ev_done[slot], main_st);
         }
         if (two) {
@@ -1538,8 +1605,9 @@ static int fit_epoch_impl(const slb_mf_step_args* x, const int64_t* users, const
         }
         // adaptive hinge: negatives of step k are the flat [B*n_neg] block the
         // reference's per-batch randint would have produced (implicit.py:256-259)
-        const int64_t* ng = negs + lo * x->n_neg;
-        const int r = launch_step(x, users + lo, items + lo, ng, B, losses_out + step, main_st, 0x1f, step);
+        const int64_t* ng = negs ? negs + lo * x->n_neg : nullptr;
+        const float* rt = x->ratings ? x->ratings + lo : nullptr;
+        const int r = launch_step(x, users + lo, items + lo, ng, rt, B, losses_out + step, main_st, 0x1f, step);
         if (r != SLB_OK) return r;
     }
     return SLB_OK;

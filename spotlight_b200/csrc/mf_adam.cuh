@@ -63,7 +63,7 @@ mf_adam_prepass_kernel(MfDev a, AdamDev o, float* vWu, float* vWi, float* vbu, f
     const int gib = threadIdx.x / LPR;
     const unsigned gmask = group_mask(LPR);
     const int D = a.D;
-    const int64_t nneg = a.B * a.n_neg;
+    const int64_t nneg = a.negs ? a.B * a.n_neg : 0;       // rating losses have no negatives
     const int64_t total = 2 * a.B + nneg;
     const int upto = o.t - 1;
     if (upto <= 0) return;

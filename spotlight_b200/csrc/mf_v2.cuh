@@ -24,9 +24,14 @@
 // spotlight/factorization/implicit.py:229-243 with a row-wise SGD / Adagrad optimizer.
 // Deterministic: no float atomics, every row has one writer that sums in ascending
 // interaction order.
+//
+// Rating losses (regression / poisson / logistic, spotlight/factorization/explicit.py:223-234) run
+// the same step in ONE-TERM mode: no negative, one item member per interaction with term id b
+// (instead of 2b / 2b+1), and the user record's j slot carries the rating's bits, so the user
+// kernel scores one item row per interaction with no extra dependent load.
 #pragma once
 
-struct __align__(16) URec { int32_t b, i, j, pad; };
+struct __align__(16) URec { int32_t b, i, j, pad; };     // one-term mode: j = the rating's bits
 struct __align__(8) IRec { int32_t t, useg; };
 
 struct PlanDev {
@@ -40,10 +45,11 @@ struct PlanDev {
     int32_t* err;
     int64_t B, U, I;
     const int64_t* users; const int64_t* items; const int64_t* negs;
+    const float* ratings;  // one-term mode (rating losses): [B], negs == nullptr
 };
 
 struct StepV2 {
-    float* t_g;            // [2B] d loss / d score of term t (already / B)
+    float* t_g;            // [2B] d loss / d score of term t (already / B); [B] in one-term mode
     float* stash;          // [B][D] old user rows, by user segment
     float* partial;        // [MF_MAX_GRID] loss partials of mf_user_kernel
     float* partial_long;   // [SEG_LONG_CTAS * 4] loss partials of the hot-row kernel
@@ -56,11 +62,11 @@ __global__ void __launch_bounds__(256) plan_count_kernel(PlanDev p) {
     const int64_t nth = static_cast<int64_t>(gridDim.x) * blockDim.x;
     if (blockIdx.x == 0 && threadIdx.x == 0) p.seg.totals[3] = 0;
     for (int64_t b = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x; b < p.B; b += nth) {
-        const int64_t u = p.users[b], i = p.items[b], j = p.negs[b];
+        const int64_t u = p.users[b], i = p.items[b], j = p.negs ? p.negs[b] : 0;
         if (u < 0 || u >= p.U || i < 0 || i >= p.I || j < 0 || j >= p.I) { atomicExch(p.err, 1); continue; }
         atomicAdd(p.seg.cnt + u, 1);
         atomicAdd(p.seg.cnt + p.U + i, 1);
-        atomicAdd(p.seg.cnt + p.U + j, 1);
+        if (p.negs) atomicAdd(p.seg.cnt + p.U + j, 1);
     }
 }
 
@@ -68,14 +74,20 @@ __global__ void __launch_bounds__(256) plan_fill_kernel(PlanDev p) {
     const int64_t nth = static_cast<int64_t>(gridDim.x) * blockDim.x;
     const int ubase = p.seg.seg_start[p.seg.totals[2]];     // user-side members come first
     for (int64_t b = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x; b < p.B; b += nth) {
-        const int64_t u = p.users[b], i = p.items[b], j = p.negs[b];
+        const int64_t u = p.users[b], i = p.items[b], j = p.negs ? p.negs[b] : 0;
         if (u < 0 || u >= p.U || i < 0 || i >= p.I || j < 0 || j >= p.I) continue;
         const int su = p.seg.off[u] + atomicSub(p.seg.cnt + u, 1) - 1;
         URec r;
-        r.b = static_cast<int32_t>(b); r.i = static_cast<int32_t>(i); r.j = static_cast<int32_t>(j); r.pad = 0;
+        r.b = static_cast<int32_t>(b); r.i = static_cast<int32_t>(i); r.pad = 0;
+        r.j = p.negs ? static_cast<int32_t>(j) : __float_as_int(p.ratings[b]);
         p.mu[su] = r;
         const int useg = p.seg.sid[u];
         const int si = p.seg.off[p.U + i] + atomicSub(p.seg.cnt + p.U + i, 1) - 1 - ubase;
+        if (!p.negs) {                                      // one-term mode: term b
+            IRec a; a.t = static_cast<int32_t>(b); a.useg = useg;
+            p.mi[si] = a;
+            continue;
+        }
         const int sj = p.seg.off[p.U + j] + atomicSub(p.seg.cnt + p.U + j, 1) - 1 - ubase;
         IRec a; a.t = static_cast<int32_t>(2 * b); a.useg = useg;
         IRec c; c.t = static_cast<int32_t>(2 * b + 1); c.useg = useg;
@@ -282,6 +294,25 @@ template <int LPR, int VPL, int LOSS, bool FULL>
 __device__ __forceinline__ void user_member(const RowV<VPL>& w, float ub, const RowV<VPL>& qi, const RowV<VPL>& qj,
                                             float bi_, float bj_, int b, float invB, unsigned gmask, int gl,
                                             float* t_g, RowV<VPL>& acc, float& bacc, bool& nz, float& lsum) {
+    if constexpr (LOSS >= SLB_LOSS_REGRESSION) {
+        // one-term mode: bj_ is the rating, qj is not used
+        float dp = 0.f;
+#pragma unroll
+        for (int q = 0; q < VPL; ++q) dp += dot4(w.v[q], qi.v[q]);
+        dp = group_sum<LPR>(dp, FULL ? 0xffffffffu : gmask);
+        float per, g;
+        rating_loss(LOSS, dp + ub + bi_, bj_, per, g);
+        g *= invB;
+        if (gl == 0) {
+            lsum += per;
+            t_g[b] = g;
+        }
+#pragma unroll
+        for (int q = 0; q < VPL; ++q) fma4(acc.v[q], g, qi.v[q]);
+        bacc += g;
+        nz = nz || g != 0.f;
+        return;
+    }
     float dp = 0.f, dn = 0.f;
 #pragma unroll
     for (int q = 0; q < VPL; ++q) { dp += dot4(w.v[q], qi.v[q]); dn += dot4(w.v[q], qj.v[q]); }
@@ -325,6 +356,7 @@ __global__ void __launch_bounds__(MF_TILE_THREADS, (VPL == 1 ? V2_UMINB : V2_UMI
     constexpr int D = LPR * 4 * VPL;
     constexpr int GPW = 32 / LPR;
     constexpr int WARPS = MF_TILE_THREADS / 32;
+    constexpr bool RATING = LOSS >= SLB_LOSS_REGRESSION;    // one-term mode: j carries the rating
     __shared__ float sh_red[WARPS];
     __shared__ int sh_inv[WARPS][32];
     __shared__ bool is_last;
@@ -398,8 +430,9 @@ __global__ void __launch_bounds__(MF_TILE_THREADS, (VPL == 1 ? V2_UMINB : V2_UMI
                 RowV<VPL> st_ = row_zero<VPL>();
                 if (adagrad) st_ = row_ldcs<LPR, VPL>(srow, gl);
                 const RowV<VPL> qi = row_ldg<LPR, VPL>(a.Wi + static_cast<int64_t>(i0) * D, gl);
-                const RowV<VPL> qj = row_ldg<LPR, VPL>(a.Wi + static_cast<int64_t>(j0) * D, gl);
-                const float ub = a.bu[s_row], bi_ = __ldg(a.bi + i0), bj_ = __ldg(a.bi + j0);
+                const RowV<VPL> qj = RATING ? row_zero<VPL>() : row_ldg<LPR, VPL>(a.Wi + static_cast<int64_t>(j0) * D, gl);
+                const float ub = a.bu[s_row], bi_ = __ldg(a.bi + i0);
+                const float bj_ = RATING ? __int_as_float(j0) : __ldg(a.bi + j0);
                 user_member<LPR, VPL, LOSS, true>(w, ub, qi, qj, bi_, bj_, b0, invB, gmask, gl, v.t_g, acc, bacc, nz, lsum);
                 user_finish<LPR, VPL>(a, o, stash_row, wrow, srow, w, st_, acc, bacc, nz, s_row, gl);
             } else if (q0 >= n1 && q0 + GPW <= n1 + n2) {
@@ -411,12 +444,14 @@ __global__ void __launch_bounds__(MF_TILE_THREADS, (VPL == 1 ? V2_UMINB : V2_UMI
                 RowV<VPL> st_ = row_zero<VPL>();
                 if (adagrad) st_ = row_ldcs<LPR, VPL>(srow, gl);
                 const RowV<VPL> qi0 = row_ldg<LPR, VPL>(a.Wi + static_cast<int64_t>(i0) * D, gl);
-                const RowV<VPL> qj0 = row_ldg<LPR, VPL>(a.Wi + static_cast<int64_t>(j0) * D, gl);
+                const RowV<VPL> qj0 = RATING ? row_zero<VPL>() : row_ldg<LPR, VPL>(a.Wi + static_cast<int64_t>(j0) * D, gl);
                 const float ub = a.bu[s_row];
-                const float bi0 = __ldg(a.bi + i0), bj0 = __ldg(a.bi + j0), bi1 = __ldg(a.bi + i1), bj1 = __ldg(a.bi + j1);
+                const float bi0 = __ldg(a.bi + i0), bi1 = __ldg(a.bi + i1);
+                const float bj0 = RATING ? __int_as_float(j0) : __ldg(a.bi + j0);
+                const float bj1 = RATING ? __int_as_float(j1) : __ldg(a.bi + j1);
                 user_member<LPR, VPL, LOSS, true>(w, ub, qi0, qj0, bi0, bj0, b0, invB, gmask, gl, v.t_g, acc, bacc, nz, lsum);
                 const RowV<VPL> qi1 = row_ldg<LPR, VPL>(a.Wi + static_cast<int64_t>(i1) * D, gl);
-                const RowV<VPL> qj1 = row_ldg<LPR, VPL>(a.Wi + static_cast<int64_t>(j1) * D, gl);
+                const RowV<VPL> qj1 = RATING ? row_zero<VPL>() : row_ldg<LPR, VPL>(a.Wi + static_cast<int64_t>(j1) * D, gl);
                 user_member<LPR, VPL, LOSS, true>(w, ub, qi1, qj1, bi1, bj1, b1, invB, gmask, gl, v.t_g, acc, bacc, nz, lsum);
                 user_finish<LPR, VPL>(a, o, stash_row, wrow, srow, w, st_, acc, bacc, nz, s_row, gl);
             } else {
@@ -431,8 +466,9 @@ __global__ void __launch_bounds__(MF_TILE_THREADS, (VPL == 1 ? V2_UMINB : V2_UMI
                     // every lane of the group reads the same (sorted) record: one broadcast transaction
                     const int4 r = __ldg(reinterpret_cast<const int4*>(p.mu + s_start + k));
                     const RowV<VPL> qi = row_ldg<LPR, VPL>(a.Wi + static_cast<int64_t>(r.y) * D, gl);
-                    const RowV<VPL> qj = row_ldg<LPR, VPL>(a.Wi + static_cast<int64_t>(r.z) * D, gl);
-                    user_member<LPR, VPL, LOSS, false>(w, ub, qi, qj, __ldg(a.bi + r.y), __ldg(a.bi + r.z), r.x, invB, gmask,
+                    const RowV<VPL> qj = RATING ? row_zero<VPL>() : row_ldg<LPR, VPL>(a.Wi + static_cast<int64_t>(r.z) * D, gl);
+                    const float bj_ = RATING ? __int_as_float(r.z) : __ldg(a.bi + r.z);
+                    user_member<LPR, VPL, LOSS, false>(w, ub, qi, qj, __ldg(a.bi + r.y), bj_, r.x, invB, gmask,
                                                        gl, v.t_g, acc, bacc, nz, lsum);
                 }
                 user_finish<LPR, VPL>(a, o, stash_row, wrow, srow, w, st_, acc, bacc, nz, s_row, gl);
@@ -495,7 +531,22 @@ __global__ void __launch_bounds__(256) mf_user_long_kernel(MfDev a, PlanDev p, S
         float bacc = 0.f, nzf = 0.f;
         for (int k = lo; k < hi; ++k) {
             const int4 r0 = __ldg(reinterpret_cast<const int4*>(p.mu + start + k));
-            const float4 a0 = ldg4(a.Wi + static_cast<int64_t>(r0.y) * D + c), b0 = ldg4(a.Wi + static_cast<int64_t>(r0.z) * D + c);
+            const float4 a0 = ldg4(a.Wi + static_cast<int64_t>(r0.y) * D + c);
+            if constexpr (LOSS >= SLB_LOSS_REGRESSION) {              // one-term mode: r0.z = rating bits
+                const float dp = group_sum<LPR>(dot4(w4, a0), gmask);
+                float per, g;
+                rating_loss(LOSS, dp + ub + __ldg(a.bi + r0.y), __int_as_float(r0.z), per, g);
+                g *= invB;
+                if (gl == 0) {
+                    lsum += per;
+                    v.t_g[r0.x] = g;
+                }
+                fma4(acc, g, a0);
+                bacc += g;
+                if (g != 0.f) nzf = 1.f;
+                continue;
+            }
+            const float4 b0 = ldg4(a.Wi + static_cast<int64_t>(r0.z) * D + c);
             const float dp = group_sum<LPR>(dot4(w4, a0), gmask);
             const float dn = group_sum<LPR>(dot4(w4, b0), gmask);
             float per, gp, gn;

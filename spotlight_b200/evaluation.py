@@ -245,3 +245,37 @@ def sequence_precision_recall_score(model, test, k=10, exclude_preceding=False, 
         _, pos = _rank_targets(scores, row_ptr, targets[lo:lo + n].reshape(-1), position=True)
         hits[lo:lo + n] = _hits_at(pos, row_ptr, [k], unique[lo:lo + n].reshape(-1))[:, 0]
     return hits / float(min(k, model._num_items)), hits / float(k)
+
+
+_RMSE_BLOCK = 1 << 22           # test pairs per predict + reduction launch
+
+
+def rmse_score(model, test):
+    """Root mean squared error of the model's predicted ratings on the test pairs
+    (evaluation.py:223-244).
+
+    The pairs are scored on the device in blocks through the model's prediction kernels
+    (``exp`` / ``sigmoid`` applied for poisson / logistic models, as ``predict`` does); each
+    block's mean squared error comes from the deterministic ``slb_rating_loss`` reduction and the
+    blocks are combined in float64.  Returns a NumPy float32 like the reference.
+    """
+    n = len(test.user_ids)
+    if test.ratings is None:
+        raise TypeError("unsupported operand type(s) for -: 'NoneType' and 'float'")
+    model._check_input(test.user_ids, test.item_ids)
+    dev = next(model._net.parameters()).device
+    predict_device = getattr(model, '_predict_device', None)
+    total = 0.0
+    for lo in range(0, n, _RMSE_BLOCK):
+        hi = min(n, lo + _RMSE_BLOCK)
+        users = torch.from_numpy(np.asarray(test.user_ids[lo:hi], dtype=np.int64)).to(dev)
+        items = torch.from_numpy(np.asarray(test.item_ids[lo:hi], dtype=np.int64)).to(dev)
+        ratings = torch.from_numpy(np.asarray(test.ratings[lo:hi], dtype=np.float32)).to(dev)
+        if predict_device is not None:
+            pred = predict_device(users, items)
+        else:
+            pred = torch.from_numpy(np.asarray(model.predict(test.user_ids[lo:hi], test.item_ids[lo:hi]),
+                                               dtype=np.float32)).to(dev)
+        mse, _ = ops.rating_loss(pred.reshape(-1).contiguous(), ratings, _lib.LOSS_KIND['regression'])
+        total += float(mse) * (hi - lo)
+    return np.float32(np.sqrt(total / n))

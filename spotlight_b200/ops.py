@@ -250,11 +250,14 @@ mf_scores.register_autograd(_mf_scores_bwd, setup_context=_mf_scores_setup)
 # fused training step       spotlight/factorization/implicit.py:229-242
 # ---------------------------------------------------------------------------
 
-def mf_step_args(Wu, Wi, bu, bi, users, items, negs, loss, n_neg, batch=None):
-    """A filled ``slb_mf_step_args`` (parameters + minibatch); caller adds outputs."""
+def mf_step_args(Wu, Wi, bu, bi, users, items, negs, loss, n_neg, batch=None, ratings=None):
+    """A filled ``slb_mf_step_args`` (parameters + minibatch); caller adds outputs.
+    Rating losses pass ``negs=None`` and the float32 ``ratings``."""
     a = MfStepArgs()
     a.batch = int(batch if batch is not None else users.numel())
-    a.users, a.items, a.negs = users.data_ptr(), items.data_ptr(), negs.data_ptr()
+    a.users, a.items = users.data_ptr(), items.data_ptr()
+    a.negs = negs.data_ptr() if negs is not None else None
+    a.ratings = ratings.data_ptr() if ratings is not None else None
     a.loss = LOSS_KIND[loss] if isinstance(loss, str) else int(loss)
     a.n_neg = int(n_neg)
     a.num_users, a.num_items, a.dim = Wu.shape[0], Wi.shape[0], Wu.shape[1]
@@ -306,21 +309,24 @@ def _(Wu, Wi, bu, bi, users, items, negs, loss, n_neg, want_scores):
 
 
 def mf_train_step_inplace(Wu, Wi, bu, bi, users, items, negs, loss, opt_kind, lr, states=None,
-                          weight_decay=0.0, eps=1e-10, planned=True):
+                          weight_decay=0.0, eps=1e-10, planned=True, ratings=None):
     """One minibatch with the row-wise optimizer fused in: parameters (and Adagrad ``states`` =
     (sWu, sWi, sbu, sbi)) are updated in place, the minibatch loss is returned.
 
     ``planned`` selects the two-kernel planned step (csrc/mf_v2.cuh) when the library supports
     the shape; otherwise the first-generation step with compact gradients runs.  This is the
     body of one iteration of ``slb_mf_fit_epoch`` (spotlight/factorization/implicit.py:229-243).
+    Rating losses pass ``negs=None`` and ``ratings`` (spotlight/factorization/explicit.py:223-234).
     """
-    require_cuda(Wu, Wi, bu, bi, users, items, negs)
+    require_cuda(Wu, Wi, bu, bi, users, items, negs, ratings)
     lib = _lib.load()
-    users, items, negs = _i64c(users).reshape(-1), _i64c(items).reshape(-1), _i64c(negs).reshape(-1)
+    users, items = _i64c(users).reshape(-1), _i64c(items).reshape(-1)
+    negs = _i64c(negs).reshape(-1) if negs is not None else None
+    ratings = _f32c(ratings).reshape(-1) if ratings is not None else None
     B = users.numel()
     dev = Wu.device
     with torch.no_grad():
-        a = mf_step_args(Wu, Wi, bu, bi, users, items, negs, loss, 1)
+        a = mf_step_args(Wu, Wi, bu, bi, users, items, negs, loss, 1, ratings=ratings)
         loss_out = torch.empty(1, dtype=torch.float32, device=dev)
         a.loss_out = loss_out.data_ptr()
         a.grad_mode = _lib.GRAD_COMPACT
@@ -544,6 +550,75 @@ def fused_mf_loss(Wu, Wi, bu, bi, users, items, negs, loss: str, n_neg: int = 1)
 
 
 # ---------------------------------------------------------------------------
+# explicit-feedback step     spotlight/factorization/explicit.py:223-234
+# ---------------------------------------------------------------------------
+
+@torch.library.custom_op('spotlight_b200::mf_rating_train_step', mutates_args=())
+def mf_rating_train_step(Wu: Tensor, Wi: Tensor, bu: Tensor, bi: Tensor, users: Tensor, items: Tensor,
+                         ratings: Tensor, loss: int, want_scores: bool
+                         ) -> Tuple[Tensor, Tensor, Tensor, Tensor, Tensor, Tensor]:
+    """Fused forward + backward of one rating minibatch with dense gradients.
+
+    Returns (loss, scores, dWu, dWi, dbu, dbi); ``scores`` (the raw BilinearNet output, before
+    poisson's exp / logistic's sigmoid) is empty unless ``want_scores``.
+    """
+    require_cuda(Wu, Wi, bu, bi, users, items, ratings)
+    lib = _lib.load()
+    Wu, Wi, bu, bi = _f32c(Wu), _f32c(Wi), _f32c(bu), _f32c(bi)
+    users, items = _i64c(users).reshape(-1), _i64c(items).reshape(-1)
+    ratings = _f32c(ratings).reshape(-1)
+    B = users.numel()
+    if items.numel() != B or ratings.numel() != B:
+        raise ValueError('mf_rating_train_step: inconsistent batch sizes')
+    dev = Wu.device
+    a = mf_step_args(Wu, Wi, bu, bi, users, items, None, loss, 1, ratings=ratings)
+    loss_out = torch.empty(1, dtype=torch.float32, device=dev)
+    pos = torch.empty(B if want_scores else 0, dtype=torch.float32, device=dev)
+    dWu, dWi = torch.zeros_like(Wu), torch.zeros_like(Wi)
+    dbu, dbi = torch.zeros_like(bu), torch.zeros_like(bi)
+    a.loss_out = loss_out.data_ptr()
+    if want_scores:
+        a.pos_out = pos.data_ptr()
+    a.grad_mode = _lib.GRAD_DENSE
+    a.dWu, a.dWi, a.dbu, a.dbi = dWu.data_ptr(), dWi.data_ptr(), dbu.data_ptr(), dbi.data_ptr()
+    need = lib.slb_mf_step_workspace_bytes(B, 1, a.loss, a.num_users, a.num_items)
+    ws = workspace('mf%d_%d' % (a.num_users, a.num_items), need, dev)
+    a.workspace, a.workspace_bytes = ws.data_ptr(), ws.numel()
+    _lib.check(lib.slb_mf_train_step(ctypes.byref(a), _stream()), 'mf_rating_train_step')
+    return loss_out.reshape(()), pos, dWu, dWi, dbu, dbi
+
+
+@mf_rating_train_step.register_fake
+def _(Wu, Wi, bu, bi, users, items, ratings, loss, want_scores):
+    B = users.numel()
+    return (Wu.new_empty(()), Wu.new_empty((B if want_scores else 0,)),
+            torch.empty_like(Wu), torch.empty_like(Wi), torch.empty_like(bu), torch.empty_like(bi))
+
+
+class _FusedRatingLoss(torch.autograd.Function):
+    """loss = fused rating step(...); backward hands out the gradients computed in forward."""
+
+    @staticmethod
+    def forward(ctx, Wu, Wi, bu, bi, users, items, ratings, loss):
+        out = mf_rating_train_step(Wu.detach(), Wi.detach(), bu.detach(), bi.detach(), users, items,
+                                   ratings, loss, False)
+        ctx.save_for_backward(*out[2:])
+        return out[0]
+
+    @staticmethod
+    def backward(ctx, g):
+        dWu, dWi, dbu, dbi = ctx.saved_tensors
+        return dWu * g, dWi * g, dbu * g, dbi * g, None, None, None, None
+
+
+def fused_rating_loss(Wu, Wi, bu, bi, users, items, ratings, loss: str):
+    """Scalar minibatch rating loss whose ``backward()`` fills dense ``.grad`` on the four
+    BilinearNet parameters: the body of the reference's explicit fit loop
+    (explicit.py:223-233) in one fused kernel per direction."""
+    return _FusedRatingLoss.apply(Wu, Wi, bu, bi, users, items, ratings, LOSS_KIND[loss])
+
+
+# ---------------------------------------------------------------------------
 # L1..L4 standalone losses                      spotlight/losses.py:18-166
 # ---------------------------------------------------------------------------
 
@@ -594,6 +669,52 @@ class _PairwiseLoss(torch.autograd.Function):
 
 def loss_op(kind: str, pos, neg, mask=None):
     return _PairwiseLoss.apply(pos, neg, mask, LOSS_KIND[kind])
+
+
+# ---------------------------------------------------------------------------
+# L5..L7 standalone rating losses                spotlight/losses.py:169-244
+# ---------------------------------------------------------------------------
+
+@torch.library.custom_op('spotlight_b200::rating_loss', mutates_args=())
+def rating_loss(pred: Tensor, ratings: Tensor, loss: int) -> Tuple[Tensor, Tensor]:
+    """(mean loss, d loss / d pred) of one rating loss; poisson takes the exponentiated
+    prediction, as the reference's ``poisson_loss`` does."""
+    require_cuda(pred, ratings)
+    lib = _lib.load()
+    p = _f32c(pred).reshape(-1)
+    n = p.numel()
+    r = ratings.reshape(-1).to(torch.float32).contiguous()
+    if n == 0 or r.numel() != n:
+        raise ValueError('rating_loss: bad shapes pred %s ratings %s' % (tuple(pred.shape), tuple(ratings.shape)))
+    out = torch.empty(1, dtype=torch.float32, device=pred.device)
+    g = torch.empty_like(p)
+    ws = workspace('loss', lib.slb_loss_workspace_bytes(n), pred.device)
+    rc = lib.slb_rating_loss(loss, _ptr(p), _ptr(r), n, _ptr(out), _ptr(g), _ptr(ws), ws.numel(), _stream())
+    _lib.check(rc, 'rating_loss')
+    return out.reshape(()), g.reshape(pred.shape)
+
+
+@rating_loss.register_fake
+def _(pred, ratings, loss):
+    return pred.new_empty(()), torch.empty_like(pred)
+
+
+def _rating_loss_setup(ctx, inputs, output):
+    ctx.save_for_backward(output[1])
+
+
+def _rating_loss_bwd(ctx, g_loss, g_grad):
+    (d,) = ctx.saved_tensors
+    return d * g_loss, None, None
+
+
+rating_loss.register_autograd(_rating_loss_bwd, setup_context=_rating_loss_setup)
+
+
+def rating_loss_op(kind: str, observed, predicted):
+    """Scalar mean rating loss of ``predicted`` against ``observed`` (differentiable in
+    ``predicted``)."""
+    return rating_loss(predicted, observed, LOSS_KIND[kind])[0]
 
 
 # ---------------------------------------------------------------------------

@@ -91,6 +91,19 @@ class FusedAdam(torch.optim.Optimizer):
         self._t = 0                      # optimizer steps taken (torch's state['step'])
         self._sched = None
 
+    # torch.optim.Optimizer pickles only defaults / state / param_groups: keep the step count so
+    # that a pickled model resumes fit() with the right bias corrections
+    def __getstate__(self):
+        st = super(FusedAdam, self).__getstate__()
+        st['_t'] = self._t
+        return st
+
+    def __setstate__(self, state):
+        state = dict(state)
+        self._t = state.pop('_t', 0)
+        self._sched = None
+        super(FusedAdam, self).__setstate__(state)
+
     # ---- state ----------------------------------------------------------------
     def fused_hparams(self):
         g = self.param_groups[0]
