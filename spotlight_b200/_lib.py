@@ -97,6 +97,7 @@ class SeqStepArgs(ctypes.Structure):
         ('state_E', c_vp), ('state_bias', c_vp),
         ('lstm_w_ih', c_vp), ('lstm_w_hh', c_vp), ('lstm_b_ih', c_vp), ('lstm_b_hh', c_vp),
         ('dlstm_w_ih', c_vp), ('dlstm_w_hh', c_vp), ('dlstm_b_ih', c_vp), ('dlstm_b_hh', c_vp),
+        ('num_mixtures', c_i32), ('mix_w', c_vp), ('mix_b', c_vp), ('dmix_w', c_vp), ('dmix_b', c_vp),
     ]
 
 

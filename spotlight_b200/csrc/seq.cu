@@ -25,6 +25,8 @@
 //   seq_fill / seq_reduce  deterministic segmented scatter into dE, dbias
 //   lstm_fwd / lstm_bwd  LSTMNet recurrence and its BPTT on thread-block clusters (seq_lstm.cuh);
 //                        the LSTM's projections and weight gradients are k = 1 conv GEMMs
+//   mix_score_kernel     MixtureLSTMNet head (seq_mix.cuh): softmax-weighted taste scores and their
+//                        gradients into the 2M projection blocks; the projection is 2M k = 1 conv GEMMs
 #include <stdlib.h>
 
 #include "segindex.cuh"
@@ -54,6 +56,9 @@ struct SeqDev {
     // fused row-wise optimizer (0 = gradients written to dE / dbias)
     int32_t opt; float lr, wd, eps; float* sE; float* sbias;
     SegIndex seg;
+    // MixtureLSTMNet head: M mixtures, P = 2M blocks of (B, T, D) (components, then mixture
+    // vectors); mix_score_kernel overwrites P with d loss / d P
+    int M; float* P;
 };
 
 // ---------------------------------------------------------------- mask count
@@ -269,10 +274,31 @@ __device__ __forceinline__ void seq_pair_loss(int loss, float p, float n, float&
     }
 }
 
-template <int LPR>
-__global__ void __launch_bounds__(SQ_THREADS) seq_score_kernel(SeqDev a) {
+// Masked loss of the step: every block writes its partial sum, the last block to finish folds the
+// partials in a fixed order (no float atomics) and writes the mean over msum positions.
+__device__ __forceinline__ void seq_loss_fold(const SeqDev& a, float lsum, float msum) {
     __shared__ float sh_red[SQ_THREADS / 32];
     __shared__ bool is_last;
+    const float bsum = block_sum<SQ_THREADS>(lsum, sh_red);
+    if (threadIdx.x == 0) {
+        a.partial[blockIdx.x] = bsum;
+        __threadfence();
+        is_last = atomicAdd(a.hdr, 1) == static_cast<int>(gridDim.x) - 1;
+    }
+    __syncthreads();
+    if (is_last && threadIdx.x < 32) {
+        __threadfence();
+        float v = 0.f;
+        for (int k = threadIdx.x; k < static_cast<int>(gridDim.x); k += 32)
+            v += *reinterpret_cast<volatile float*>(a.partial + k);
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) v += __shfl_down_sync(0xffffffffu, v, o);
+        if (threadIdx.x == 0) *a.loss_out = v / msum;
+    }
+}
+
+template <int LPR>
+__global__ void __launch_bounds__(SQ_THREADS) seq_score_kernel(SeqDev a) {
     constexpr int GROUPS = SQ_THREADS / LPR;
     const int gl = threadIdx.x & (LPR - 1);
     const unsigned gmask = group_mask(LPR);
@@ -341,22 +367,7 @@ __global__ void __launch_bounds__(SQ_THREADS) seq_score_kernel(SeqDev a) {
             if (kn) atomicAdd(a.seg.cnt + nid, 1);
         }
     }
-    const float bsum = block_sum<SQ_THREADS>(lsum, sh_red);
-    if (threadIdx.x == 0) {
-        a.partial[blockIdx.x] = bsum;
-        __threadfence();
-        is_last = atomicAdd(a.hdr, 1) == static_cast<int>(gridDim.x) - 1;
-    }
-    __syncthreads();
-    if (is_last && threadIdx.x < 32) {
-        __threadfence();
-        float v = 0.f;
-        for (int k = threadIdx.x; k < static_cast<int>(gridDim.x); k += 32)
-            v += *reinterpret_cast<volatile float*>(a.partial + k);
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) v += __shfl_down_sync(0xffffffffu, v, o);
-        if (threadIdx.x == 0) *a.loss_out = v / msum;
-    }
+    seq_loss_fold(a, lsum, msum);
 }
 
 __global__ void __launch_bounds__(256) seq_fill_kernel(SeqDev a) {
@@ -460,8 +471,8 @@ struct ConvGemm {
     int k; int shift[16];
     int64_t B; int D;
     int mode;                     // 0 forward, 1 input gradient
-    // forward epilogue
-    const float* bias; int nonlin; float* Aout;     // activation (pre-residual)
+    // forward epilogue; nonlin 0 tanh, 1 relu, 2 identity (a bias-only projection)
+    const float* bias; int nonlin; float* Aout;     // activation (pre-residual), nullable
     const float* Res; int res_T; int res_shift;     // Res[b, t + res_shift] added when in range
     // input-gradient epilogue: Out = acc + Res[...]; accumulate != 0 -> Out += ...
     int accumulate;
@@ -511,6 +522,10 @@ __device__ __forceinline__ void warp_mma_chunk(const float (*As)[TS], const floa
             mma_tf32(acc[ns], ah, bh);
         }
     }
+}
+
+__device__ __forceinline__ float conv_act(float v, int nonlin) {
+    return nonlin == 0 ? tanhf(v) : (nonlin == 1 ? fmaxf(v, 0.f) : v);
 }
 
 __global__ void __launch_bounds__(256) conv_gemm_kernel(ConvGemm g) {
@@ -567,10 +582,9 @@ __global__ void __launch_bounds__(256) conv_gemm_kernel(ConvGemm g) {
             if (resok) res = *reinterpret_cast<const float2*>(g.Res + (b * g.res_T + rt) * D + n);
             if (g.mode == 0) {
                 const float2 bb = *reinterpret_cast<const float2*>(g.bias + n);
-                v0 += bb.x; v1 += bb.y;
-                v0 = g.nonlin == 0 ? tanhf(v0) : fmaxf(v0, 0.f);
-                v1 = g.nonlin == 0 ? tanhf(v1) : fmaxf(v1, 0.f);
-                *reinterpret_cast<float2*>(g.Aout + m * D + n) = make_float2(v0, v1);
+                v0 = conv_act(v0 + bb.x, g.nonlin);
+                v1 = conv_act(v1 + bb.y, g.nonlin);
+                if (g.Aout) *reinterpret_cast<float2*>(g.Aout + m * D + n) = make_float2(v0, v1);
             }
             float2 o = make_float2(v0 + res.x, v1 + res.y);
             if (g.accumulate) {
@@ -615,6 +629,7 @@ struct ConvDw {
 }  // namespace
 #include "seq_tc.cuh"
 #include "seq_lstm.cuh"
+#include "seq_mix.cuh"
 namespace {
 
 __global__ void __launch_bounds__(256) conv_dw_kernel(ConvDw g) {
@@ -732,6 +747,8 @@ struct SeqLayout {
     float* C; int32_t* keys; float* gs;
     float* part; float* bpart; int splits; int64_t slab;
     float* G; float* Cs; float* WT;      // LSTM: (4,B,T,D) gates, (B,T,D) cells, 4 x (D,D) W_ih^T blocks
+    float* P; float* WTm;                // mixture: (2M,B,T,D) projection (d loss / d P in training),
+                                         // 2M x (D,D) transposed projection blocks
     size_t bytes;
 };
 
@@ -781,7 +798,12 @@ SeqLayout seq_layout(void* base, const slb_seq_step_args* x, bool training) {
         l.G = ws.take<float>(4 * B * T * D);
         l.Cs = ws.take<float>(B * T * D);
         l.WT = ws.take<float>(4 * D * D);
-        if (training) {
+        if (x->mix_w) {
+            const int64_t J = 2 * static_cast<int64_t>(x->num_mixtures);
+            l.P = ws.take<float>(J * B * T * D);
+            l.WTm = ws.take<float>(J * D * D);
+        }
+        if (training) {                                  // k = 1 weight gradients over B * T positions
             l.splits = use_tc(static_cast<int>(D)) ? dw_splits_tc(B * T, 1) : dw_splits(B * T, static_cast<int>(D), 1);
             l.part = ws.take<float>(static_cast<size_t>(l.splits) * D * D);
             l.bpart = ws.take<float>(static_cast<size_t>(l.splits) * D);
@@ -846,6 +868,13 @@ int seq_validate(const slb_seq_step_args* x, bool training) {
         SLB_REQUIRE(x->lstm_w_hh && x->lstm_b_ih && x->lstm_b_hh, "seq: LSTM parameters missing");
         if (training)
             SLB_REQUIRE(x->dlstm_w_ih && x->dlstm_w_hh && x->dlstm_b_ih && x->dlstm_b_hh, "seq: LSTM grads missing");
+    }
+    if (x->mix_w) {
+        SLB_REQUIRE(x->lstm_w_ih != nullptr, "seq: the mixture head needs the LSTM parameters");
+        SLB_REQUIRE(x->num_mixtures >= 1 && x->num_mixtures <= mix::MAX_M,
+                    "seq: num_mixtures must be in [1, %d] (got %d)", mix::MAX_M, x->num_mixtures);
+        SLB_REQUIRE(x->mix_b != nullptr, "seq: mixture projection bias missing");
+        if (training) SLB_REQUIRE(x->dmix_w && x->dmix_b, "seq: mixture projection grads missing");
     }
     if (training) {
         SLB_REQUIRE(x->negs && x->bias && x->loss_out, "seq: null pointer");
@@ -1045,11 +1074,62 @@ int run_lstm_backward(const slb_seq_step_args* x, const SeqLayout& l, cudaStream
     return SLB_OK;
 }
 
+// ------------------------------------------------------------------ MixtureLSTMNet host side
+// P_j = W_p[j] h + b_p[j] for the 2M projection blocks (representations.py:549-553): shift-0
+// k = 1 conv GEMMs over the LSTM's h_t with the identity epilogue.
+int run_mix_forward(const slb_seq_step_args* x, const SeqLayout& l, cudaStream_t st) {
+    const int64_t B = x->batch;
+    const int T = x->seq_len + 1, D = x->dim;
+    const int64_t BTD = B * T * D, DD = static_cast<int64_t>(D) * D;
+    for (int j = 0; j < 2 * x->num_mixtures; ++j) {
+        conv_wt_kernel<<<sq_grid((DD + 255) / 256), 256, 0, st>>>(x->mix_w + j * DD, 1, D, l.WTm + j * DD, nullptr);
+        SLB_LAUNCH_CHECK("conv_wt_kernel(mixture)");
+        ConvGemm p = {};
+        p.In = l.rep_pool; p.Tin = T; p.Out = l.P + j * BTD; p.Tout = T; p.k = 1; p.shift[0] = 0;
+        p.B = B; p.D = D; p.mode = 0; p.bias = x->mix_b + j * D; p.nonlin = 2;
+        const int rc = launch_conv_gemm(p, x->mix_w + j * DD, l.WTm + j * DD, st, "conv_gemm(mixture projection)");
+        if (rc != SLB_OK) return rc;
+    }
+    return SLB_OK;
+}
+
+// From dP (in place of P): per block dW_p[j], db_p[j] and dh = sum_j W_p[j]^T dP_j into dR,
+// accumulated in block order.
+int run_mix_backward(const slb_seq_step_args* x, const SeqLayout& l, cudaStream_t st) {
+    const int64_t B = x->batch;
+    const int T = x->seq_len + 1, D = x->dim;
+    const int64_t BTD = B * T * D, DD = static_cast<int64_t>(D) * D;
+    for (int j = 0; j < 2 * x->num_mixtures; ++j) {
+        ConvDw w = {};
+        w.In = l.rep_pool; w.Tin = T; w.dZ = l.P + j * BTD; w.Tout = T; w.k = 1; w.shift[0] = 0;
+        w.B = B; w.D = D; w.part = l.part; w.bpart = l.bpart;
+        int rc = launch_conv_dw(w, x->dmix_w + j * DD, x->dmix_b + j * D, st);
+        if (rc != SLB_OK) return rc;
+        ConvGemm d = {};
+        d.In = l.P + j * BTD; d.Tin = T; d.Out = l.dR; d.Tout = T; d.k = 1; d.shift[0] = 0;
+        d.B = B; d.D = D; d.mode = 1; d.accumulate = j > 0;
+        rc = launch_conv_gemm(d, l.WTm + j * DD, x->mix_w + j * DD, st, "conv_gemm(mixture dh)");
+        if (rc != SLB_OK) return rc;
+    }
+    return SLB_OK;
+}
+
 // representation forward; returns pointer to the (B,T,D) result inside the workspace
 int run_representation(const slb_seq_step_args* x, const SeqLayout& l, float* rep_dst, cudaStream_t st,
                        float** rep_out) {
     const int64_t B = x->batch;
     const int S = x->seq_len, T = S + 1, D = x->dim;
+    if (x->lstm_w_ih && x->mix_w) {
+        int rc = run_lstm_forward(x, l, l.rep_pool, st);     // h_t stays for the projection's backward
+        if (rc == SLB_OK) rc = run_mix_forward(x, l, st);
+        if (rc == SLB_OK && rep_dst) {
+            const int J = 2 * x->num_mixtures;
+            mix::mix_rep_kernel<<<sq_grid((B * T * J * D / 4 + 255) / 256), 256, 0, st>>>(l.P, B * T, D, J, rep_dst);
+            SLB_LAUNCH_CHECK("mix_rep_kernel");
+        }
+        *rep_out = l.rep_pool;
+        return rc;
+    }
     if (x->lstm_w_ih) {
         float* H = rep_dst ? rep_dst : l.rep_pool;
         const int rc = run_lstm_forward(x, l, H, st);
@@ -1100,6 +1180,7 @@ extern "C" {
 size_t slb_seq_step_workspace_bytes(const slb_seq_step_args* x) {
     if (!x || x->batch <= 0 || x->seq_len <= 0 || x->dim <= 0) return 0;
     if (x->n_layers > 0 && !x->kernel_width) return 0;
+    if (x->mix_w && (x->num_mixtures < 1 || x->num_mixtures > mix::MAX_M)) return 0;
     return seq_layout(nullptr, x, x->negs != nullptr || x->loss_out != nullptr).bytes;
 }
 
@@ -1145,8 +1226,16 @@ int slb_seq_train_step(const slb_seq_step_args* x, slb_stream_t stream) {
     a.loss_out = x->loss_out; a.pos_out = x->pos_out; a.neg_out = x->neg_out;
     a.dE = x->dE; a.dbias = x->dbias; a.seg = l.seg;
     a.opt = x->opt; a.lr = x->lr; a.wd = x->weight_decay; a.eps = x->eps; a.sE = x->state_E; a.sbias = x->state_bias;
-    SQ_DISPATCH_LPR(lpr, seq_score_kernel, sq_grid((B * T + groups - 1) / groups), st, a);
-    SLB_LAUNCH_CHECK("seq_score_kernel");
+    if (x->mix_w) {
+        a.M = x->num_mixtures; a.P = l.P;
+        SQ_DISPATCH_LPR(lpr, mix::mix_score_kernel, sq_grid((B * T + groups - 1) / groups), st, a);
+        SLB_LAUNCH_CHECK("mix_score_kernel");
+        rc = run_mix_backward(x, l, st);
+        if (rc != SLB_OK) return rc;
+    } else {
+        SQ_DISPATCH_LPR(lpr, seq_score_kernel, sq_grid((B * T + groups - 1) / groups), st, a);
+        SLB_LAUNCH_CHECK("seq_score_kernel");
+    }
 
     if (x->lstm_w_ih) {
         rc = run_lstm_backward(x, l, st);

@@ -178,10 +178,9 @@ __global__ void __launch_bounds__(128) tc_conv_gemm_kernel(ConvGemm g) {
                 if (resok) res = *reinterpret_cast<const float2*>(g.Res + (b * g.res_T + rt) * D + n);
                 if (g.mode == 0) {
                     const float2 bb = *reinterpret_cast<const float2*>(g.bias + n);
-                    v0 += bb.x; v1 += bb.y;
-                    v0 = g.nonlin == 0 ? tanhf(v0) : fmaxf(v0, 0.f);
-                    v1 = g.nonlin == 0 ? tanhf(v1) : fmaxf(v1, 0.f);
-                    *reinterpret_cast<float2*>(g.Aout + m * D + n) = make_float2(v0, v1);
+                    v0 = conv_act(v0 + bb.x, g.nonlin);
+                    v1 = conv_act(v1 + bb.y, g.nonlin);
+                    if (g.Aout) *reinterpret_cast<float2*>(g.Aout + m * D + n) = make_float2(v0, v1);
                 }
                 float2 o = make_float2(v0 + res.x, v1 + res.y);
                 if (g.accumulate) {

@@ -738,9 +738,10 @@ class _HostPtrArray(object):
         return ctypes.cast(arr, ctypes.c_void_p)
 
 
-def seq_step_args(E, bias, seqs, negs, loss, n_neg, cnn=None, keep=None, lstm=None):
+def seq_step_args(E, bias, seqs, negs, loss, n_neg, cnn=None, keep=None, lstm=None, mixture=None):
     """cnn: None (PoolNet) or dict(kernel_width, dilation, nonlinearity, residual, weights, biases);
-    lstm: None or dict(w_ih, w_hh, b_ih, b_hh) (LSTMNet, nn.LSTM shapes)."""
+    lstm: None or dict(w_ih, w_hh, b_ih, b_hh) (LSTMNet, nn.LSTM shapes);
+    mixture: None or dict(num_mixtures, w, b) (MixtureLSTMNet's projection, with ``lstm``)."""
     keep = keep if keep is not None else _HostPtrArray()
     a = SeqStepArgs()
     a.batch, a.seq_len = int(seqs.shape[0]), int(seqs.shape[1])
@@ -761,6 +762,9 @@ def seq_step_args(E, bias, seqs, negs, loss, n_neg, cnn=None, keep=None, lstm=No
     if lstm is not None:
         a.lstm_w_ih, a.lstm_w_hh = lstm['w_ih'].data_ptr(), lstm['w_hh'].data_ptr()
         a.lstm_b_ih, a.lstm_b_hh = lstm['b_ih'].data_ptr(), lstm['b_hh'].data_ptr()
+    if mixture is not None:
+        a.num_mixtures = int(mixture['num_mixtures'])
+        a.mix_w, a.mix_b = mixture['w'].data_ptr(), mixture['b'].data_ptr()
     return a, keep
 
 
@@ -774,15 +778,32 @@ def _lstm_params(lstm):
     return {k: _f32c(lstm[k]) for k in _LSTM_KEYS}
 
 
+def _mixture_params(mixture, lstm, D):
+    """The Conv1d projection (2MD, D, 1) / (2MD,) as contiguous (2MD, D) / (2MD,) float32."""
+    if mixture is None:
+        return None
+    if lstm is None:
+        raise ValueError('mixture= needs lstm=: the mixture head sits on the LSTM representation')
+    require_cuda(mixture['w'], mixture['b'])
+    M = int(mixture['num_mixtures'])
+    w = _f32c(mixture['w'])
+    if w.numel() != 2 * M * D * D or w.shape[0] != 2 * M * D or mixture['b'].numel() != 2 * M * D:
+        raise ValueError('mixture: projection of shape %s / %s does not map %d channels to 2 * %d * %d'
+                         % (tuple(w.shape), tuple(mixture['b'].shape), D, M, D))
+    return dict(num_mixtures=M, w=w.reshape(w.shape[0], -1), b=_f32c(mixture['b']))
+
+
 def seq_train_step(E, bias, seqs, negs, loss, n_neg, cnn=None, want_scores=False, norm_count=None, fused=None,
-                   lstm=None):
+                   lstm=None, mixture=None):
     """Fused forward + backward of one sequence minibatch, dense gradients.
 
     Returns dict(loss, pos, neg, dE, dbias, dconv_w, dconv_b, dlstm).  ``fused`` = dict(kind, lr,
     weight_decay, eps, state_E, state_bias): the row-wise optimizer is applied to ``E`` / ``bias`` in
     place inside the step (no dense item-table gradient exists; ``dE`` / ``dbias`` are None).
     ``lstm`` = dict(w_ih, w_hh, b_ih, b_hh) selects the LSTMNet representation; ``dlstm`` then holds
-    the gradients under the same keys.
+    the gradients under the same keys.  ``mixture`` = dict(num_mixtures, w (2MD, D, 1), b (2MD,)), with
+    ``lstm``, adds MixtureLSTMNet's projection and mixture-of-tastes scoring; ``dmix`` = dict(w, b)
+    then holds the projection gradients in the shapes given.
     """
     require_cuda(E, bias, seqs, negs)
     lib = _lib.load()
@@ -795,9 +816,10 @@ def seq_train_step(E, bias, seqs, negs, loss, n_neg, cnn=None, want_scores=False
         cnn['weights'] = [_f32c(w) for w in cnn['weights']]
         cnn['biases'] = [_f32c(b) for b in cnn['biases']]
     lstm = _lstm_params(lstm)
-    a, keep = seq_step_args(E, bias, seqs, negs, loss, n_neg, cnn, lstm=lstm)
+    mix = _mixture_params(mixture, lstm, int(E.shape[1]))
+    a, keep = seq_step_args(E, bias, seqs, negs, loss, n_neg, cnn, lstm=lstm, mixture=mix)
     out = dict(loss=torch.empty(1, dtype=torch.float32, device=dev), dE=None, dbias=None, dconv_w=[], dconv_b=[],
-               dlstm=None)
+               dlstm=None, dmix=None)
     if fused is None:
         out['dE'], out['dbias'] = torch.zeros_like(E), torch.zeros_like(bias)
     a.loss_out = out['loss'].data_ptr()
@@ -822,6 +844,10 @@ def seq_train_step(E, bias, seqs, negs, loss, n_neg, cnn=None, want_scores=False
         out['dlstm'] = {k: torch.zeros_like(lstm[k]) for k in _LSTM_KEYS}
         a.dlstm_w_ih, a.dlstm_w_hh = out['dlstm']['w_ih'].data_ptr(), out['dlstm']['w_hh'].data_ptr()
         a.dlstm_b_ih, a.dlstm_b_hh = out['dlstm']['b_ih'].data_ptr(), out['dlstm']['b_hh'].data_ptr()
+    if mix is not None:
+        out['dmix'] = dict(w=torch.zeros(mixture['w'].shape, dtype=torch.float32, device=dev),
+                           b=torch.zeros_like(mix['b']))
+        a.dmix_w, a.dmix_b = out['dmix']['w'].data_ptr(), out['dmix']['b'].data_ptr()
     need = lib.slb_seq_step_workspace_bytes(ctypes.byref(a))
     ws = workspace('seq%d' % a.num_items, need, dev)
     a.workspace, a.workspace_bytes = ws.data_ptr(), ws.numel()
@@ -830,8 +856,9 @@ def seq_train_step(E, bias, seqs, negs, loss, n_neg, cnn=None, want_scores=False
     return out
 
 
-def seq_representation(E, seqs, cnn=None, lstm=None):
-    """(B, S+1, D) causal representations: entry t has seen items < t."""
+def seq_representation(E, seqs, cnn=None, lstm=None, mixture=None):
+    """(B, S+1, D) causal representations: entry t has seen items < t.  With ``mixture`` (see
+    seq_train_step) the projection output, (B, S+1, 2MD), channel j*D + d of block j."""
     require_cuda(E, seqs)
     lib = _lib.load()
     E = _f32c(E)
@@ -842,9 +869,11 @@ def seq_representation(E, seqs, cnn=None, lstm=None):
         cnn['weights'] = [_f32c(w) for w in cnn['weights']]
         cnn['biases'] = [_f32c(b) for b in cnn['biases']]
     lstm = _lstm_params(lstm)
+    mix = _mixture_params(mixture, lstm, int(E.shape[1]))
     dummy_bias = torch.zeros(1, dtype=torch.float32, device=E.device)
-    a, keep = seq_step_args(E, dummy_bias, seqs, None, 0, 1, cnn, lstm=lstm)
-    rep = torch.empty((B, S + 1, E.shape[1]), dtype=torch.float32, device=E.device)
+    a, keep = seq_step_args(E, dummy_bias, seqs, None, 0, 1, cnn, lstm=lstm, mixture=mix)
+    width = E.shape[1] * (2 * mix['num_mixtures'] if mix is not None else 1)
+    rep = torch.empty((B, S + 1, width), dtype=torch.float32, device=E.device)
     need = lib.slb_seq_step_workspace_bytes(ctypes.byref(a))
     ws = workspace('seq%d' % a.num_items, need, E.device)
     a.workspace, a.workspace_bytes = ws.data_ptr(), ws.numel()

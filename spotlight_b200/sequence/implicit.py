@@ -3,12 +3,13 @@
 ``fit(interactions, verbose)``, ``predict(sequences, item_ids=None)``.
 
 ``fit`` routes
-  fused    PoolNet / CNNNet / LSTMNet (D <= 256) on a plain ``ScaledEmbedding(padding_idx=0)``: one C
+  fused    PoolNet / CNNNet / LSTMNet (D <= 256) / MixtureLSTMNet (D <= 256, at most 8
+           mixtures) on a plain ``ScaledEmbedding(padding_idx=0)``: one C
            call per minibatch runs representation, scoring, masked loss and the
            whole backward (deterministic segmented scatter into the embedding
            gradient); the gradients are handed to whatever ``torch.optim``
            optimizer the model holds.
-  generic  any other representation (mixture, Bloom-embedded, custom): the
+  generic  any other representation (Bloom-embedded, custom): the
            reference's loop shape over this package's gather and loss ops.
 """
 
@@ -107,7 +108,7 @@ class ImplicitSequenceModel(object):
 
     def _route(self):
         net = self._net
-        if isinstance(net, (PoolNet, CNNNet, LSTMNet)) and net.fusable() and not self._sparse:
+        if isinstance(net, (PoolNet, CNNNet, LSTMNet, MixtureLSTMNet)) and net.fusable() and not self._sparse:
             return 'fused'
         return 'generic'
 
@@ -174,6 +175,7 @@ class ImplicitSequenceModel(object):
         net = self._net
         spec = net._cnn_spec()
         lstm = net._lstm_spec()
+        mixture = net._mixture_spec()
         fused = None
         opt = self._optimizer
         kind = getattr(opt, 'fused_kind', None)
@@ -188,7 +190,7 @@ class ImplicitSequenceModel(object):
         with torch.no_grad():
             out = ops.seq_train_step(net.item_embeddings.weight, net.item_biases.weight,
                                      batch_sequence, batch_neg, self._loss, n_neg, spec, fused=fused,
-                                     lstm=lstm)
+                                     lstm=lstm, mixture=mixture)
         net.item_embeddings.weight.grad = out['dE']
         net.item_biases.weight.grad = out['dbias']
         if spec is not None:
@@ -199,6 +201,9 @@ class ImplicitSequenceModel(object):
             g = out['dlstm']
             net.lstm.weight_ih_l0.grad, net.lstm.weight_hh_l0.grad = g['w_ih'], g['w_hh']
             net.lstm.bias_ih_l0.grad, net.lstm.bias_hh_l0.grad = g['b_ih'], g['b_hh']
+        if mixture is not None:
+            net.projection.weight.grad = out['dmix']['w']
+            net.projection.bias.grad = out['dmix']['b']
         return out['loss']
 
     def _generic_step(self, batch_sequence, batch_neg, n_neg):

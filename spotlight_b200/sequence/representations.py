@@ -1,13 +1,11 @@
 """Sequence representations with the reference's classes, constructor
 arguments and parameter names (spotlight/sequence/representations.py:27-596).
 
-``PoolNet``, ``CNNNet`` and ``LSTMNet`` run on the kernels of csrc/seq.cu; all
-keep the reference's module protocol -- ``user_representation(item_sequences) ->
-(all_steps (B, D, S), final (B, D))`` and ``forward(user_representations,
-targets) -> (B, S)`` -- so they also work with external training loops and the
-reference's evaluation code.  ``MixtureLSTMNet`` is outside the accelerated path
-and is provided as stock ``torch.nn`` modules on top of this package's embedding
-layers so ``representation='mixture'`` still constructs.
+``PoolNet``, ``CNNNet``, ``LSTMNet`` and ``MixtureLSTMNet`` run on the kernels of
+csrc/seq.cu; all keep the reference's module protocol -- ``user_representation(item_sequences)
+-> (all_steps (B, D, S), final (B, D))`` (``MixtureLSTMNet``: ``(B, 2M, D, S)``, ``(B, 2M, D,
+1)``) and ``forward(user_representations, targets) -> (B, S)`` -- so they also work with
+external training loops and the reference's evaluation code.
 """
 
 import torch
@@ -36,6 +34,9 @@ class _SeqNetBase(nn.Module):
         return None
 
     def _lstm_spec(self):
+        return None
+
+    def _mixture_spec(self):
         return None
 
     def _autograd_params(self):
@@ -194,9 +195,20 @@ class LSTMNet(_SeqNetBase):
                     b_ih=self.lstm.bias_ih_l0.detach(), b_hh=self.lstm.bias_hh_l0.detach())
 
 
-class MixtureLSTMNet(nn.Module):
-    """Mixture-of-tastes LSTM (representations.py:456-596).  Stock torch ops;
-    not on the accelerated path."""
+class MixtureLSTMNet(_SeqNetBase):
+    """Mixture-of-tastes LSTM (representations.py:456-596).
+
+    Parameters: ``LSTMNet``'s plus ``projection.weight (2MD, D, 1)`` and ``projection.bias (2MD,)``,
+    the reference's ``nn.Conv1d``, so ``state_dict``s interchange.  ``user_representation`` returns
+    the reference's ``(B, 2M, D, S)`` and ``(B, 2M, D, 1)``: blocks 0..M-1 are the taste components,
+    M..2M-1 the mixture vectors.  On a plain item table with ``D <= 256`` and ``1 <= M <= 8`` it
+    runs on the LSTM kernels and the projection GEMMs of csrc/seq.cu; otherwise, and whenever
+    autograd needs the representation, ``nn.LSTM`` and ``nn.Conv1d`` compute it.  ``forward`` is
+    the reference's softmax head in torch ops (the fused training step has its own kernel).
+    """
+
+    LSTM_MAX_DIM = 256
+    MAX_MIXTURES = 8
 
     def __init__(self, num_items, embedding_dim=32, num_mixtures=4, item_embedding_layer=None,
                  sparse=False):
@@ -212,9 +224,37 @@ class MixtureLSTMNet(nn.Module):
                                     kernel_size=1)
 
     def fusable(self):
-        return False
+        p = self.projection
+        return (super(MixtureLSTMNet, self).fusable()
+                and self.item_embeddings.embedding_dim <= self.LSTM_MAX_DIM
+                and 1 <= self.num_mixtures <= self.MAX_MIXTURES
+                and self.lstm.num_layers == 1 and self.lstm.bias and not self.lstm.bidirectional
+                and type(p) is nn.Conv1d and p.bias is not None and p.kernel_size == (1,)
+                and p.groups == 1 and p.stride == (1,) and p.padding == (0,) and p.dilation == (1,))
+
+    def _autograd_params(self):
+        return ((self.item_embeddings.weight,) + tuple(self.lstm.parameters())
+                + tuple(self.projection.parameters()))
+
+    def _lstm_spec(self):
+        return dict(w_ih=self.lstm.weight_ih_l0.detach(), w_hh=self.lstm.weight_hh_l0.detach(),
+                    b_ih=self.lstm.bias_ih_l0.detach(), b_hh=self.lstm.bias_hh_l0.detach())
+
+    def _mixture_spec(self):
+        return dict(num_mixtures=int(self.num_mixtures), w=self.projection.weight.detach(),
+                    b=self.projection.bias.detach())
 
     def user_representation(self, item_sequences):
+        if not self.fusable() or (torch.is_grad_enabled()
+                                  and any(p.requires_grad for p in self._autograd_params())):
+            return self._user_representation_autograd(item_sequences)
+        rep = ops.seq_representation(self.item_embeddings.weight.detach(), item_sequences, None,
+                                     lstm=self._lstm_spec(), mixture=self._mixture_spec())
+        B, T = rep.shape[0], rep.shape[1]
+        rep = rep.view(B, T, 2 * self.num_mixtures, self.embedding_dim).permute(0, 2, 3, 1)
+        return rep[:, :, :, :-1], rep[:, :, :, -1:]
+
+    def _user_representation_autograd(self, item_sequences):
         batch_size, sequence_length = item_sequences.size()
         emb = self.item_embeddings(item_sequences).permute(0, 2, 1).unsqueeze(3)
         emb = F.pad(emb, (0, 0, 1, 0)).squeeze(3).permute(0, 2, 1)
