@@ -90,12 +90,19 @@ def apply_rowwise(params, grads, touched, opt, lr, weight_decay=0.0, eps=1e-10, 
     """The fused row-wise optimizer (spotlight_b200.optim.FusedSGD / FusedAdagrad): the rows in
     ``touched`` (a boolean mask per table; rows with a non-zero score-gradient term) take
     torch.optim's SGD / Adagrad step with ``g + weight_decay * w``; other rows stay.  ``params``,
-    ``grads``, ``touched`` and ``states`` are (Wu, Wi, bu, bi)-ordered; updated in place."""
+    ``grads``, ``touched``, ``states`` and a per-table ``weight_decay`` tuple are (Wu, Wi, bu,
+    bi)-ordered; updated in place.  The mutation ``adagrad_div_before_add`` divides by the state
+    before adding ``g^2`` to it."""
+    wds = tuple(weight_decay) if np.ndim(weight_decay) else (weight_decay,) * 4
     for k, (w, g, rows) in enumerate(zip(params, grads, touched)):
-        wd = 0.0 if ('no_decay_items' in mutate and k in (1, 3)) else weight_decay
+        wd = 0.0 if ('no_decay_items' in mutate and k in (1, 3)) else wds[k]
         gg = g[rows] + wd * w[rows]
         if opt == 'sgd':
             w[rows] -= lr * gg
+        elif 'adagrad_div_before_add' in mutate:
+            st = states[k]
+            w[rows] -= lr * gg / (np.sqrt(st[rows]) + eps)
+            st[rows] += gg * gg
         else:
             st = states[k]
             st[rows] += gg * gg

@@ -14,9 +14,28 @@ TEST INFRASTRUCTURE ONLY.  Restates, in NumPy:
 ``dtype`` selects the arithmetic (float32 mimics the reference, float64 gives
 a tighter arbiter).  tests/test_oracle_mf.py pins it against golden vectors
 produced by the live reference (tests/golden/make_golden.py).
+
+``fused_step`` / ``fit`` restate, in float64, the planned step with its fused row-wise SGD /
+Adagrad (csrc/mf_v2.cuh) and the reference's fit loop around it.  ``mutate`` (a tuple of
+names, empty by default) restates plausible kernel mistakes, so that
+tests/test_mf_planned_oracle_cpu.py can show that the GPU tolerances catch each of them:
+
+``stash_post_update``     the item side reads the user rows after the user-side update
+``neg_to_pos_row``        the negative's item term credited to the positive's row
+``user_bias_no_gn``       the user-bias gradient without the negative's term
+``hinge_strict``          hinge active at z > 0 instead of z >= 0
+``decay_all_rows``        weight decay on every row of the batch, not only rows with a non-zero term
+``no_decay_user_rows``    weight decay skipped on the user embedding rows
+``no_decay_biases``       weight decay skipped on both bias tables
+``adagrad_div_before_add`` Adagrad divides by the state before adding g^2
+``item_first4``           item lists of 5..cap terms sum only their first 4 terms
+``hot_drop_last``         the last member of each hot list (longer than ``cap``) dropped
+``local_norm``            the gradient normalised by the local batch instead of ``norm``
 """
 
 import numpy as np
+
+from oracle.explicit import apply_rowwise
 
 LOSSES = ('pointwise', 'bpr', 'hinge', 'adaptive_hinge')
 
@@ -167,3 +186,121 @@ def mf_bloom_step(Wu, Wi, bu, bi, users, items, negs, loss, num_hash, pad=0, dty
     np.add.at(dbi.reshape(-1), negs, gn)
     return dict(loss=l, pos=pos, neg=neg, dWu=dWu, dWi=dWi, dbu=dbu, dbi=dbi)
 
+
+
+def _rank_in_list(rows):
+    """Position of every member in its row's member list (members in ascending term order)
+    and that list's length."""
+    order = np.argsort(rows, kind='stable')
+    sr = rows[order]
+    rank = np.empty(len(rows), dtype=np.int64)
+    rank[order] = np.arange(len(rows)) - np.searchsorted(sr, sr, side='left')
+    return rank, np.bincount(rows)[rows]
+
+
+def _row_sums(shape, rows, vals):
+    """Dense (shape) array of the sums of ``vals`` per row id (np.add.at, by sorting)."""
+    out = np.zeros(shape)
+    if len(rows) == 0:
+        return out
+    order = np.argsort(rows, kind='stable')
+    r = rows[order]
+    starts = np.flatnonzero(np.r_[True, r[1:] != r[:-1]])
+    out.reshape(shape[0], -1)[r[starts]] = np.add.reduceat(vals[order].reshape(len(rows), -1), starts, axis=0)
+    return out
+
+
+def fused_step(params, users, items, negs, loss, opt, lr, weight_decay=0.0, eps=1e-10, states=None,
+               norm=None, mutate=(), cap=128):
+    """One in-place float64 step of the planned route (pointwise / bpr / hinge) with the fused
+    row-wise optimizer.  ``params`` = (Wu, Wi, bu, bi) and Adagrad ``states`` are float64 arrays,
+    updated in place.  ``norm`` is the batch the loss is averaged over (default len(users); the
+    global batch in gradient-out mode).  A user row is touched when one of its interactions has
+    gp != 0 or gn != 0, an item row when one of its terms (positive or negative) has g != 0;
+    touched rows take ``g + weight_decay * w``, the others stay bit-identical.
+
+    Returns dict(loss, pos, neg, gp, gn, dWu, dWi, dbu, dbi, touched_u, touched_i), the gradients and the
+    loss already divided by ``norm``."""
+    Wu, Wi, bu, bi = params
+    users, items, negs = (np.asarray(x, dtype=np.int64) for x in (users, items, negs))
+    B = len(users)
+    norm = B if (norm is None or 'local_norm' in mutate) else norm
+    # mf_step's scores and score gradients; the row sums below are mf_step's, per term
+    pos = bilinear_scores(Wu, Wi, bu, bi, users, items, np.float64)
+    neg = bilinear_scores(Wu, Wi, bu, bi, users, negs, np.float64)
+    lval, gp, gn = loss_and_score_grads(loss, pos, neg, None, np.float64)
+    gp, gn = gp * (B / norm), gn * (B / norm)
+    if 'hinge_strict' in mutate and loss == 'hinge':
+        act = (neg - pos + 1.0) > 0.0
+        gp, gn = np.where(act, gp, 0.0), np.where(act, gn, 0.0)
+
+    keep_u = np.ones(B, dtype=bool)
+    t_row = np.stack([items, negs], axis=1).reshape(-1)          # term 2b: positive, 2b + 1: negative
+    if 'neg_to_pos_row' in mutate:
+        t_row = np.repeat(items, 2)
+    t_g = np.stack([gp, gn], axis=1).reshape(-1)
+    t_user = np.repeat(users, 2)
+    keep_i = np.ones(2 * B, dtype=bool)
+    if 'item_first4' in mutate:
+        rank, length = _rank_in_list(t_row)
+        keep_i &= (rank < 4) | (length > cap)
+    if 'hot_drop_last' in mutate:
+        for keep, rows in ((keep_u, users), (keep_i, t_row)):
+            rank, length = _rank_in_list(rows)
+            keep &= ~((length > cap) & (rank == length - 1))
+
+    wds = [weight_decay] * 4
+    if 'no_decay_user_rows' in mutate:
+        wds[0] = 0.0
+    if 'no_decay_biases' in mutate:
+        wds[2] = wds[3] = 0.0
+
+    # user side: forward against the old item rows, then the user rows' update
+    Wu_old = Wu.copy()
+    ku = np.nonzero(keep_u)[0]
+    dWu = _row_sums(Wu.shape, users[ku], gp[ku, None] * Wi[items[ku]] + gn[ku, None] * Wi[negs[ku]])
+    gbu = gp if 'user_bias_no_gn' in mutate else gp + gn
+    dbu = _row_sums(bu.shape, users[ku], gbu[ku])
+    tu = np.zeros(Wu.shape[0], dtype=bool)
+    tu[users[((gp != 0) | (gn != 0)) & keep_u]] = True
+    if 'decay_all_rows' in mutate:
+        tu[users] = True
+    apply_rowwise((Wu, bu), (dWu, dbu), (tu, tu), opt, lr, (wds[0], wds[2]), eps,
+                  None if states is None else (states[0], states[2]), mutate)
+
+    # item side: the stash holds the pre-update user rows
+    src = Wu if 'stash_post_update' in mutate else Wu_old
+    ki = np.nonzero(keep_i)[0]
+    dWi = _row_sums(Wi.shape, t_row[ki], t_g[ki, None] * src[t_user[ki]])
+    dbi = _row_sums(bi.shape, t_row[ki], t_g[ki])
+    ti = np.zeros(Wi.shape[0], dtype=bool)
+    ti[t_row[(t_g != 0) & keep_i]] = True
+    if 'decay_all_rows' in mutate:
+        ti[t_row] = True
+    apply_rowwise((Wi, bi), (dWi, dbi), (ti, ti), opt, lr, (wds[1], wds[3]), eps,
+                  None if states is None else (states[1], states[3]), mutate)
+    return dict(loss=float(lval) * B / norm, pos=pos, neg=neg, gp=gp, gn=gn, dWu=dWu, dWi=dWi, dbu=dbu, dbi=dbi,
+                touched_u=tu, touched_i=ti)
+
+
+def fit(params, users, items, num_items, loss, batch_size, n_iter, random_state, opt, lr,
+        weight_decay=0.0, eps=1e-10, states=None, mutate=()):
+    """The reference's fit loop (spotlight/factorization/implicit.py:184-252) on the planned
+    route, in float64: per epoch one ``shuffle(arange(n))``, then per minibatch one
+    ``randint(0, num_items, len(batch))`` for the negatives and a ``fused_step``.
+    ``random_state`` stands where the model's constructor left it.  Parameters and states are
+    updated in place; returns the epoch losses (mean of the minibatch losses)."""
+    n = len(users)
+    losses = []
+    for _ in range(n_iter):
+        order = np.arange(n)
+        random_state.shuffle(order)
+        u, i = np.asarray(users)[order].astype(np.int64), np.asarray(items)[order].astype(np.int64)
+        ep = []
+        for lo in range(0, n, batch_size):
+            bu_, bi_ = u[lo:lo + batch_size], i[lo:lo + batch_size]
+            negs = random_state.randint(0, num_items, len(bu_), dtype=np.int64)
+            ep.append(fused_step(params, bu_, bi_, negs, loss, opt, lr, weight_decay, eps, states,
+                                 mutate=mutate)['loss'])
+        losses.append(float(np.mean(ep)))
+    return losses

@@ -1368,6 +1368,8 @@ int v2_launch_plan(const slb_mf_step_args* x, PlanDev p, int32_t* err, const int
     int sg = static_cast<int>(tiles < static_cast<int64_t>(sms) * 16 ? tiles : static_cast<int64_t>(sms) * 16);
     plan_sort_kernel<<<sg, 128, 0, st>>>(p, p.seg.long_cap);
     SLB_LAUNCH_CHECK("plan_sort_kernel");
+    plan_order_long_kernel<<<1, 256, 0, st>>>(p);                      // no-op unless two or more hot rows
+    SLB_LAUNCH_CHECK("plan_order_long_kernel");
     plan_sort_long_kernel<<<SEG_LONG_CTAS, 256, 0, st>>>(p);          // no-op unless hot rows exist
     SLB_LAUNCH_CHECK("plan_sort_long_kernel");
     return SLB_OK;

@@ -225,6 +225,43 @@ __device__ void plan_sort_long_one(Rec* base, Rec* tmp, int start, int len, uint
     __syncthreads();
 }
 
+// The scan appends hot segments to long_list in atomic order, which varies from run to run.
+// One CTA puts the list in ascending segment order (segment ids are distinct and < nseg: set
+// their bits, then each thread enumerates its own run of words after an exclusive prefix of
+// the popcounts), so every hot row lands on the same CTA of the long kernels in every run and
+// mf_user_kernel folds the hot-row loss partials in a fixed order.  Uses the first bitmap of
+// p.bits (2 * words >= ceil(3B / 32) words), which plan_sort_long_kernel only touches later.
+__global__ void __launch_bounds__(256) plan_order_long_kernel(PlanDev p) {
+    __shared__ uint32_t sh_scan[256];
+    const int nlong = p.seg.totals[3];
+    if (nlong < 2) return;                        // block-uniform
+    uint32_t* bits = p.bits;
+    const int W = (p.seg.totals[0] + 31) / 32;
+    const int per = (W + 255) / 256;
+    for (int w = threadIdx.x; w < W; w += 256) bits[w] = 0u;
+    __syncthreads();
+    for (int i = threadIdx.x; i < nlong; i += 256) {
+        const int s = p.seg.long_list[i];
+        atomicOr(bits + (s >> 5), 1u << (s & 31));
+    }
+    __syncthreads();
+    const int lo = threadIdx.x * per, hi = lo + per < W ? lo + per : W;
+    uint32_t sum = 0;
+    for (int w = lo; w < hi; ++w) sum += __popc(bits[w]);
+    sh_scan[threadIdx.x] = sum;
+    __syncthreads();
+    for (int o = 1; o < 256; o <<= 1) {
+        const uint32_t v = threadIdx.x >= o ? sh_scan[threadIdx.x - o] : 0u;
+        __syncthreads();
+        sh_scan[threadIdx.x] += v;
+        __syncthreads();
+    }
+    uint32_t run = sh_scan[threadIdx.x] - sum;
+    for (int w = lo; w < hi; ++w) {
+        for (uint32_t m = bits[w]; m; m &= m - 1u) p.seg.long_list[run++] = w * 32 + __ffs(m) - 1;
+    }
+}
+
 __global__ void __launch_bounds__(256) plan_sort_long_kernel(PlanDev p) {
     __shared__ uint32_t sh_scan[256];
     const int nlong = p.seg.totals[3];

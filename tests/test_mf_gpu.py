@@ -291,63 +291,7 @@ def test_fused_step_full_size_properties():
 
 
 # ------------------------------------------------- planned two-kernel step
-
-def _planned_problem(U, I, D, B, seed=0, scale=0.3):
-    rs = np.random.RandomState(seed)
-    Wu = (rs.randn(U, D) * scale).astype(np.float32)
-    Wi = (rs.randn(I, D) * scale).astype(np.float32)
-    bu = (rs.randn(U, 1) * 0.1).astype(np.float32)
-    bi = (rs.randn(I, 1) * 0.1).astype(np.float32)
-    users = rs.randint(0, U, B).astype(np.int64)
-    items = rs.randint(0, I, B).astype(np.int64)
-    negs = rs.randint(0, I, B).astype(np.int64)
-    return (Wu, Wi, bu, bi), (users, items, negs)
-
-
-@pytest.mark.parametrize('loss', ['bpr', 'hinge', 'pointwise'])
-@pytest.mark.parametrize('D,B', [(8, 300), (16, 2048), (32, 5000), (64, 70001), (128, 4096)])
-def test_planned_step_sgd_vs_oracle(loss, D, B):
-    """mf_user_kernel + mf_item_kernel (plan, forward, both gradient halves, in-place SGD) against
-    the float64 oracle: the learning rate is chosen so that the update is as large as the
-    weights, which makes the updated table a 1e-5-grade measurement of the gradient itself."""
-    from spotlight_b200 import _lib, ops
-    U, I = 700, 211
-    params, (users, items, negs) = _planned_problem(U, I, D, B, seed=D + B)
-    ref = omf.mf_step(*params, users, items, negs, loss, 1, np.float64)
-    lr = 0.3 / max(np.abs(ref['dWu']).max(), np.abs(ref['dWi']).max())
-    dev_p = [t(p.copy()) for p in params]
-    got_loss = ops.mf_train_step_inplace(*dev_p, t(users), t(items), t(negs), loss, _lib.OPT_SGD, lr)
-    assert_close(got_loss.item(), float(ref['loss']), 1e-5, what='loss')
-    for p0, pd, g, nm in zip(params, dev_p, (ref['dWu'], ref['dWi'], ref['dbu'], ref['dbi']),
-                             ('Wu', 'Wi', 'bu', 'bi')):
-        want = p0.astype(np.float64) - lr * g.reshape(p0.shape)
-        assert_close(pd.cpu().numpy(), want, 4e-6, what=nm)
-        if nm in ('Wu', 'Wi'):                      # untouched rows are bit-identical
-            untouched = np.abs(g).sum(1) == 0
-            assert (pd.cpu().numpy()[untouched] == p0[untouched]).all()
-
-
-def test_planned_step_adagrad_state_and_reproducible():
-    from spotlight_b200 import _lib, ops
-    U, I, D, B = 5000, 900, 64, 30000
-    params, (users, items, negs) = _planned_problem(U, I, D, B, seed=9)
-    ref = omf.mf_step(*params, users, items, negs, 'bpr', 1, np.float64)
-    outs = []
-    for _ in range(2):
-        dev_p = [t(p.copy()) for p in params]
-        states = [torch.zeros_like(p) for p in dev_p]
-        ops.mf_train_step_inplace(*dev_p, t(users), t(items), t(negs), 'bpr', _lib.OPT_ADAGRAD, 0.05,
-                                  states=states)
-        outs.append((dev_p, states))
-    for a, b in zip(outs[0][0] + outs[0][1], outs[1][0] + outs[1][1]):
-        assert torch.equal(a, b), 'planned step is not bit-reproducible'
-    for s_, g, nm in zip(outs[0][1], (ref['dWu'], ref['dWi'], ref['dbu'], ref['dbi']), ('sWu', 'sWi', 'sbu', 'sbi')):
-        assert_close(s_.cpu().numpy().astype(np.float64), (g * g).reshape(tuple(s_.shape)), 2e-5, atol=1e-30, what=nm)
-    # first Adagrad step: w -= lr * g / (|g| + eps)
-    want = params[1].astype(np.float64) - 0.05 * ref['dWi'] / (np.abs(ref['dWi']) + 1e-10)
-    big = np.abs(ref['dWi']) > 1e-7                 # sign(g) is ill-conditioned at g ~ 0
-    assert np.abs(outs[0][0][1].cpu().numpy() - want)[big].max() < 1e-6
-
+# (against the float64 oracle: tests/test_mf_planned_oracle_gpu.py)
 
 @pytest.mark.parametrize('opt', ['sgd', 'adagrad'])
 def test_planned_step_equals_first_generation(opt):
