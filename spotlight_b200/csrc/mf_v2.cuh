@@ -388,6 +388,12 @@ __device__ __forceinline__ void user_finish(const MfDev& a, const OptV2& o, floa
     }
 }
 
+// One segment of a user tile as a group reads it: h = {lane of the segment in the tile, length,
+// user row, first member}, r0 / r1 = its first two member records (r1 only for lists of two).
+// Staged in shared memory in length-class order once per tile, so no lane keeps per-segment
+// copies live across the tile's iterations.
+struct __align__(16) USeg { int4 h; int4 r0; int4 r1; };
+
 template <int LPR, int VPL, int LOSS, int TI>
 __global__ void __launch_bounds__(MF_TILE_THREADS, (VPL == 1 ? V2_UMINB : V2_UMINB2)) mf_user_kernel(MfDev a, PlanDev p, StepV2 v, int n_long_partials) {
     constexpr int D = LPR * 4 * VPL;
@@ -395,7 +401,8 @@ __global__ void __launch_bounds__(MF_TILE_THREADS, (VPL == 1 ? V2_UMINB : V2_UMI
     constexpr int WARPS = MF_TILE_THREADS / 32;
     constexpr bool RATING = LOSS >= SLB_LOSS_REGRESSION;    // one-term mode: j carries the rating
     __shared__ float sh_red[WARPS];
-    __shared__ int sh_inv[WARPS][32];
+    __shared__ USeg sh_seg[WARPS][32];
+    __shared__ int4 sh_cls[WARPS];          // {n1, n1 + n2, n1 + n2 + n3}: length-class boundaries
     __shared__ bool is_last;
     const int lane = threadIdx.x & 31;
     const int warp = threadIdx.x >> 5;
@@ -405,14 +412,18 @@ __global__ void __launch_bounds__(MF_TILE_THREADS, (VPL == 1 ? V2_UMINB : V2_UMI
     const unsigned below = (1u << lane) - 1u;
     const float invB = 1.0f / static_cast<float>(a.NB);
     const OptV2 o = {a.opt, a.lr, a.wd, a.eps};
-    const int nsegA = p.seg.totals[2];
-    const int ntiles = (nsegA + TI - 1) / TI;
+    // the number of user segments is re-read from shared memory where it is used, so it holds
+    // no register across the tile loop
+    __shared__ int sh_nsegA;
+    if (threadIdx.x == 0) sh_nsegA = p.seg.totals[2];
+    __syncthreads();
+    const volatile int& nsegA = sh_nsegA;
     const int wstride = gridDim.x * WARPS;
     const int cap = p.seg.long_cap;
     const bool adagrad = a.opt == SLB_OPT_ADAGRAD;
     float lsum = 0.f;
 
-    for (int tile = blockIdx.x * WARPS + warp; tile < ntiles; tile += wstride) {
+    for (int tile = blockIdx.x * WARPS + warp; tile < (nsegA + TI - 1) / TI; tile += wstride) {
         const int sidx = tile * TI + lane;
         const bool valid = lane < TI && sidx < nsegA;
         int start = 0, len = 0, row = 0;
@@ -441,19 +452,22 @@ __global__ void __launch_bounds__(MF_TILE_THREADS, (VPL == 1 ? V2_UMINB : V2_UMI
         else if (len == 2) pos = n1 + __popc(m2 & below);
         else if (len > 2) pos = n1 + n2 + __popc(m3 & below);
         else pos = n1 + n2 + n3 + __popc(~(m1 | m2 | m3) & below);
+        __syncwarp();                                   // the previous tile's reads are done
+        sh_seg[warp][pos] = USeg{make_int4(lane, len, row, start), r0, r1};
+        if (lane == 0) sh_cls[warp] = make_int4(n1, n1 + n2, n1 + n2 + n3, 0);
         __syncwarp();
-        sh_inv[warp][pos] = lane;
-        __syncwarp();
-        const int nvalid = n1 + n2 + n3;
 
-        for (int q0 = 0; q0 < nvalid; q0 += GPW) {
+        // the class boundaries are re-read from shared memory at every iteration (volatile), so
+        // they take no registers across the loop
+        const volatile int4* cls = sh_cls + warp;
+        for (int q0 = 0; q0 < cls->z; q0 += GPW) {
             const int q = q0 + grp;
-            const int src = sh_inv[warp][q & 31];
-            const int s_len = __shfl_sync(0xffffffffu, len, src);
-            const int s_row = __shfl_sync(0xffffffffu, row, src);
-            const int b0 = __shfl_sync(0xffffffffu, r0.x, src);
-            const int i0 = __shfl_sync(0xffffffffu, r0.y, src);
-            const int j0 = __shfl_sync(0xffffffffu, r0.z, src);
+            const int n1 = cls->x, n12 = cls->y, nvalid = cls->z;
+            const USeg& m = sh_seg[warp][q & 31];
+            const int4 h = m.h;
+            const int4 m0 = m.r0;
+            const int src = h.x, s_len = h.y, s_row = h.z;
+            const int b0 = m0.x, i0 = m0.y, j0 = m0.z;
             const int s = tile * TI + src;
             float* wrow = a.Wu + static_cast<int64_t>(s_row) * D;
             float* srow = adagrad ? a.sWu + static_cast<int64_t>(s_row) * D : nullptr;
@@ -472,14 +486,11 @@ __global__ void __launch_bounds__(MF_TILE_THREADS, (VPL == 1 ? V2_UMINB : V2_UMI
                 const float bj_ = RATING ? __int_as_float(j0) : __ldg(a.bi + j0);
                 user_member<LPR, VPL, LOSS, true>(w, ub, qi, qj, bi_, bj_, b0, invB, gmask, gl, v.t_g, acc, bacc, nz, lsum);
                 user_finish<LPR, VPL>(a, o, stash_row, wrow, srow, w, st_, acc, bacc, nz, s_row, gl);
-            } else if (q0 >= n1 && q0 + GPW <= n1 + n2) {
+            } else if (q0 >= n1 && q0 + GPW <= n12) {
                 // ---- every group of the warp: two interactions
-                const int b1 = __shfl_sync(0xffffffffu, r1.x, src);
-                const int i1 = __shfl_sync(0xffffffffu, r1.y, src);
-                const int j1 = __shfl_sync(0xffffffffu, r1.z, src);
+                const int4 m1 = m.r1;
+                const int b1 = m1.x, i1 = m1.y, j1 = m1.z;
                 const RowV<VPL> w = row_ldcs<LPR, VPL>(wrow, gl);
-                RowV<VPL> st_ = row_zero<VPL>();
-                if (adagrad) st_ = row_ldcs<LPR, VPL>(srow, gl);
                 const RowV<VPL> qi0 = row_ldg<LPR, VPL>(a.Wi + static_cast<int64_t>(i0) * D, gl);
                 const RowV<VPL> qj0 = RATING ? row_zero<VPL>() : row_ldg<LPR, VPL>(a.Wi + static_cast<int64_t>(j0) * D, gl);
                 const float ub = a.bu[s_row];
@@ -489,15 +500,16 @@ __global__ void __launch_bounds__(MF_TILE_THREADS, (VPL == 1 ? V2_UMINB : V2_UMI
                 user_member<LPR, VPL, LOSS, true>(w, ub, qi0, qj0, bi0, bj0, b0, invB, gmask, gl, v.t_g, acc, bacc, nz, lsum);
                 const RowV<VPL> qi1 = row_ldg<LPR, VPL>(a.Wi + static_cast<int64_t>(i1) * D, gl);
                 const RowV<VPL> qj1 = RATING ? row_zero<VPL>() : row_ldg<LPR, VPL>(a.Wi + static_cast<int64_t>(j1) * D, gl);
+                // the state row is loaded with the second member's rows, once the first one's are dead
+                RowV<VPL> st_ = row_zero<VPL>();
+                if (adagrad) st_ = row_ldcs<LPR, VPL>(srow, gl);
                 user_member<LPR, VPL, LOSS, true>(w, ub, qi1, qj1, bi1, bj1, b1, invB, gmask, gl, v.t_g, acc, bacc, nz, lsum);
                 user_finish<LPR, VPL>(a, o, stash_row, wrow, srow, w, st_, acc, bacc, nz, s_row, gl);
             } else {
                 // ---- mixed iteration (class boundaries, lists of 3+): group-divergent generic path
-                const int s_start = __shfl_sync(0xffffffffu, start, src);
+                const int s_start = h.w;
                 if (q >= nvalid || s_len > cap) continue;         // idle group / hot row (mf_user_long_kernel)
                 const RowV<VPL> w = row_ldcs<LPR, VPL>(wrow, gl);
-                RowV<VPL> st_ = row_zero<VPL>();
-                if (adagrad) st_ = row_ldcs<LPR, VPL>(srow, gl);
                 const float ub = a.bu[s_row];
                 for (int k = 0; k < s_len; ++k) {
                     // every lane of the group reads the same (sorted) record: one broadcast transaction
@@ -508,6 +520,9 @@ __global__ void __launch_bounds__(MF_TILE_THREADS, (VPL == 1 ? V2_UMINB : V2_UMI
                     user_member<LPR, VPL, LOSS, false>(w, ub, qi, qj, __ldg(a.bi + r.y), bj_, r.x, invB, gmask,
                                                        gl, v.t_g, acc, bacc, nz, lsum);
                 }
+                // the state row is only needed by the update: not held across the member loop
+                RowV<VPL> st_ = row_zero<VPL>();
+                if (adagrad) st_ = row_ldcs<LPR, VPL>(srow, gl);
                 user_finish<LPR, VPL>(a, o, stash_row, wrow, srow, w, st_, acc, bacc, nz, s_row, gl);
             }
         }
@@ -632,6 +647,11 @@ __global__ void __launch_bounds__(256) mf_user_long_kernel(MfDev a, PlanDev p, S
 #ifndef V2_IFAST
 #define V2_IFAST 4
 #endif
+static_assert(V2_IFAST == 4, "ISeg stages exactly four short-list members");
+
+// One segment of an item tile as a group reads it: h = {length, item row, first member}, and for
+// lists of up to V2_IFAST members their user segments u and gradients g, loaded by the owning lane.
+struct __align__(16) ISeg { int4 h; int4 u; float4 g; };
 #ifndef V2_IMINB
 #define V2_IMINB 6
 #endif
@@ -647,7 +667,9 @@ __global__ void __launch_bounds__(MF_TILE_THREADS, V2_IMINB) mf_item_kernel(MfDe
     constexpr int WARPS = MF_TILE_THREADS / 32;
     constexpr int CAP = seg_sort_cap(LPR);
     __shared__ int32_t sh_all[WARPS * GPW * 2 * CAP];
+    __shared__ ISeg sh_seg[WARPS][32];
     const int lane = threadIdx.x & 31;
+    const int warp = threadIdx.x >> 5;
     const int gl = lane & (LPR - 1);
     const int grp = lane / LPR;
     const int c = gl * 4;
@@ -664,42 +686,45 @@ __global__ void __launch_bounds__(MF_TILE_THREADS, V2_IMINB) mf_item_kernel(MfDe
     for (int tile = blockIdx.x * WARPS + (threadIdx.x >> 5); tile < ntiles; tile += wstride) {
         const int sidx = nsegA + tile * TI + lane;
         const bool valid = lane < TI && sidx < nseg;
-        int start = 0, len = 0, row = 0;
-        int pu[V2_IFAST] = {};
-        float pg[V2_IFAST] = {};
-        if (valid) {
-            start = p.seg.seg_start[sidx] - ubase;
-            len = p.seg.seg_start[sidx + 1] - ubase - start;
-            row = p.seg.seg_row[sidx] - static_cast<int>(a.U);
-            if (len <= V2_IFAST) {
+        {
+            int start = 0, len = 0, row = 0;
+            int pu[V2_IFAST] = {};
+            float pg[V2_IFAST] = {};
+            if (valid) {
+                start = p.seg.seg_start[sidx] - ubase;
+                len = p.seg.seg_start[sidx + 1] - ubase - start;
+                row = p.seg.seg_row[sidx] - static_cast<int>(a.U);
+                if (len <= V2_IFAST) {
 #pragma unroll
-                for (int k = 0; k < V2_IFAST; ++k)
-                    if (k < len) {
-                        const int2 r = __ldg(reinterpret_cast<const int2*>(p.mi + start + k));
-                        pu[k] = r.y;
-                        pg[k] = t_g[r.x];
-                    }
+                    for (int k = 0; k < V2_IFAST; ++k)
+                        if (k < len) {
+                            const int2 r = __ldg(reinterpret_cast<const int2*>(p.mi + start + k));
+                            pu[k] = r.y;
+                            pg[k] = t_g[r.x];
+                        }
+                }
             }
+            __syncwarp();                                     // the previous tile's reads are done
+            sh_seg[warp][lane] = ISeg{make_int4(len, row, start, 0), make_int4(pu[0], pu[1], pu[2], pu[3]),
+                                      make_float4(pg[0], pg[1], pg[2], pg[3])};
+            __syncwarp();
         }
         for (int it = 0; it < ITERS; ++it) {
             const int src = it * GPW + grp;
-            const int s_len = __shfl_sync(0xffffffffu, len, src & 31);
-            const int s_row = __shfl_sync(0xffffffffu, row, src & 31);
-            const int s_start = __shfl_sync(0xffffffffu, start, src & 31);
-            int su[V2_IFAST];
-            float sg[V2_IFAST];
-#pragma unroll
-            for (int k = 0; k < V2_IFAST; ++k) {
-                su[k] = __shfl_sync(0xffffffffu, pu[k], src & 31);
-                sg[k] = __shfl_sync(0xffffffffu, pg[k], src & 31);
-            }
             const int s = nsegA + tile * TI + src;
             if (src >= TI || s >= nseg) continue;             // group-uniform
+            const ISeg& m = sh_seg[warp][src];
+            const int4 h = m.h;
+            const int s_len = h.x, s_row = h.y, s_start = h.z;
             if (s_len > CAP) continue;                        // hot row: mf_item_long_kernel
             float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
             float bacc = 0.f;
             bool nz = false;
             if (s_len <= V2_IFAST) {
+                const int4 u4 = m.u;
+                const float4 g4 = m.g;
+                const int su[V2_IFAST] = {u4.x, u4.y, u4.z, u4.w};
+                const float sg[V2_IFAST] = {g4.x, g4.y, g4.z, g4.w};
                 float4 x[V2_IFAST];
 #pragma unroll
                 for (int k = 0; k < V2_IFAST; ++k)
