@@ -39,7 +39,11 @@ EXPORTS = (
     'slb_unique_workspace_bytes', 'slb_unique_bucket', 'slb_shard_gather_batch', 'slb_adagrad_dense',
     'slb_loss_workspace_bytes', 'slb_pairwise_loss', 'slb_rating_loss',
     'slb_seq_step_workspace_bytes', 'slb_seq_train_step', 'slb_seq_representation',
+    'slb_sort_keys', 'slb_radix_order_workspace_bytes', 'slb_radix_order',
+    'slb_sequence_windows_workspace_bytes', 'slb_sequence_windows', 'slb_sequence_emit',
+    'slb_user_split_workspace_bytes', 'slb_user_split_order', 'slb_gather_elements',
 )
+
 
 
 class MfStepArgs(ctypes.Structure):
@@ -171,6 +175,18 @@ def _declare(lib):
     lib.slb_seq_step_workspace_bytes.restype = c_sz
     lib.slb_seq_train_step.argtypes = [P(SeqStepArgs), c_vp]
     lib.slb_seq_representation.argtypes = [P(SeqStepArgs), c_vp, c_vp]
+    c_u32, c_u64 = ctypes.c_uint32, ctypes.c_uint64
+    lib.slb_sort_keys.argtypes = [c_vp, c_i32, c_vp, c_i32, c_i64, c_vp, c_vp, c_vp, c_vp]
+    for name in ('slb_radix_order_workspace_bytes', 'slb_sequence_windows_workspace_bytes',
+                 'slb_user_split_workspace_bytes'):
+        getattr(lib, name).argtypes = [c_i64]
+        getattr(lib, name).restype = c_sz
+    lib.slb_radix_order.argtypes = [c_vp, c_u64, c_i32, c_vp, c_u64, c_i32, c_i64, c_vp, c_vp, c_sz, c_vp]
+    lib.slb_sequence_windows.argtypes = [c_vp, c_vp, c_i64, c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_sz, c_vp]
+    lib.slb_sequence_emit.argtypes = [c_vp, c_vp, c_i32, c_vp, c_i32, c_vp, c_vp, c_i64, c_i64, c_i32, c_i64,
+                                      c_vp, c_vp, c_vp]
+    lib.slb_user_split_order.argtypes = [c_vp, c_i64, c_u32, c_u64, c_u64, c_vp, c_vp, c_vp, c_sz, c_vp]
+    lib.slb_gather_elements.argtypes = [c_vp, c_i32, c_i64, c_vp, c_i32, c_vp, c_vp]
     for name in EXPORTS:
         fn = getattr(lib, name)
         if fn.restype is ctypes.c_int:   # default -> status code

@@ -16,6 +16,9 @@ predictions with ``FLOAT_MAX``, so excluded targets are ranked with that score.
 Ties: where exactly equal scores straddle the k boundary, precision/recall order them by
 ascending item id (numpy's ``kind='stable'``); the reference's default ``argsort`` breaks such
 ties in an unspecified order.
+
+Test and train sets may also hold CUDA tensors (``Interactions`` / ``SequenceInteractions`` made on
+the device); each scorer downloads them once at entry.
 """
 
 import numpy as np
@@ -23,6 +26,7 @@ import torch
 
 from spotlight_b200 import _lib, ops
 from spotlight_b200.factorization.representations import BilinearNet
+from spotlight_b200.interactions import _to_host
 from spotlight_b200.layers import ScaledEmbedding
 from spotlight_b200.sequence.representations import LSTMNet, _SeqNetBase
 
@@ -147,6 +151,7 @@ def mrr_score(model, test, train=None, user_block=2048):
     negated predictions) over the user's test items; train items, when given, are pushed to
     the bottom.  ``user_block`` users are scored per GEMM.
     """
+    test, train = _to_host(test), None if train is None else _to_host(train)
     n_users = int((np.diff(test.tocsr().indptr) > 0).sum())
     out = np.empty(n_users, dtype=np.float64)
     for lo, scores, te in _user_blocks(model, test, train, user_block):
@@ -179,6 +184,7 @@ def precision_recall_score(model, test, train=None, k=10, user_block=2048):
     array.  Exact score ties across the k boundary are ordered by ascending item id (numpy's
     ``argsort(kind='stable')``); the reference's default argsort orders them arbitrarily.
     """
+    test, train = _to_host(test), None if train is None else _to_host(train)
     ks = np.array([k]) if np.isscalar(k) else np.asarray(k)
     n_users = int((np.diff(test.tocsr().indptr) > 0).sum())
     hits = np.empty((n_users, len(ks)), dtype=np.int64)
@@ -211,6 +217,7 @@ def sequence_mrr_score(model, test, exclude_preceding=False, sequence_block=256)
     With ``exclude_preceding`` every item of the input prefix -- padding id 0 included, as in the
     reference -- is pushed to the bottom.  ``sequence_block`` sequences are scored at once.
     """
+    test = _to_host(test)
     _check_items(test.sequences.reshape(-1), model._num_items)
     sequences = test.sequences[:, :-1]
     targets = test.sequences[:, -1].astype(np.int64)
@@ -230,6 +237,7 @@ def sequence_precision_recall_score(model, test, k=10, exclude_preceding=False, 
     precision = hits / min(k, num_items), recall = hits / k.  ``k`` must be shorter than the
     sequences.  Exact score ties across the k boundary are ordered by ascending item id.
     """
+    test = _to_host(test)
     S = test.sequences.shape[1]
     if not 0 < k < S:
         raise ValueError('k = %d must be in [1, sequence length %d)' % (k, S))
@@ -259,6 +267,7 @@ def rmse_score(model, test):
     block's mean squared error comes from the deterministic ``slb_rating_loss`` reduction and the
     blocks are combined in float64.  Returns a NumPy float32 like the reference.
     """
+    test = _to_host(test)
     n = len(test.user_ids)
     if test.ratings is None:
         raise TypeError("unsupported operand type(s) for -: 'NoneType' and 'float'")

@@ -190,7 +190,10 @@ class ExplicitFactorizationModel(object):
             raise TypeError("object of type 'NoneType' has no len()")
         if len(interactions.ratings) != n:
             raise ValueError('All inputs to shuffle must have the same length.')
-        ratings_dev = torch.from_numpy(np.ascontiguousarray(interactions.ratings, dtype=np.float32)).to(device)
+        if torch.is_tensor(interactions.ratings) and interactions.ratings.is_cuda:
+            ratings_dev = interactions.ratings.to(device, torch.float32).contiguous()
+        else:
+            ratings_dev = torch.from_numpy(np.ascontiguousarray(interactions.ratings, dtype=np.float32)).to(device)
 
         on_device = DEVICE_SHUFFLE_MIN <= n <= SHUFFLE_DEVICE_MAX and \
             self._random_state.get_state()[0] == 'MT19937'

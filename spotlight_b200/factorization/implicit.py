@@ -32,6 +32,7 @@ from spotlight_b200 import _lib, ops
 from spotlight_b200.factorization._components import _predict_process_ids
 from spotlight_b200.factorization.representations import BilinearNet
 from spotlight_b200.helpers import _repr_model
+from spotlight_b200.interactions import _device_of
 from spotlight_b200.losses import adaptive_hinge_loss, bpr_loss, hinge_loss, pointwise_loss
 from spotlight_b200.rng import (SHUFFLE_DEVICE_MAX, permute_ids, shuffle_begin, shuffle_end,
                                 shuffled_order_device)
@@ -67,7 +68,12 @@ def _to_device_ids(ids, device):
 
 def _to_device_narrow(ids, device):
     """Host id array -> CUDA tensor in its own width (int32 stays int32 on the wire and in
-    HBM; the permutation gather widens)."""
+    HBM; the permutation gather widens).  An int32 / int64 CUDA tensor already on ``device``
+    is used as it is."""
+    if torch.is_tensor(ids) and ids.is_cuda:
+        if ids.dtype not in (torch.int32, torch.int64):
+            ids = ids.long()
+        return ids.to(device).contiguous()
     arr = np.ascontiguousarray(ids)
     if arr.dtype not in (np.int32, np.int64):
         arr = arr.astype(np.int64)
@@ -231,6 +237,8 @@ class ImplicitFactorizationModel(object):
         # ids go to the device once per fit(); each epoch only the permutation is made
         # there (the reference re-uploads both shuffled id arrays, implicit.py:216-219)
         copy_stream = _side_stream(device)          # independent of the shuffle kernels just queued
+        if _device_of(interactions, ('user_ids', 'item_ids')) is not None:
+            copy_stream.wait_stream(main)           # CUDA ids: any widening runs after their producer
         with torch.cuda.stream(copy_stream):
             users_dev = _to_device_narrow(user_ids, device)
             items_dev = _to_device_narrow(item_ids, device)

@@ -1,11 +1,53 @@
 """Data containers with the reference's attributes and behaviour
-(spotlight/interactions.py:38-312).  Host-side NumPy, run once before ``fit``;
-``to_sequence`` is vectorised instead of the reference's per-window Python
-generator (interactions.py:11-35, 250-257) but returns the same matrices.
+(spotlight/interactions.py:38-312).
+
+An ``Interactions`` holds either NumPy arrays or CUDA tensors on one device.  With NumPy
+arrays ``to_sequence`` is host code, vectorised instead of the reference's per-window Python
+generator (interactions.py:11-35, 250-257) but returning the same matrices; with CUDA tensors
+it runs on the device (csrc/prepare.cu) and returns the same matrices as CUDA tensors.
 """
 
 import numpy as np
 import scipy.sparse as sp
+import torch
+
+_COLUMNS = ('user_ids', 'item_ids', 'ratings', 'timestamps', 'weights')
+
+
+def _device_of(data, names=_COLUMNS):
+    """The CUDA device of ``data``'s present columns, or None when none is a CUDA tensor.
+    A mix of CUDA tensors and other arrays, or of CUDA devices, raises ``ValueError``."""
+    cols = [getattr(data, name) for name in names if getattr(data, name) is not None]
+    on_cuda = [torch.is_tensor(c) and c.is_cuda for c in cols]
+    if not any(on_cuda):
+        return None
+    if not all(on_cuda) or len(set(c.device for c in cols)) != 1:
+        raise ValueError('Interactions must hold either all NumPy arrays or all CUDA tensors on one device')
+    return cols[0].device
+
+
+def _to_host(data):
+    """``data`` itself when it holds no CUDA tensor, otherwise a copy with NumPy columns."""
+    if isinstance(data, SequenceInteractions):
+        if _device_of(data, ('sequences', 'user_ids')) is None:
+            return data
+        return SequenceInteractions(data.sequences.cpu().numpy(),
+                                    user_ids=None if data.user_ids is None else data.user_ids.cpu().numpy(),
+                                    num_items=data.num_items)
+    if _device_of(data) is None:
+        return data
+    cols = {name: None if getattr(data, name) is None else getattr(data, name).cpu().numpy()
+            for name in _COLUMNS}
+    return Interactions(cols.pop('user_ids'), cols.pop('item_ids'), num_users=data.num_users,
+                        num_items=data.num_items, **cols)
+
+
+def _column_index(min_sequence_length, L):
+    """The column ``sequences[:, -min_sequence_length]`` reads, with NumPy's IndexError."""
+    i = -int(min_sequence_length)
+    if not -L <= i < L:
+        raise IndexError('index %d is out of bounds for axis 1 with size %d' % (i, L))
+    return i + L if i < 0 else i
 
 
 class Interactions(object):
@@ -64,6 +106,9 @@ class Interactions(object):
         """
         if self.timestamps is None:
             raise ValueError('Cannot convert to sequences, timestamps not available.')
+        dev = _device_of(self)
+        if dev is not None:
+            return self._to_sequence_device(max_sequence_length, min_sequence_length, step_size)
         if 0 in self.item_ids:
             raise ValueError('0 is used as an item id, conflicting with the sequence '
                              'padding value.')
@@ -92,6 +137,35 @@ class Interactions(object):
             sequences = sequences[keep]
             sequence_users = sequence_users[keep]
 
+        return SequenceInteractions(sequences, user_ids=sequence_users, num_items=self.num_items)
+
+    def _to_sequence_device(self, max_sequence_length, min_sequence_length, step_size):
+        """``to_sequence`` of CUDA columns: a stable radix sort of (user, timestamp) and one
+        kernel writing the windows; the same matrices as the host branch, as CUDA tensors."""
+        from spotlight_b200 import prepare
+        users, items, ts = self.user_ids, self.item_ids, self.timestamps
+        if users.dtype not in (torch.int32, torch.int64) or items.dtype not in (torch.int32, torch.int64):
+            raise TypeError('to_sequence on the device needs int32 or int64 user and item ids')
+        if ts.dtype not in (torch.int32, torch.int64, torch.float32, torch.float64):
+            raise TypeError('to_sequence on the device needs int32, int64, float32 or float64 timestamps, '
+                            'got %s' % ts.dtype)
+        if self.num_items >= 2 ** 31:
+            raise ValueError('to_sequence on the device needs num_items < 2**31')
+        n = len(users)
+        if not 1 <= n < 2 ** 31:
+            raise ValueError('to_sequence on the device needs 1 <= n < 2**31 interactions')
+        if bool((items == 0).any()):
+            raise ValueError('0 is used as an item id, conflicting with the sequence '
+                             'padding value.')
+        L = int(max_sequence_length)
+        step = L if step_size is None else int(step_size)
+        if L < 1 or step < 1 or (step_size is not None and step != step_size):
+            raise ValueError('to_sequence on the device needs integer max_sequence_length >= 1 '
+                             'and step_size >= 1')
+        need = -1 if min_sequence_length is None else L - _column_index(min_sequence_length, L)
+        with torch.cuda.device(users.device):
+            sequences, sequence_users = prepare.sequence_rows(users.contiguous(), items.contiguous(),
+                                                              ts.contiguous(), L, step, need)
         return SequenceInteractions(sequences, user_ids=sequence_users, num_items=self.num_items)
 
 

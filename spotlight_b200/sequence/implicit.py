@@ -114,7 +114,8 @@ class ImplicitSequenceModel(object):
 
     def fit(self, interactions, verbose=False):
         """Fit the model; repeated calls resume (implicit.py:193-264)."""
-        sequences = interactions.sequences.astype(np.int64)
+        on_device = torch.is_tensor(interactions.sequences) and interactions.sequences.is_cuda
+        sequences = interactions.sequences if on_device else interactions.sequences.astype(np.int64)
 
         if not self._initialized:
             self._initialize(interactions)
@@ -129,7 +130,10 @@ class ImplicitSequenceModel(object):
         # the sequences go to the device once per fit(); every epoch permutes the resident rows
         # (cumulatively, as the reference's `sequences = sequences[shuffle_indices]` does,
         # implicit.py:217-220) instead of re-indexing on the host and re-uploading
-        sequences_tensor = gpu(torch.from_numpy(np.ascontiguousarray(sequences)), self._use_cuda)
+        if on_device:       # a device SequenceInteractions (to_sequence of CUDA interactions) stays there
+            sequences_tensor = sequences.to(device, torch.int64).contiguous()
+        else:
+            sequences_tensor = gpu(torch.from_numpy(np.ascontiguousarray(sequences)), self._use_cuda)
         n_seq = len(sequences)
 
         for epoch_num in range(self._n_iter):
