@@ -896,6 +896,7 @@ struct BloomSpec {
     int64_t num_users, num_items;   // id spaces (bias tables)
     int64_t* ids_u2; int64_t* ids_i2;   // [2B] bias scatter ids
     float* g_u2; float* g_i2;           // [2B] bias scatter values
+    int idle_ids;                       // fused mode: a pair that touches no bias gets id -1
 };
 
 __device__ __forceinline__ int64_t hashed_row(int64_t id, int k, int H, const uint32_t* seeds,
@@ -968,17 +969,20 @@ __global__ void __launch_bounds__(MF_THREADS) mf_fwd_bloom_kernel(MfDev a, const
             if (a.pos_out) a.pos_out[bb] = p;
             // user-bias gradient: when the negative is scored with the same user (every loss but
             // adaptive hinge) the two halves are emitted as ONE pair, so that bpr / hinge's
-            // gp + gn = 0 is an exact zero (dropped downstream) and not a rounding residue of two
-            // sums that Adagrad would turn into a full step
+            // gp + gn = 0 is an exact zero and not a rounding residue of two sums that Adagrad
+            // would turn into a full step.  In fused mode a bias is touched (and so decayed) when
+            // one of its interaction sides has g != 0, even if its summed gradient is exactly 0:
+            // the pairs name their bias by id, and a pair that touches nothing gets id -1
+            const bool idle = h.idle_ids != 0;
             if (nuid == u) {
-                h.ids_u2[bb] = u; h.g_u2[bb] = gp + gn;
-                h.ids_u2[a.B + bb] = u; h.g_u2[a.B + bb] = 0.f;
+                h.ids_u2[bb] = (!idle || gp != 0.f || gn != 0.f) ? u : -1; h.g_u2[bb] = gp + gn;
+                h.ids_u2[a.B + bb] = idle ? -1 : u; h.g_u2[a.B + bb] = 0.f;
             } else {
-                h.ids_u2[bb] = u; h.g_u2[bb] = gp;
-                h.ids_u2[a.B + bb] = nuid; h.g_u2[a.B + bb] = gn;
+                h.ids_u2[bb] = (!idle || gp != 0.f) ? u : -1; h.g_u2[bb] = gp;
+                h.ids_u2[a.B + bb] = (!idle || gn != 0.f) ? nuid : -1; h.g_u2[a.B + bb] = gn;
             }
-            h.ids_i2[bb] = i; h.g_i2[bb] = gp;
-            h.ids_i2[a.B + bb] = njid; h.g_i2[a.B + bb] = gn;
+            h.ids_i2[bb] = (!idle || gp != 0.f) ? i : -1; h.g_i2[bb] = gp;
+            h.ids_i2[a.B + bb] = (!idle || gn != 0.f) ? njid : -1; h.g_i2[a.B + bb] = gn;
             const int64_t t0 = bb * 2 * pairs;
             for (int side = 0; side < 2; ++side) {
                 const float g = side ? gn : gp;
@@ -1724,7 +1728,9 @@ int slb_mf_scores_backward(const float* gscores, const int64_t* users, const int
 // The pairs are grouped through a hash-bucket segment index (bucket = id & (NB - 1), NB ~ 2n a
 // power of two: count -> scan -> fill), each bucket's few members are ordered by (id, pair) and
 // every distinct id gets its gradient summed in pair order and one optimizer update.
-// Deterministic, O(n) traffic.
+// Deterministic, O(n) traffic.  A pair takes part when g != 0 (``by_id`` = 0, the C entry point:
+// g == 0 pairs are padding) or when id >= 0 (``by_id`` = 1, the fused hashed step, whose touched
+// biases may sum to exactly 0 and still take their weight decay).
 // ---------------------------------------------------------------------------
 namespace {
 
@@ -1733,18 +1739,23 @@ struct BiasSparse {
     const int64_t* ids; const float* g; int64_t n; int64_t mask;
     float* b; float* sb;
     int32_t opt; float lr, wd, eps;
+    int32_t by_id;
 };
+
+__device__ __forceinline__ bool bias_pair_live(const BiasSparse& p, int64_t k) {
+    return p.by_id ? p.ids[k] >= 0 : p.g[k] != 0.f;
+}
 
 __global__ void __launch_bounds__(256) bias_count_kernel(BiasSparse p) {
     const int64_t nth = static_cast<int64_t>(gridDim.x) * blockDim.x;
     for (int64_t k = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x; k < p.n; k += nth)
-        if (p.g[k] != 0.f) atomicAdd(p.seg.cnt + (p.ids[k] & p.mask), 1);
+        if (bias_pair_live(p, k)) atomicAdd(p.seg.cnt + (p.ids[k] & p.mask), 1);
 }
 
 __global__ void __launch_bounds__(256) bias_fill_kernel(BiasSparse p) {
     const int64_t nth = static_cast<int64_t>(gridDim.x) * blockDim.x;
     for (int64_t k = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x; k < p.n; k += nth)
-        if (p.g[k] != 0.f) seg_place(p.seg, p.ids[k] & p.mask, static_cast<int32_t>(k));
+        if (bias_pair_live(p, k)) seg_place(p.seg, p.ids[k] & p.mask, static_cast<int32_t>(k));
 }
 
 __global__ void __launch_bounds__(256) bias_apply_kernel(BiasSparse p) {
@@ -1791,14 +1802,14 @@ size_t bias_sparse_bytes(int64_t n) {
 }
 
 int bias_sparse_apply(void* wsp, const int64_t* ids, const float* g, int64_t n, float* b, float* sb,
-                      int32_t opt, float lr, float wd, float eps, cudaStream_t st) {
+                      int32_t opt, float lr, float wd, float eps, bool by_id, cudaStream_t st) {
     int64_t nb = 4096;
     while (nb < 2 * n) nb <<= 1;
     WsCarver ws(wsp);
     BiasSparse p;
     p.seg = seg_index_carve(ws, nb, n);
     p.ids = ids; p.g = g; p.n = n; p.mask = nb - 1; p.b = b; p.sb = sb;
-    p.opt = opt; p.lr = lr; p.wd = wd; p.eps = eps;
+    p.opt = opt; p.lr = lr; p.wd = wd; p.eps = eps; p.by_id = by_id ? 1 : 0;
     const int sms = slb_sms();
     int grid = static_cast<int>((n + 255) / 256);
     if (grid > sms * 8) grid = sms * 8;
@@ -1922,6 +1933,7 @@ int slb_mf_bloom_train_step(const slb_mf_bloom_args* x, slb_stream_t stream) {
     for (int k = 0; k < 24; ++k) { h.su[k] = x->user_seeds[k]; h.si[k] = x->item_seeds[k]; }
     h.num_users = b.num_users; h.num_items = b.num_items;
     h.ids_u2 = l.ids_u2; h.ids_i2 = l.ids_i2; h.g_u2 = l.g_u2; h.g_i2 = l.g_i2;
+    h.idle_ids = fused ? 1 : 0;
     if (!fused && pairs_u) { h.ids_u2 = x->pair_ids_u; h.g_u2 = x->pair_g_u; }
     if (!fused && pairs_i) { h.ids_i2 = x->pair_ids_i; h.g_i2 = x->pair_g_i; }
 
@@ -1962,9 +1974,11 @@ int slb_mf_bloom_train_step(const slb_mf_bloom_args* x, slb_stream_t stream) {
         const int agrid = static_cast<int>(aw < static_cast<int64_t>(sms) * 8 ? aw : static_cast<int64_t>(sms) * 8);
         DISPATCH_LPR2(lpr, mf_apply_kernel, 1, agrid, MF_THREADS, st, a);
         SLB_LAUNCH_CHECK("mf_apply_kernel<items>");
-        int rcb = bias_sparse_apply(l.bws_u, l.ids_u2, l.g_u2, 2 * B, b.bu, b.state_bu, b.opt, b.lr, b.weight_decay, b.eps, st);
+        int rcb = bias_sparse_apply(l.bws_u, l.ids_u2, l.g_u2, 2 * B, b.bu, b.state_bu, b.opt, b.lr, b.weight_decay,
+                                    b.eps, true, st);
         if (rcb != SLB_OK) return rcb;
-        return bias_sparse_apply(l.bws_i, l.ids_i2, l.g_i2, 2 * B, b.bi, b.state_bi, b.opt, b.lr, b.weight_decay, b.eps, st);
+        return bias_sparse_apply(l.bws_i, l.ids_i2, l.g_i2, 2 * B, b.bi, b.state_bi, b.opt, b.lr, b.weight_decay,
+                                 b.eps, true, st);
     }
     DISPATCH_LPR3(lpr, mf_bwd_tile_kernel, 0, 32, tgrid, MF_TILE_THREADS, st, a);
     SLB_LAUNCH_CHECK("mf_bwd_tile_kernel");
@@ -1995,7 +2009,7 @@ int slb_bias_sparse_apply(const int64_t* ids, const float* g, int64_t n, float* 
         slb_set_error("bias_sparse_apply: workspace too small");
         return SLB_ENOSPC;
     }
-    return bias_sparse_apply(workspace, ids, g, n, bias, state, opt, lr, weight_decay, eps,
+    return bias_sparse_apply(workspace, ids, g, n, bias, state, opt, lr, weight_decay, eps, false,
                              static_cast<cudaStream_t>(stream));
 }
 

@@ -49,7 +49,8 @@ class FusedAdagrad(torch.optim.Adagrad):
     rows a minibatch updates only, in every element of such a row; torch's dense Adagrad decays
     every row on every step.  A row is updated when one of its terms has a non-zero score
     gradient (in a sequence step also when its embedding gradient is non-zero, through the
-    item's input role), even if its own embedding gradient is exactly zero.  With
+    item's input role), even if its own embedding gradient is exactly zero; a bias is updated
+    with its row, so the user bias of a bpr / hinge interaction (gp + gn = 0) is decayed too.  With
     ``weight_decay = 0`` (the default) this is the dense update; with ``weight_decay > 0`` rows
     outside the minibatch are not decayed."""
 
