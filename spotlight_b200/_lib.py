@@ -102,6 +102,8 @@ class SeqStepArgs(ctypes.Structure):
         ('lstm_w_ih', c_vp), ('lstm_w_hh', c_vp), ('lstm_b_ih', c_vp), ('lstm_b_hh', c_vp),
         ('dlstm_w_ih', c_vp), ('dlstm_w_hh', c_vp), ('dlstm_b_ih', c_vp), ('dlstm_b_hh', c_vp),
         ('num_mixtures', c_i32), ('mix_w', c_vp), ('mix_b', c_vp), ('dmix_w', c_vp), ('dmix_b', c_vp),
+        ('item_rows', c_i64), ('item_hashes', c_i32), ('item_seeds', ctypes.c_uint32 * 24),
+        ('item_padding_idx', c_i64),
     ]
 
 

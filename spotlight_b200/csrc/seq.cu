@@ -27,6 +27,13 @@
 //                        the LSTM's projections and weight gradients are k = 1 conv GEMMs
 //   mix_score_kernel     MixtureLSTMNet head (seq_mix.cuh): softmax-weighted taste scores and their
 //                        gradients into the 2M projection blocks; the projection is 2M k = 1 conv GEMMs
+//
+// Hashed item table (BloomEmbedding, item_hashes > 0): seq_gather_hashed_kernel sums each
+// position's H hashed rows once into Xs (B, S, D) -- the X0 of CNN / LSTM / mixture -- and the pool,
+// score and mixture kernels read the input and target rows from it by position (template row
+// source); negatives are summed from their hashed rows where they are scored.  The backward keys
+// every term once per hash onto table rows and once onto its id's bias, in one segment index over
+// the two key spaces; hot rows go through seg_sort_long_kernel.
 #include <stdlib.h>
 
 #include "segindex.cuh"
@@ -59,7 +66,27 @@ struct SeqDev {
     // MixtureLSTMNet head: M mixtures, P = 2M blocks of (B, T, D) (components, then mixture
     // vectors); mix_score_kernel overwrites P with d loss / d P
     int M; float* P;
+    // hashed item table (H > 0): E holds Mrows rows, an item is the sum of its H rows (item4);
+    // Xs (B, S, D) holds the summed rows of the sequence positions, read by position
+    int H; int64_t Mrows; uint32_t seeds[24];
+    const float* Xs;
 };
+
+// Row source of the item reads: a plain table by id, or the hashed sum of the H rows of the
+// id in hash order (BloomEmbedding, layers.py:132-244; the padding id maps to row 0).
+template <bool HASHED>
+__device__ __forceinline__ float4 item4(const SeqDev& a, int64_t id, int c) {
+    if (!HASHED) return ldg4(a.E + id * a.D + c);
+    float4 s = make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll
+    for (int k = 0; k < 24; ++k) {          // static seed indices: the seeds stay in the parameter bank
+        if (k < a.H) {
+            const float4 v = ldg4(a.E + bloom_row(id, a.seeds[k], a.Mrows, 0) * a.D + c);
+            s.x += v.x; s.y += v.y; s.z += v.z; s.w += v.w;
+        }
+    }
+    return s;
+}
 
 // ---------------------------------------------------------------- mask count
 __global__ void __launch_bounds__(256)
@@ -93,10 +120,18 @@ seq_mask_kernel(const int64_t* __restrict__ seqs, const int64_t* __restrict__ ne
 
 __device__ __forceinline__ int64_t clamp_id(int64_t v, int64_t I) { return v < 0 || v >= I ? 0 : v; }
 
+// Input row of position (b, t): E[seq] of a plain table, or (BYPOS) row b * S + t of the
+// materialised (B, S, D) rows of a hashed one.
+template <bool BYPOS>
+__device__ __forceinline__ const float* in_row(const float* E, const int64_t* sq, int64_t b, int t, int S, int D,
+                                               int64_t I) {
+    return BYPOS ? E + (b * S + t) * D : E + clamp_id(sq[t], I) * D;
+}
+
 // ------------------------------------------------------------------ PoolNet
 // r_t = sum_{s<t} e_s / (sum_{s<t} [e_s != 0] + 1)      representations.py:91-114
 // One CTA per sequence; warp w owns time chunk [w*ch, (w+1)*ch).
-template <int NCH>
+template <int NCH, bool BYPOS>
 __global__ void __launch_bounds__(SQ_THREADS)
 pool_rep_kernel(const float* __restrict__ E, const int64_t* __restrict__ seqs, int S, int D,
                 int64_t I, float* __restrict__ rep) {
@@ -110,7 +145,7 @@ pool_rep_kernel(const float* __restrict__ E, const int64_t* __restrict__ seqs, i
 #pragma unroll
     for (int q = 0; q < NCH; ++q) { sum[q] = make_float4(0, 0, 0, 0); cnt[q] = make_float4(0, 0, 0, 0); }
     for (int t = lo; t < hi; ++t) {
-        const float* row = E + clamp_id(sq[t], I) * D;
+        const float* row = in_row<BYPOS>(E, sq, b, t, S, D, I);
 #pragma unroll
         for (int q = 0; q < NCH; ++q) {
             const int c = lane * 4 + q * 128;
@@ -141,7 +176,7 @@ pool_rep_kernel(const float* __restrict__ E, const int64_t* __restrict__ seqs, i
     }
     float* out = rep + static_cast<int64_t>(b) * (S + 1) * D;
     for (int t = lo; t < hi; ++t) {
-        const float* row = E + clamp_id(sq[t], I) * D;
+        const float* row = in_row<BYPOS>(E, sq, b, t, S, D, I);
 #pragma unroll
         for (int q = 0; q < NCH; ++q) {
             const int c = lane * 4 + q * 128;
@@ -169,7 +204,7 @@ pool_rep_kernel(const float* __restrict__ E, const int64_t* __restrict__ seqs, i
 
 // d e_s (input role) = sum_{t>s} dR_t / (c_t + 1), added onto the seq-role
 // contribution rows C[b, s].   Same chunking as the forward.
-template <int NCH>
+template <int NCH, bool BYPOS>
 __global__ void __launch_bounds__(SQ_THREADS)
 pool_bwd_kernel(const float* __restrict__ E, const int64_t* __restrict__ seqs, int S, int D,
                 int64_t I, const float* __restrict__ dR, float* __restrict__ C) {
@@ -185,7 +220,7 @@ pool_bwd_kernel(const float* __restrict__ E, const int64_t* __restrict__ seqs, i
 #pragma unroll
     for (int q = 0; q < NCH; ++q) cnt[q] = make_float4(0, 0, 0, 0);
     for (int t = lo; t < hi; ++t) {
-        const float* row = E + clamp_id(sq[t], I) * D;
+        const float* row = in_row<BYPOS>(E, sq, b, t, S, D, I);
 #pragma unroll
         for (int q = 0; q < NCH; ++q) {
             const int c = lane * 4 + q * 128;
@@ -227,7 +262,7 @@ pool_bwd_kernel(const float* __restrict__ E, const int64_t* __restrict__ seqs, i
                 }
         }
         for (int t = hi - 1; t >= lo; --t) {
-            const float* row = E + clamp_id(sq[t], I) * D;
+            const float* row = in_row<BYPOS>(E, sq, b, t, S, D, I);
 #pragma unroll
             for (int q = 0; q < NCH; ++q) {
                 const int c = lane * 4 + q * 128;
@@ -297,9 +332,45 @@ __device__ __forceinline__ void seq_loss_fold(const SeqDev& a, float lsum, float
     }
 }
 
-template <int LPR>
+// Backward keys of one position's terms.  Plain table: the seq-role term pidx and the credited
+// negative's term BS + pidx are keyed by item id (row 0 frozen).  Hashed table (H > 0), one
+// segment index over two key spaces: [0, Mrows) table rows, term m = t * H + k for hash k of
+// term t's id (a key on the frozen row 0 dropped); [Mrows, Mrows + I) bias ids, term 2 * BS * H + t,
+// keyed as the plain table keys its rows.
+template <bool HASHED>
+__device__ __forceinline__ void seq_keys(const SeqDev& a, int64_t BS, int64_t pidx, int64_t id, int64_t nid,
+                                         float gn) {
+    const bool ks = id != 0, kn = nid != 0 && gn != 0.f;
+    if (!HASHED) {
+        a.keys[pidx] = ks ? static_cast<int32_t>(id) : -1;
+        a.keys[BS + pidx] = kn ? static_cast<int32_t>(nid) : -1;
+        if (ks) atomicAdd(a.seg.cnt + id, 1);
+        if (kn) atomicAdd(a.seg.cnt + nid, 1);
+        return;
+    }
+    const int H = a.H;
+#pragma unroll
+    for (int k = 0; k < 24; ++k) {          // static seed indices, as item4
+        if (k < H) {
+            const int64_t rs = bloom_row(id, a.seeds[k], a.Mrows, 0);
+            const int64_t rn = kn ? bloom_row(nid, a.seeds[k], a.Mrows, 0) : 0;
+            a.keys[pidx * H + k] = rs != 0 ? static_cast<int32_t>(rs) : -1;
+            a.keys[(BS + pidx) * H + k] = rn != 0 ? static_cast<int32_t>(rn) : -1;
+            if (rs != 0) atomicAdd(a.seg.cnt + rs, 1);
+            if (rn != 0) atomicAdd(a.seg.cnt + rn, 1);
+        }
+    }
+    const int64_t TH = 2 * BS * H;
+    a.keys[TH + pidx] = ks ? static_cast<int32_t>(a.Mrows + id) : -1;
+    a.keys[TH + BS + pidx] = kn ? static_cast<int32_t>(a.Mrows + nid) : -1;
+    if (ks) atomicAdd(a.seg.cnt + a.Mrows + id, 1);
+    if (kn) atomicAdd(a.seg.cnt + a.Mrows + nid, 1);
+}
+
+template <int LPR, bool HASHED>
 __global__ void __launch_bounds__(SQ_THREADS) seq_score_kernel(SeqDev a) {
     constexpr int GROUPS = SQ_THREADS / LPR;
+    if (HASHED && blockIdx.x == 0 && threadIdx.x == 0) a.seg.totals[3] = 0;   // hot-row list of this step
     const int gl = threadIdx.x & (LPR - 1);
     const unsigned gmask = group_mask(LPR);
     const int D = a.D, S = a.S, T = a.T;
@@ -324,7 +395,8 @@ __global__ void __launch_bounds__(SQ_THREADS) seq_score_kernel(SeqDev a) {
         const int64_t pidx = b * S + t;
         const int64_t id = clamp_id(a.seqs[pidx], a.I);
         const float* r = a.rep + mm * D;
-        const float* et = a.E + id * D;
+        // the target is the input item of position t: its summed row is Xs[b, t] on a hashed table
+        const float* et = HASHED ? a.Xs + pidx * D : a.E + id * D;
         float dp = 0.f;
         for (int c = gl * 4; c < D; c += LPR * 4) dp += dot4(ld4(r + c), ldg4(et + c));
         const float p = group_sum<LPR>(dp, gmask) + __ldg(a.bias + id);
@@ -335,7 +407,8 @@ __global__ void __launch_bounds__(SQ_THREADS) seq_score_kernel(SeqDev a) {
             const int64_t j = clamp_id(a.negs[nidx], a.I);
             const float* en = a.E + j * D;
             float dn = 0.f;
-            for (int c = gl * 4; c < D; c += LPR * 4) dn += dot4(ld4(r + c), ldg4(en + c));
+            for (int c = gl * 4; c < D; c += LPR * 4)
+                dn += dot4(ld4(r + c), HASHED ? item4<true>(a, j, c) : ldg4(en + c));
             const float nk = group_sum<LPR>(dn, gmask) + __ldg(a.bias + j);
             if (valid && gl == 0 && a.neg_out) a.neg_out[nidx] = nk;
             if (k == 0 || nk > nbest) { nbest = nk; nid = j; }
@@ -350,7 +423,7 @@ __global__ void __launch_bounds__(SQ_THREADS) seq_score_kernel(SeqDev a) {
         float* cs = a.C + pidx * D;
         float* cn = a.C + (BS + pidx) * D;
         for (int c = gl * 4; c < D; c += LPR * 4) {
-            const float4 rv = ld4(r + c), ev = ldg4(et + c), nv = ldg4(en + c);
+            const float4 rv = ld4(r + c), ev = ldg4(et + c), nv = HASHED ? item4<true>(a, nid, c) : ldg4(en + c);
             st4(drow + c, make_float4(gp * ev.x + gn * nv.x, gp * ev.y + gn * nv.y,
                                       gp * ev.z + gn * nv.z, gp * ev.w + gn * nv.w));
             st4(cs + c, make_float4(gp * rv.x, gp * rv.y, gp * rv.z, gp * rv.w));
@@ -359,12 +432,8 @@ __global__ void __launch_bounds__(SQ_THREADS) seq_score_kernel(SeqDev a) {
         if (gl == 0) {
             if (a.pos_out) a.pos_out[pidx] = p;
             // rows of the padding id are frozen (padding_idx=0): drop their terms
-            const bool ks = id != 0, kn = nid != 0 && gn != 0.f;
-            a.keys[pidx] = ks ? static_cast<int32_t>(id) : -1;
-            a.keys[BS + pidx] = kn ? static_cast<int32_t>(nid) : -1;
+            seq_keys<HASHED>(a, BS, pidx, id, nid, gn);
             a.gs[pidx] = gp; a.gs[BS + pidx] = gn;
-            if (ks) atomicAdd(a.seg.cnt + id, 1);
-            if (kn) atomicAdd(a.seg.cnt + nid, 1);
         }
     }
     seq_loss_fold(a, lsum, msum);
@@ -372,7 +441,7 @@ __global__ void __launch_bounds__(SQ_THREADS) seq_score_kernel(SeqDev a) {
 
 __global__ void __launch_bounds__(256) seq_fill_kernel(SeqDev a) {
     seg_rearm(a.seg);
-    const int64_t T2 = 2 * a.B * a.S;
+    const int64_t T2 = 2 * a.B * a.S * (a.H + 1);      // keys of the step (plain: H = 0)
     const int64_t nth = static_cast<int64_t>(gridDim.x) * blockDim.x;
     for (int64_t t = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x; t < T2; t += nth) {
         const int32_t k = a.keys[t];
@@ -387,7 +456,11 @@ __global__ void __launch_bounds__(256) seq_fill_kernel(SeqDev a) {
 // (mf_v2.cuh user_member / user_finish) extended by the input role, whose gradient reaches a
 // row through later positions' scores.  With weight decay an updated row is decayed in every
 // element, including those whose gradient is zero.
-template <int LPR>
+// Hashed table (H > 0): a table-row segment sums C[m / H] over its terms m (a row named by two
+// hashes of one id takes the term twice) and owns no bias; a bias segment (row >= Mrows) sums
+// gs[m - 2 BS H] and, fused, updates the bias of id row - Mrows when one of its terms has a
+// non-zero score gradient (the MF Bloom rule).  Hot rows were pre-sorted by seg_sort_long_kernel.
+template <int LPR, bool HASHED>
 __global__ void __launch_bounds__(SQ_THREADS) seq_reduce_kernel(SeqDev a) {
     constexpr int GROUPS = SQ_THREADS / LPR;
     constexpr int CAP = seg_sort_cap(LPR);
@@ -398,38 +471,56 @@ __global__ void __launch_bounds__(SQ_THREADS) seq_reduce_kernel(SeqDev a) {
     const unsigned gmask = group_mask(LPR);
     int32_t* sh = sh_sort + gib * 2 * CAP;
     const int D = a.D;
+    const int H = HASHED ? a.H : 0;
+    const int64_t TH = 2 * a.B * a.S * H;    // first bias term of a hashed step
     const int nseg = a.seg.totals[0];
     for (int64_t s = static_cast<int64_t>(blockIdx.x) * GROUPS + gib; s < nseg;
          s += static_cast<int64_t>(gridDim.x) * GROUPS) {
         const int start = a.seg.seg_start[s];
         const int len = a.seg.seg_start[s + 1] - start;
         const int64_t row = a.seg.seg_row[s];
+        const bool bseg = H > 0 && row >= a.Mrows;    // a bias segment of a hashed step (group-uniform)
         float4 acc[NCH];
 #pragma unroll
         for (int q = 0; q < NCH; ++q) acc[q] = make_float4(0, 0, 0, 0);
         float bacc = 0.f;
         bool nz = false;                     // a term with a non-zero score gradient (group-uniform)
-        seg_visit_sorted<LPR>(a.seg.members, start, len, gl, gmask, sh, [&](int32_t t) {
-            const float* src = a.C + static_cast<int64_t>(t) * D;
+        seg_visit_sorted<LPR>(a.seg.members, start, len, gl, gmask, sh, [&](int32_t m) {
+            const int64_t t = H == 0 ? m : (bseg ? m - TH : m / H);
+            if (!bseg) {
+                const float* src = a.C + t * D;
 #pragma unroll
-            for (int q = 0; q < NCH; ++q) {
-                const int c = gl * 4 + q * LPR * 4;
-                if (c < D) {
-                    const float4 v = ld4(src + c);
-                    acc[q].x += v.x; acc[q].y += v.y; acc[q].z += v.z; acc[q].w += v.w;
+                for (int q = 0; q < NCH; ++q) {
+                    const int c = gl * 4 + q * LPR * 4;
+                    if (c < D) {
+                        const float4 v = ld4(src + c);
+                        acc[q].x += v.x; acc[q].y += v.y; acc[q].z += v.z; acc[q].w += v.w;
+                    }
                 }
             }
             const float g = a.gs[t];
             bacc += g;
             nz = nz || g != 0.f;
-        });
+        }, HASHED);
+        if (bseg) {
+            if (gl == 0) {
+                if (a.opt == SLB_OPT_NONE) {
+                    a.dbias[row - a.Mrows] = bacc;
+                } else if (nz) {
+                    const OptV2 o = {a.opt, a.lr, a.wd, a.eps};
+                    bias_update(o, const_cast<float*>(a.bias) + (row - a.Mrows),
+                                a.opt == SLB_OPT_ADAGRAD ? a.sbias + (row - a.Mrows) : nullptr, bacc);
+                }
+            }
+            continue;
+        }
         if (a.opt == SLB_OPT_NONE) {
 #pragma unroll
             for (int q = 0; q < NCH; ++q) {
                 const int c = gl * 4 + q * LPR * 4;
                 if (c < D) st4(a.dE + row * D + c, acc[q]);
             }
-            if (gl == 0) a.dbias[row] = bacc;
+            if (gl == 0 && H == 0) a.dbias[row] = bacc;
             continue;
         }
 #pragma unroll
@@ -452,7 +543,7 @@ __global__ void __launch_bounds__(SQ_THREADS) seq_reduce_kernel(SeqDev a) {
                 if (srow) st4(srow, s4);
             }
         }
-        if (gl == 0)
+        if (gl == 0 && H == 0)
             bias_update(o, const_cast<float*>(a.bias) + row, a.opt == SLB_OPT_ADAGRAD ? a.sbias + row : nullptr, bacc);
     }
 }
@@ -736,6 +827,21 @@ seq_gather_kernel(const float* __restrict__ E, const int64_t* __restrict__ seqs,
     }
 }
 
+// Xs[b, t, :] = sum_k E[bloom(seq[b, t], k)]: a hashed table's input rows, summed once per step
+// and then read by position (the representation's X0 and the target rows of the scores).
+template <int LPR>
+__global__ void __launch_bounds__(SQ_THREADS) seq_gather_hashed_kernel(SeqDev a, float* __restrict__ X) {
+    constexpr int GROUPS = SQ_THREADS / LPR;
+    const int gl = threadIdx.x & (LPR - 1);
+    const int D = a.D;
+    const int64_t n = a.B * a.S;
+    for (int64_t p = static_cast<int64_t>(blockIdx.x) * GROUPS + threadIdx.x / LPR; p < n;
+         p += static_cast<int64_t>(gridDim.x) * GROUPS) {
+        const int64_t id = clamp_id(a.seqs[p], a.I);
+        for (int c = gl * 4; c < D; c += LPR * 4) st4(X + p * D + c, item4<true>(a, id, c));
+    }
+}
+
 // ------------------------------------------------------------------ host side
 struct SeqLayout {
     int32_t* hdr; float* partial; SegIndex seg;
@@ -788,10 +894,13 @@ SeqLayout seq_layout(void* base, const slb_seq_step_args* x, bool training) {
     SeqLayout l = {};
     const int64_t B = x->batch, S = x->seq_len, T = S + 1, D = x->dim;
     const int L = x->n_layers;
-    // zero-at-rest region first (offsets depend on num_items only)
+    const int64_t H = x->item_hashes;
+    // zero-at-rest region first (offsets depend on the key space only: num_items, plus item_rows
+    // on a hashed table)
     l.hdr = ws.take<int32_t>(16);
-    l.seg = seg_index_carve(ws, x->num_items, training ? 2 * B * S : 1);
+    l.seg = seg_index_carve(ws, H ? x->item_rows + x->num_items : x->num_items, training ? 2 * B * S * (H + 1) : 1);
     l.partial = ws.take<float>(SQ_MAX_GRID);
+    if (H && !x->lstm_w_ih && L == 0) l.X0 = ws.take<float>(B * S * D);   // PoolNet's summed input rows
     if (x->lstm_w_ih) {
         l.rep_pool = ws.take<float>(B * T * D);          // h_t
         l.X0 = ws.take<float>(B * S * D);
@@ -840,11 +949,15 @@ SeqLayout seq_layout(void* base, const slb_seq_step_args* x, bool training) {
     if (training) {
         l.dR = ws.take<float>(B * T * D);
         l.C = ws.take<float>(2 * B * S * D);
-        l.keys = ws.take<int32_t>(2 * B * S);
+        l.keys = ws.take<int32_t>(2 * B * S * (H + 1));
         l.gs = ws.take<float>(2 * B * S);
     }
     l.bytes = ws.bytes();
     return l;
+}
+
+int64_t seq_hashed_terms(const slb_seq_step_args* x) {
+    return 2 * x->batch * static_cast<int64_t>(x->seq_len) * (x->item_hashes + 1);
 }
 
 int seq_validate(const slb_seq_step_args* x, bool training) {
@@ -875,6 +988,16 @@ int seq_validate(const slb_seq_step_args* x, bool training) {
                     "seq: num_mixtures must be in [1, %d] (got %d)", mix::MAX_M, x->num_mixtures);
         SLB_REQUIRE(x->mix_b != nullptr, "seq: mixture projection bias missing");
         if (training) SLB_REQUIRE(x->dmix_w && x->dmix_b, "seq: mixture projection grads missing");
+    }
+    SLB_REQUIRE(x->item_hashes >= 0 && x->item_hashes <= 24, "seq: item_hashes must be in [0, 24] (got %d)", x->item_hashes);
+    if (x->item_hashes > 0) {
+        SLB_REQUIRE(x->item_rows > 0 && x->item_rows + x->num_items < (1ll << 31) - SEG_SCAN_TILE,
+                    "seq: hashed table needs 0 < item_rows, item_rows + num_items < 2^31 - %d", SEG_SCAN_TILE);
+        SLB_REQUIRE(x->item_padding_idx == 0, "seq: a hashed item table's padding_idx must be 0 (PADDING_IDX)");
+        if (training)
+            SLB_REQUIRE(seq_hashed_terms(x) < (1ll << 31),
+                        "seq: 2 * batch * seq_len * (item_hashes + 1) = %lld gradient terms, must stay below 2^31",
+                        static_cast<long long>(seq_hashed_terms(x)));
     }
     if (training) {
         SLB_REQUIRE(x->negs && x->bias && x->loss_out, "seq: null pointer");
@@ -912,10 +1035,55 @@ int lpr_of(int D) {
         default: KERNEL<32><<<grid, SQ_THREADS, 0, stream>>>(__VA_ARGS__); break;        \
     }
 
-#define SQ_DISPATCH_NCH(D, KERNEL, grid, smem, stream, ...)                              \
-    if ((D) <= 128) KERNEL<1><<<grid, SQ_THREADS, smem, stream>>>(__VA_ARGS__);          \
-    else if ((D) <= 256) KERNEL<2><<<grid, SQ_THREADS, smem, stream>>>(__VA_ARGS__);     \
-    else KERNEL<4><<<grid, SQ_THREADS, smem, stream>>>(__VA_ARGS__);
+// row-source variants: HASHED is a compile-time bool of the kernel
+#define SQ_DISPATCH_LPR_T(lpr, KERNEL, HASHED, grid, stream, ...)                        \
+    switch (lpr) {                                                                       \
+        case 1: KERNEL<1, HASHED><<<grid, SQ_THREADS, 0, stream>>>(__VA_ARGS__); break;  \
+        case 2: KERNEL<2, HASHED><<<grid, SQ_THREADS, 0, stream>>>(__VA_ARGS__); break;  \
+        case 4: KERNEL<4, HASHED><<<grid, SQ_THREADS, 0, stream>>>(__VA_ARGS__); break;  \
+        case 8: KERNEL<8, HASHED><<<grid, SQ_THREADS, 0, stream>>>(__VA_ARGS__); break;  \
+        case 16: KERNEL<16, HASHED><<<grid, SQ_THREADS, 0, stream>>>(__VA_ARGS__); break; \
+        default: KERNEL<32, HASHED><<<grid, SQ_THREADS, 0, stream>>>(__VA_ARGS__); break; \
+    }
+
+#define SQ_DISPATCH_LPR_ROWS(hashed, lpr, KERNEL, grid, stream, ...)                     \
+    if (hashed) { SQ_DISPATCH_LPR_T(lpr, KERNEL, true, grid, stream, __VA_ARGS__) }      \
+    else { SQ_DISPATCH_LPR_T(lpr, KERNEL, false, grid, stream, __VA_ARGS__) }
+
+#define SQ_DISPATCH_NCH_T(D, KERNEL, BYPOS, grid, smem, stream, ...)                     \
+    if ((D) <= 128) KERNEL<1, BYPOS><<<grid, SQ_THREADS, smem, stream>>>(__VA_ARGS__);   \
+    else if ((D) <= 256) KERNEL<2, BYPOS><<<grid, SQ_THREADS, smem, stream>>>(__VA_ARGS__); \
+    else KERNEL<4, BYPOS><<<grid, SQ_THREADS, smem, stream>>>(__VA_ARGS__);
+
+#define SQ_DISPATCH_NCH(D, KERNEL, bypos, grid, smem, stream, ...)                       \
+    if (bypos) { SQ_DISPATCH_NCH_T(D, KERNEL, true, grid, smem, stream, __VA_ARGS__) }   \
+    else { SQ_DISPATCH_NCH_T(D, KERNEL, false, grid, smem, stream, __VA_ARGS__) }
+
+// The item-table part of the device arguments: E, its shape and, on a hashed table, the hashes.
+SeqDev seq_dev_table(const slb_seq_step_args* x) {
+    SeqDev a = {};
+    a.B = x->batch; a.S = x->seq_len; a.T = x->seq_len + 1; a.I = x->num_items; a.D = x->dim;
+    a.seqs = x->seqs; a.E = x->E;
+    a.H = x->item_hashes;
+    a.Mrows = a.H ? x->item_rows : x->num_items;
+    for (int k = 0; k < 24; ++k) a.seeds[k] = x->item_seeds[k];
+    return a;
+}
+
+// X0 = the input rows of every position: E[seq], or the hashed sums
+int launch_gather(const slb_seq_step_args* x, const SeqLayout& l, cudaStream_t st) {
+    const int64_t n = x->batch * x->seq_len;
+    const int lpr = lpr_of(x->dim);
+    const int grid = sq_grid((n + SQ_THREADS / lpr - 1) / (SQ_THREADS / lpr));
+    if (x->item_hashes) {
+        SQ_DISPATCH_LPR(lpr, seq_gather_hashed_kernel, grid, st, seq_dev_table(x), l.X0);
+        SLB_LAUNCH_CHECK("seq_gather_hashed_kernel");
+    } else {
+        SQ_DISPATCH_LPR(lpr, seq_gather_kernel, grid, st, x->E, x->seqs, n, x->dim, x->num_items, l.X0);
+        SLB_LAUNCH_CHECK("seq_gather_kernel");
+    }
+    return SLB_OK;
+}
 
 void conv_shifts(const slb_seq_step_args* x, int layer, int* shift, int* Tin) {
     const int k = x->kernel_width[layer], d = x->dilation[layer];
@@ -1028,10 +1196,8 @@ int run_lstm_forward(const slb_seq_step_args* x, const SeqLayout& l, float* H, c
     const int64_t B = x->batch;
     const int S = x->seq_len, T = S + 1, D = x->dim;
     const int64_t BTD = B * T * D, DD = static_cast<int64_t>(D) * D;
-    const int lpr = lpr_of(D);
-    SQ_DISPATCH_LPR(lpr, seq_gather_kernel, sq_grid((B * S + SQ_THREADS / lpr - 1) / (SQ_THREADS / lpr)), st,
-                    x->E, x->seqs, B * S, D, x->num_items, l.X0);
-    SLB_LAUNCH_CHECK("seq_gather_kernel");
+    const int grc = launch_gather(x, l, st);
+    if (grc != SLB_OK) return grc;
     for (int g = 0; g < 4; ++g) {
         conv_wt_kernel<<<sq_grid((DD + 255) / 256), 256, 0, st>>>(x->lstm_w_ih + g * DD, 1, D, l.WT + g * DD, nullptr);
         SLB_LAUNCH_CHECK("conv_wt_kernel(lstm)");
@@ -1139,15 +1305,19 @@ int run_representation(const slb_seq_step_args* x, const SeqLayout& l, float* re
     if (x->n_layers == 0) {
         float* rep = rep_dst ? rep_dst : l.rep_pool;
         const size_t smem = static_cast<size_t>(16) * D * sizeof(float);
-        SQ_DISPATCH_NCH(D, pool_rep_kernel, static_cast<unsigned>(B), smem, st, x->E, x->seqs, S, D, x->num_items, rep);
+        const bool hashed = x->item_hashes != 0;
+        if (hashed) {
+            const int grc = launch_gather(x, l, st);
+            if (grc != SLB_OK) return grc;
+        }
+        SQ_DISPATCH_NCH(D, pool_rep_kernel, hashed, static_cast<unsigned>(B), smem, st, hashed ? l.X0 : x->E,
+                        x->seqs, S, D, x->num_items, rep);
         SLB_LAUNCH_CHECK("pool_rep_kernel");
         *rep_out = rep;
         return SLB_OK;
     }
-    const int lpr = lpr_of(D);
-    SQ_DISPATCH_LPR(lpr, seq_gather_kernel, sq_grid((B * S + SQ_THREADS / lpr - 1) / (SQ_THREADS / lpr)), st,
-                    x->E, x->seqs, B * S, D, x->num_items, l.X0);
-    SLB_LAUNCH_CHECK("seq_gather_kernel");
+    const int grc = launch_gather(x, l, st);
+    if (grc != SLB_OK) return grc;
     for (int i = 0; i < x->n_layers; ++i) {
         const int k = x->kernel_width[i];
         conv_wt_kernel<<<sq_grid((static_cast<int64_t>(k) * D * D + 255) / 256), 256, 0, st>>>(
@@ -1181,6 +1351,7 @@ size_t slb_seq_step_workspace_bytes(const slb_seq_step_args* x) {
     if (!x || x->batch <= 0 || x->seq_len <= 0 || x->dim <= 0) return 0;
     if (x->n_layers > 0 && !x->kernel_width) return 0;
     if (x->mix_w && (x->num_mixtures < 1 || x->num_mixtures > mix::MAX_M)) return 0;
+    if (x->item_hashes > 0 && seq_hashed_terms(x) >= (1ll << 31)) return 0;      // the step rejects it
     return seq_layout(nullptr, x, x->negs != nullptr || x->loss_out != nullptr).bytes;
 }
 
@@ -1218,22 +1389,24 @@ int slb_seq_train_step(const slb_seq_step_args* x, slb_stream_t stream) {
     rc = run_representation(x, l, nullptr, st, &rep);
     if (rc != SLB_OK) return rc;
 
-    SeqDev a = {};
-    a.B = B; a.S = S; a.T = T; a.I = x->num_items; a.D = D;
-    a.seqs = x->seqs; a.negs = x->negs; a.loss = x->loss; a.n_neg = x->n_neg;
-    a.E = x->E; a.bias = x->bias; a.rep = rep; a.dR = l.dR; a.C = l.C; a.keys = l.keys; a.gs = l.gs;
+    const bool hashed = x->item_hashes != 0;
+    SeqDev a = seq_dev_table(x);
+    a.negs = x->negs; a.loss = x->loss; a.n_neg = x->n_neg; a.Xs = l.X0;
+    a.bias = x->bias; a.rep = rep; a.dR = l.dR; a.C = l.C; a.keys = l.keys; a.gs = l.gs;
     a.hdr = l.hdr; a.partial = l.partial; a.norm = x->norm_count;
     a.loss_out = x->loss_out; a.pos_out = x->pos_out; a.neg_out = x->neg_out;
     a.dE = x->dE; a.dbias = x->dbias; a.seg = l.seg;
+    // hashed rows are hot at small item_rows: sort their member lists with seg_sort_long_kernel
+    if (hashed) a.seg.long_cap = seg_sort_cap(lpr);
     a.opt = x->opt; a.lr = x->lr; a.wd = x->weight_decay; a.eps = x->eps; a.sE = x->state_E; a.sbias = x->state_bias;
     if (x->mix_w) {
         a.M = x->num_mixtures; a.P = l.P;
-        SQ_DISPATCH_LPR(lpr, mix::mix_score_kernel, sq_grid((B * T + groups - 1) / groups), st, a);
+        SQ_DISPATCH_LPR_ROWS(hashed, lpr, mix::mix_score_kernel, sq_grid((B * T + groups - 1) / groups), st, a);
         SLB_LAUNCH_CHECK("mix_score_kernel");
         rc = run_mix_backward(x, l, st);
         if (rc != SLB_OK) return rc;
     } else {
-        SQ_DISPATCH_LPR(lpr, seq_score_kernel, sq_grid((B * T + groups - 1) / groups), st, a);
+        SQ_DISPATCH_LPR_ROWS(hashed, lpr, seq_score_kernel, sq_grid((B * T + groups - 1) / groups), st, a);
         SLB_LAUNCH_CHECK("seq_score_kernel");
     }
 
@@ -1242,7 +1415,8 @@ int slb_seq_train_step(const slb_seq_step_args* x, slb_stream_t stream) {
         if (rc != SLB_OK) return rc;
     } else if (x->n_layers == 0) {
         const size_t smem = static_cast<size_t>(16) * D * sizeof(float);
-        SQ_DISPATCH_NCH(D, pool_bwd_kernel, static_cast<unsigned>(B), smem, st, x->E, x->seqs, S, D, x->num_items, l.dR, l.C);
+        SQ_DISPATCH_NCH(D, pool_bwd_kernel, hashed, static_cast<unsigned>(B), smem, st, hashed ? l.X0 : x->E,
+                        x->seqs, S, D, x->num_items, l.dR, l.C);
         SLB_LAUNCH_CHECK("pool_bwd_kernel");
     } else {
         const float* dY = l.dR;
@@ -1277,9 +1451,14 @@ int slb_seq_train_step(const slb_seq_step_args* x, slb_stream_t stream) {
     }
     seg_scan_launch(a.seg, a.seg.Rpad, st);
     SLB_LAUNCH_CHECK("seg_scan_kernel");
-    seq_fill_kernel<<<sq_grid((2 * B * S + 255) / 256), 256, 0, st>>>(a);
+    const int64_t nkeys = 2 * B * S * (a.H + 1);
+    seq_fill_kernel<<<sq_grid((nkeys + 255) / 256), 256, 0, st>>>(a);
     SLB_LAUNCH_CHECK("seq_fill_kernel");
-    SQ_DISPATCH_LPR(lpr, seq_reduce_kernel, sq_grid((2 * B * S + groups - 1) / groups), st, a);
+    if (hashed) {
+        seg_sort_long_kernel<<<SEG_LONG_CTAS, 256, 0, st>>>(a.seg);     // no-op unless hot rows exist
+        SLB_LAUNCH_CHECK("seg_sort_long_kernel");
+    }
+    SQ_DISPATCH_LPR_ROWS(hashed, lpr, seq_reduce_kernel, sq_grid((nkeys + groups - 1) / groups), st, a);
     SLB_LAUNCH_CHECK("seq_reduce_kernel");
     return SLB_OK;
 }

@@ -21,17 +21,18 @@ namespace mix {
 
 constexpr int MAX_M = 8;         // logits and scores of a position stay in registers
 
-// Scores one item row e against the position whose 2M rows start at p (row j at p + j * BTD):
-// returns beta + s_bar and leaves the softmax weights w, the taste scores z and s_bar.
-template <int LPR>
-__device__ __forceinline__ float mix_item(const float* p, int64_t BTD, int M, int D, const float* __restrict__ e,
+// Scores one item row against the position whose 2M rows start at p (row j at p + j * BTD):
+// returns beta + s_bar and leaves the softmax weights w, the taste scores z and s_bar.  e(c) is
+// the row's float4 at channel c (the row source: a table row, or a hashed item's summed rows).
+template <int LPR, typename Row>
+__device__ __forceinline__ float mix_item(const float* p, int64_t BTD, int M, int D, Row e,
                                           float beta, int gl, unsigned gmask, float (&w)[MAX_M], float (&z)[MAX_M],
                                           float& sbar) {
     float av[MAX_M];
 #pragma unroll
     for (int m = 0; m < MAX_M; ++m) { av[m] = 0.f; z[m] = 0.f; }
     for (int c = gl * 4; c < D; c += LPR * 4) {
-        const float4 ev = ldg4(e + c);
+        const float4 ev = e(c);
 #pragma unroll
         for (int m = 0; m < MAX_M; ++m)
             if (m < M) {
@@ -62,9 +63,10 @@ __device__ __forceinline__ float mix_item(const float* p, int64_t BTD, int M, in
     return beta + sbar;
 }
 
-template <int LPR>
+template <int LPR, bool HASHED>
 __global__ void __launch_bounds__(SQ_THREADS) mix_score_kernel(SeqDev a) {
     constexpr int GROUPS = SQ_THREADS / LPR;
+    if (HASHED && blockIdx.x == 0 && threadIdx.x == 0) a.seg.totals[3] = 0;   // hot-row list of this step
     const int gl = threadIdx.x & (LPR - 1);
     const unsigned gmask = group_mask(LPR);
     const int D = a.D, S = a.S, T = a.T, M = a.M;
@@ -90,9 +92,11 @@ __global__ void __launch_bounds__(SQ_THREADS) mix_score_kernel(SeqDev a) {
         }
         const int64_t pidx = b * S + t;
         const int64_t id = clamp_id(a.seqs[pidx], a.I);
-        const float* et = a.E + id * D;
+        // the target is the input item of position t: its summed row is Xs[b, t] on a hashed table
+        const float* et = HASHED ? a.Xs + pidx * D : a.E + id * D;
         float wt[MAX_M], zt[MAX_M], st;
-        const float p = mix_item<LPR>(prow, BTD, M, D, et, __ldg(a.bias + id), gl, gmask, wt, zt, st);
+        const float p = mix_item<LPR>(prow, BTD, M, D, [&](int c) { return ldg4(et + c); }, __ldg(a.bias + id), gl,
+                                      gmask, wt, zt, st);
         float nbest = -INFINITY, sn = 0.f;
         float wn[MAX_M], zn[MAX_M];
         int64_t nid = 0;
@@ -100,7 +104,8 @@ __global__ void __launch_bounds__(SQ_THREADS) mix_score_kernel(SeqDev a) {
             const int64_t nidx = (static_cast<int64_t>(k) * a.B + b) * S + t;   // implicit.py:281-286
             const int64_t j = clamp_id(a.negs[nidx], a.I);
             float wk[MAX_M], zk[MAX_M], sk;
-            const float nk = mix_item<LPR>(prow, BTD, M, D, a.E + j * D, __ldg(a.bias + j), gl, gmask, wk, zk, sk);
+            const float nk = mix_item<LPR>(prow, BTD, M, D, [&](int c) { return item4<HASHED>(a, j, c); },
+                                           __ldg(a.bias + j), gl, gmask, wk, zk, sk);
             if (valid && gl == 0 && a.neg_out) a.neg_out[nidx] = nk;
             if (k == 0 || nk > nbest) {               // the first of bit-identical maxima
                 nbest = nk; nid = j; sn = sk;
@@ -114,11 +119,10 @@ __global__ void __launch_bounds__(SQ_THREADS) mix_score_kernel(SeqDev a) {
         lsum += (valid && gl == 0) ? per * mk : 0.f;
         gp *= mk * inv; gn *= mk * inv;
         if (!valid) continue;                         // no shuffles below
-        const float* en = a.E + nid * D;
         float* cs = a.C + pidx * D;
         float* cn = a.C + (BS + pidx) * D;
         for (int c = gl * 4; c < D; c += LPR * 4) {
-            const float4 ev = ldg4(et + c), nv = ldg4(en + c);
+            const float4 ev = ldg4(et + c), nv = item4<HASHED>(a, nid, c);
             float4 dt = make_float4(0, 0, 0, 0), dn = make_float4(0, 0, 0, 0);
 #pragma unroll
             for (int q = 0; q < MAX_M; ++q)
@@ -140,13 +144,9 @@ __global__ void __launch_bounds__(SQ_THREADS) mix_score_kernel(SeqDev a) {
         }
         if (gl == 0) {
             if (a.pos_out) a.pos_out[pidx] = p;
-            // rows of the padding id are frozen (padding_idx=0): drop their terms
-            const bool ks = id != 0, kn = nid != 0 && gn != 0.f;
-            a.keys[pidx] = ks ? static_cast<int32_t>(id) : -1;
-            a.keys[BS + pidx] = kn ? static_cast<int32_t>(nid) : -1;
             a.gs[pidx] = gp; a.gs[BS + pidx] = gn;
-            if (ks) atomicAdd(a.seg.cnt + id, 1);
-            if (kn) atomicAdd(a.seg.cnt + nid, 1);
+            // rows of the padding id are frozen (padding_idx=0): drop their terms
+            seq_keys<HASHED>(a, BS, pidx, id, nid, gn);
         }
     }
     seq_loss_fold(a, lsum, msum);

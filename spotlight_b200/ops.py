@@ -738,10 +738,13 @@ class _HostPtrArray(object):
         return ctypes.cast(arr, ctypes.c_void_p)
 
 
-def seq_step_args(E, bias, seqs, negs, loss, n_neg, cnn=None, keep=None, lstm=None, mixture=None):
+def seq_step_args(E, bias, seqs, negs, loss, n_neg, cnn=None, keep=None, lstm=None, mixture=None,
+                  item_hash=None, num_items=None):
     """cnn: None (PoolNet) or dict(kernel_width, dilation, nonlinearity, residual, weights, biases);
     lstm: None or dict(w_ih, w_hh, b_ih, b_hh) (LSTMNet, nn.LSTM shapes);
-    mixture: None or dict(num_mixtures, w, b) (MixtureLSTMNet's projection, with ``lstm``)."""
+    mixture: None or dict(num_mixtures, w, b) (MixtureLSTMNet's projection, with ``lstm``);
+    item_hash: None or dict(seeds, padding_idx): ``E`` is a BloomEmbedding's hashed table and
+    ``num_items`` the id space (the bias rows)."""
     keep = keep if keep is not None else _HostPtrArray()
     a = SeqStepArgs()
     a.batch, a.seq_len = int(seqs.shape[0]), int(seqs.shape[1])
@@ -751,6 +754,14 @@ def seq_step_args(E, bias, seqs, negs, loss, n_neg, cnn=None, keep=None, lstm=No
     a.n_neg = int(n_neg)
     a.num_items, a.dim = int(E.shape[0]), int(E.shape[1])
     a.E, a.bias = E.data_ptr(), bias.data_ptr()
+    if item_hash is not None:
+        seeds = list(item_hash['seeds'])
+        if not 1 <= len(seeds) <= 24:
+            raise ValueError('item_hash: 1 to 24 seeds (got %d)' % len(seeds))
+        a.num_items, a.item_rows, a.item_hashes = int(num_items), int(E.shape[0]), len(seeds)
+        for k, s in enumerate(seeds):
+            a.item_seeds[k] = int(s) & 0xFFFFFFFF
+        a.item_padding_idx = int(item_hash['padding_idx'])
     if cnn is not None:
         a.n_layers = len(cnn['weights'])
         a.kernel_width = keep.i32(cnn['kernel_width'])
@@ -794,7 +805,7 @@ def _mixture_params(mixture, lstm, D):
 
 
 def seq_train_step(E, bias, seqs, negs, loss, n_neg, cnn=None, want_scores=False, norm_count=None, fused=None,
-                   lstm=None, mixture=None):
+                   lstm=None, mixture=None, item_hash=None):
     """Fused forward + backward of one sequence minibatch, dense gradients.
 
     Returns dict(loss, pos, neg, dE, dbias, dconv_w, dconv_b, dlstm).  ``fused`` = dict(kind, lr,
@@ -803,7 +814,9 @@ def seq_train_step(E, bias, seqs, negs, loss, n_neg, cnn=None, want_scores=False
     ``lstm`` = dict(w_ih, w_hh, b_ih, b_hh) selects the LSTMNet representation; ``dlstm`` then holds
     the gradients under the same keys.  ``mixture`` = dict(num_mixtures, w (2MD, D, 1), b (2MD,)), with
     ``lstm``, adds MixtureLSTMNet's projection and mixture-of-tastes scoring; ``dmix`` = dict(w, b)
-    then holds the projection gradients in the shapes given.
+    then holds the projection gradients in the shapes given.  ``item_hash`` = dict(seeds, padding_idx)
+    makes ``E`` a ``BloomEmbedding``'s compressed (M, D) table: an item is the sum of its hashed rows,
+    ``bias`` stays (num_items, 1), and ``dE`` is (M, D).
     """
     require_cuda(E, bias, seqs, negs)
     lib = _lib.load()
@@ -817,7 +830,8 @@ def seq_train_step(E, bias, seqs, negs, loss, n_neg, cnn=None, want_scores=False
         cnn['biases'] = [_f32c(b) for b in cnn['biases']]
     lstm = _lstm_params(lstm)
     mix = _mixture_params(mixture, lstm, int(E.shape[1]))
-    a, keep = seq_step_args(E, bias, seqs, negs, loss, n_neg, cnn, lstm=lstm, mixture=mix)
+    a, keep = seq_step_args(E, bias, seqs, negs, loss, n_neg, cnn, lstm=lstm, mixture=mix, item_hash=item_hash,
+                            num_items=bias.shape[0])
     out = dict(loss=torch.empty(1, dtype=torch.float32, device=dev), dE=None, dbias=None, dconv_w=[], dconv_b=[],
                dlstm=None, dmix=None)
     if fused is None:
@@ -849,7 +863,9 @@ def seq_train_step(E, bias, seqs, negs, loss, n_neg, cnn=None, want_scores=False
                            b=torch.zeros_like(mix['b']))
         a.dmix_w, a.dmix_b = out['dmix']['w'].data_ptr(), out['dmix']['b'].data_ptr()
     need = lib.slb_seq_step_workspace_bytes(ctypes.byref(a))
-    ws = workspace('seq%d' % a.num_items, need, dev)
+    # the zero-at-rest counters sit at offsets set by the key space: a hashed table has its own
+    kind = 'seq%d' % a.num_items if item_hash is None else 'seqh%d_%d' % (a.num_items, a.item_rows)
+    ws = workspace(kind, need, dev)
     a.workspace, a.workspace_bytes = ws.data_ptr(), ws.numel()
     _lib.check(lib.slb_seq_train_step(ctypes.byref(a), _stream()), 'seq_train_step')
     out['loss'] = out['loss'].reshape(())

@@ -9,8 +9,13 @@
            whole backward (deterministic segmented scatter into the embedding
            gradient); the gradients are handed to whatever ``torch.optim``
            optimizer the model holds.
-  generic  any other representation (Bloom-embedded, custom): the
-           reference's loop shape over this package's gather and loss ops.
+  fused_hashed
+           the same four nets on a ``BloomEmbedding(padding_idx=0)`` item layer (dense table,
+           within each net's fused limits) trained with ``optim.fused_sgd`` / ``fused_adagrad``:
+           the same C call, with items summed from their hashed rows, and the compressed
+           table and the biases updated in place by the row-wise optimizer.
+  generic  any other representation (custom, Bloom-embedded under a ``torch.optim``
+           optimizer): the reference's loop shape over this package's gather and loss ops.
 """
 
 import numpy as np
@@ -108,8 +113,13 @@ class ImplicitSequenceModel(object):
 
     def _route(self):
         net = self._net
-        if isinstance(net, (PoolNet, CNNNet, LSTMNet, MixtureLSTMNet)) and net.fusable() and not self._sparse:
-            return 'fused'
+        if isinstance(net, (PoolNet, CNNNet, LSTMNet, MixtureLSTMNet)) and not self._sparse:
+            if net.fusable():
+                return 'fused'
+            # a hashed table has no dense gradient to hand to torch.optim: row-wise optimizers only
+            if net.hashed_spec() is not None and \
+                    getattr(self._optimizer, 'fused_kind', None) in (_lib.OPT_SGD, _lib.OPT_ADAGRAD):
+                return 'fused_hashed'
         return 'generic'
 
     def fit(self, interactions, verbose=False):
@@ -159,7 +169,7 @@ class ImplicitSequenceModel(object):
                 batch_neg = negatives[lo * n_neg:(lo + B) * n_neg]      # rows k*B + b
                 lo += B
                 self._optimizer.zero_grad()
-                if route == 'fused':
+                if route in ('fused', 'fused_hashed'):
                     loss = self._fused_step(batch_sequence, batch_neg, n_neg)
                 else:
                     loss = self._generic_step(batch_sequence, batch_neg, n_neg)
@@ -183,19 +193,21 @@ class ImplicitSequenceModel(object):
         fused = None
         opt = self._optimizer
         kind = getattr(opt, 'fused_kind', None)
+        item_hash = net.hashed_spec()
+        table = net._item_table()
         if kind in (_lib.OPT_SGD, _lib.OPT_ADAGRAD):
             # row-wise optimizer inside the step (spotlight_b200.optim): the item table and its bias
             # are updated in place by the gradient kernel, no dense (num_items, D) gradient exists;
             # optimizer.step() below then only sees the (tiny) conv parameters
             hp = opt.fused_hparams()
             fused = dict(kind=kind, lr=hp['lr'], weight_decay=hp['weight_decay'], eps=hp['eps'],
-                         state_E=opt.fused_state(net.item_embeddings.weight),
+                         state_E=opt.fused_state(table),
                          state_bias=opt.fused_state(net.item_biases.weight))
         with torch.no_grad():
-            out = ops.seq_train_step(net.item_embeddings.weight, net.item_biases.weight,
+            out = ops.seq_train_step(table, net.item_biases.weight,
                                      batch_sequence, batch_neg, self._loss, n_neg, spec, fused=fused,
-                                     lstm=lstm, mixture=mixture)
-        net.item_embeddings.weight.grad = out['dE']
+                                     lstm=lstm, mixture=mixture, item_hash=item_hash)
+        table.grad = out['dE']
         net.item_biases.weight.grad = out['dbias']
         if spec is not None:
             for layer, dw, db in zip(net.cnn_layers, out['dconv_w'], out['dconv_b']):

@@ -13,7 +13,7 @@ import torch.nn as nn
 import torch.nn.functional as F
 
 from spotlight_b200 import ops
-from spotlight_b200.layers import ScaledEmbedding, ZeroEmbedding
+from spotlight_b200.layers import BloomEmbedding, ScaledEmbedding, ZeroEmbedding
 
 PADDING_IDX = 0
 
@@ -47,6 +47,26 @@ class _SeqNetBase(nn.Module):
         return (type(emb) is ScaledEmbedding and emb.padding_idx == PADDING_IDX and not emb.sparse
                 and emb.embedding_dim % 4 == 0 and emb.embedding_dim <= 512
                 and not self.item_biases.sparse)
+
+    def _kernel_limits(self):
+        """The representation's own limits of the fused step (dimension, layer shapes)."""
+        return self.item_embeddings.embedding_dim <= 512
+
+    def hashed_spec(self):
+        """``dict(seeds, padding_idx)`` when the item layer is a ``BloomEmbedding`` the fused sequence
+        step can train (padding id 0, dense table, ``D % 4 == 0``, within the net's kernel limits);
+        None otherwise."""
+        emb = self.item_embeddings
+        if not (isinstance(emb, BloomEmbedding) and emb.padding_idx == PADDING_IDX
+                and not emb.embeddings.sparse and emb.embedding_dim % 4 == 0 and emb.num_hash_functions >= 1
+                and emb.compressed_num_embeddings >= 1 and not self.item_biases.sparse and self._kernel_limits()):
+            return None
+        return dict(seeds=list(emb._masks), padding_idx=PADDING_IDX)
+
+    def _item_table(self):
+        """The item table the fused step trains: the plain weight, or a BloomEmbedding's compressed one."""
+        emb = self.item_embeddings
+        return emb.embeddings.weight if isinstance(emb, BloomEmbedding) else emb.weight
 
     def user_representation(self, item_sequences):
         """``(all, final)``: ``all[:, :, t]`` has seen items before ``t``
@@ -176,8 +196,10 @@ class LSTMNet(_SeqNetBase):
         self.lstm = nn.LSTM(batch_first=True, input_size=embedding_dim, hidden_size=embedding_dim)
 
     def fusable(self):
-        return (super(LSTMNet, self).fusable()
-                and self.item_embeddings.embedding_dim <= self.LSTM_MAX_DIM
+        return super(LSTMNet, self).fusable() and self._kernel_limits()
+
+    def _kernel_limits(self):
+        return (self.item_embeddings.embedding_dim <= self.LSTM_MAX_DIM
                 and self.lstm.num_layers == 1 and self.lstm.bias and not self.lstm.bidirectional)
 
     def _autograd_params(self):
@@ -224,9 +246,11 @@ class MixtureLSTMNet(_SeqNetBase):
                                     kernel_size=1)
 
     def fusable(self):
+        return super(MixtureLSTMNet, self).fusable() and self._kernel_limits()
+
+    def _kernel_limits(self):
         p = self.projection
-        return (super(MixtureLSTMNet, self).fusable()
-                and self.item_embeddings.embedding_dim <= self.LSTM_MAX_DIM
+        return (self.item_embeddings.embedding_dim <= self.LSTM_MAX_DIM
                 and 1 <= self.num_mixtures <= self.MAX_MIXTURES
                 and self.lstm.num_layers == 1 and self.lstm.bias and not self.lstm.bidirectional
                 and type(p) is nn.Conv1d and p.bias is not None and p.kernel_size == (1,)
