@@ -32,7 +32,7 @@ GEOMETRIES = [
 
 
 def lpr_of(D):
-    """Lanes per row of the sequence kernels (seq.cu lpr_of): D / 4 rounded up to a power of two, <= 32."""
+    """Lanes per row of the sequence kernels (common.cuh lpr_for_dim): D / 4 rounded up to a power of two, <= 32."""
     l, p = D // 4, 1
     if l >= 32:
         return 32

@@ -8,6 +8,6 @@ cd "$(dirname "$0")/../spotlight_b200/csrc"
 make >/dev/null
 mkdir -p ../../variants
 nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -lineinfo -Xcompiler -fPIC $flags -c mf.cu -o build/mf_$name.o
-nvcc -gencode arch=compute_90a,code=sm_90a -shared -o ../../variants/lib_$name.so \
-    build/api.o build/rng.o build/mf_$name.o build/embed.o build/loss.o build/seq.o build/shard.o build/shuffle.o build/host_shuffle.o
+objs=$(make -s print-objs)
+nvcc -gencode arch=compute_90a,code=sm_90a -shared -o ../../variants/lib_$name.so ${objs/build\/mf.o/build/mf_$name.o}
 echo "built variants/lib_$name.so"

@@ -5,6 +5,8 @@
 #include <stdint.h>
 #include <stdio.h>
 
+#include <type_traits>
+
 #include "../../include/spotlight_b200.h"
 
 void slb_set_error(const char* fmt, ...);
@@ -28,6 +30,37 @@ int slb_sms();
     } while (0)
 
 static inline size_t slb_align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
+
+// Grid of `want` blocks, at least one and at most per_sm per SM.
+static inline int slb_grid(int64_t want, int per_sm) {
+    const int64_t cap = static_cast<int64_t>(slb_sms()) * per_sm;
+    const int64_t g = want < cap ? want : cap;
+    return g < 1 ? 1 : static_cast<int>(g);
+}
+
+// Lanes per row of width D: one 128-bit piece per lane, a power of two, at most a warp.
+static inline int lpr_for_dim(int D) {
+    const int l = D / 4;
+    int p = 1;
+    while (p < l && p < 32) p <<= 1;
+    return p;
+}
+
+// Calls f(std::integral_constant<int, L>{}) for the lane count L == lpr, L a power of two from
+// FIRST to 32 (any other lpr gets 32): a launch site names its kernel once, for every L.
+template <int FIRST = 1, typename F>
+void with_lpr(int lpr, F&& f) {
+    if constexpr (FIRST == 32) f(std::integral_constant<int, 32>{});
+    else if (lpr == FIRST) f(std::integral_constant<int, FIRST>{});
+    else with_lpr<2 * FIRST>(lpr, f);
+}
+
+// f(std::true_type{}) or f(std::false_type{}): a run-time flag as a compile-time kernel parameter.
+template <typename F>
+void with_bool(bool b, F&& f) {
+    if (b) f(std::true_type{});
+    else f(std::false_type{});
+}
 
 // Carves sub-buffers out of a caller-owned workspace (256 B aligned).
 struct WsCarver {
@@ -96,6 +129,62 @@ __device__ __forceinline__ float block_sum(float v, float* smem /* THREADS/32 fl
         for (int o = 16; o > 0; o >>= 1) v += __shfl_down_sync(0xffffffffu, v, o);
     }
     return v;
+}
+
+// Deterministic grid-wide sum without float atomics: every block stores its block_sum of v in
+// partial[blockIdx.x] and takes a ticket; the last block to arrive sums the partials, then (EXTRA)
+// extra[0..n_extra), lane-strided in a fixed order, and folds the warp with a fixed shuffle tree.
+// Returns true in that block's thread 0, with the sum in `total`.  The caller writes the result
+// and, if it reuses the ticket, resets it.  sh_red (THREADS / 32 floats) and is_last are the
+// caller's shared memory, so that they keep their place in its layout.  EXTRA is a compile-time
+// switch because the compiler keeps the second loop even for a constant n_extra == 0.
+template <int THREADS, bool EXTRA = false>
+__device__ __forceinline__ bool grid_fold(float v, float* sh_red, bool& is_last, float* partial, int32_t* ticket,
+                                          float& total, const float* extra = nullptr, int n_extra = 0) {
+    const float bsum = block_sum<THREADS>(v, sh_red);
+    if (threadIdx.x == 0) {
+        partial[blockIdx.x] = bsum;
+        __threadfence();
+        is_last = atomicAdd(ticket, 1) == static_cast<int>(gridDim.x) - 1;
+    }
+    __syncthreads();
+    bool first = false;
+    if (is_last && threadIdx.x < 32) {
+        __threadfence();
+        float t = 0.f;
+        for (int k = threadIdx.x; k < static_cast<int>(gridDim.x); k += 32)
+            t += *reinterpret_cast<volatile float*>(partial + k);
+        if (EXTRA)
+            for (int k = threadIdx.x; k < n_extra; k += 32)
+                t += *reinterpret_cast<const volatile float*>(extra + k);
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) t += __shfl_down_sync(0xffffffffu, t, o);
+        total = t;
+        first = threadIdx.x == 0;
+    }
+    return first;
+}
+
+// d loss_b / d pos and d loss_b / d neg (unscaled by 1/B), and the loss term, of one pair of
+// scores: bpr, pointwise, or hinge (adaptive hinge on its selected negative).
+__device__ __forceinline__ void pair_loss(int loss, float p, float n, float& per, float& gp, float& gn) {
+    if (loss == SLB_LOSS_BPR) {
+        const float s = sigmoidf_(p - n);
+        per = 1.0f - s;
+        gp = -s * (1.0f - s);
+        gn = -gp;
+    } else if (loss == SLB_LOSS_POINTWISE) {
+        const float sp = sigmoidf_(p), sn = sigmoidf_(n);
+        per = (1.0f - sp) + sn;
+        gp = -sp * (1.0f - sp);
+        gn = sn * (1.0f - sn);
+    } else {
+        const float z = n - p + 1.0f;
+        per = fmaxf(z, 0.0f);
+        const float act = z >= 0.0f ? 1.0f : 0.0f;  // clamp backward passes at the boundary
+        gp = -act;
+        gn = act;
+    }
 }
 
 // MurmurHash3_x86_32 of the 4 little-endian bytes of a 32-bit key

@@ -145,33 +145,6 @@ EmbLayout emb_layout(void* base, int64_t T, int64_t rows) {
     return l;
 }
 
-#define DISPATCH_EMB(lpr, vec4, KERNEL, grid, stream, ...)                                        \
-    if (vec4) {                                                                                   \
-        switch (lpr) {                                                                            \
-            case 1: KERNEL<1, true><<<grid, EMB_THREADS, 0, stream>>>(__VA_ARGS__); break;        \
-            case 2: KERNEL<2, true><<<grid, EMB_THREADS, 0, stream>>>(__VA_ARGS__); break;        \
-            case 4: KERNEL<4, true><<<grid, EMB_THREADS, 0, stream>>>(__VA_ARGS__); break;        \
-            case 8: KERNEL<8, true><<<grid, EMB_THREADS, 0, stream>>>(__VA_ARGS__); break;        \
-            case 16: KERNEL<16, true><<<grid, EMB_THREADS, 0, stream>>>(__VA_ARGS__); break;      \
-            default: KERNEL<32, true><<<grid, EMB_THREADS, 0, stream>>>(__VA_ARGS__); break;      \
-        }                                                                                         \
-    } else {                                                                                      \
-        switch (lpr) {                                                                            \
-            case 1: KERNEL<1, false><<<grid, EMB_THREADS, 0, stream>>>(__VA_ARGS__); break;       \
-            case 2: KERNEL<2, false><<<grid, EMB_THREADS, 0, stream>>>(__VA_ARGS__); break;       \
-            case 4: KERNEL<4, false><<<grid, EMB_THREADS, 0, stream>>>(__VA_ARGS__); break;       \
-            case 8: KERNEL<8, false><<<grid, EMB_THREADS, 0, stream>>>(__VA_ARGS__); break;       \
-            case 16: KERNEL<16, false><<<grid, EMB_THREADS, 0, stream>>>(__VA_ARGS__); break;     \
-            default: KERNEL<32, false><<<grid, EMB_THREADS, 0, stream>>>(__VA_ARGS__); break;     \
-        }                                                                                         \
-    }
-
-int grid_for(int64_t work_groups) {
-    const int64_t cap = static_cast<int64_t>(slb_sms()) * 8;
-    int64_t g = work_groups < cap ? work_groups : cap;
-    return g < 1 ? 1 : static_cast<int>(g);
-}
-
 }  // namespace
 
 extern "C" {
@@ -187,9 +160,13 @@ int slb_embedding_forward(const float* W, int64_t rows, int32_t dim, const int64
     if (rc != SLB_OK) return rc;
     const bool vec4 = dim % 4 == 0;
     const int lpr = pow2_lanes(vec4 ? dim / 4 : dim);
-    const int grid = grid_for((n + EMB_THREADS / lpr - 1) / (EMB_THREADS / lpr));
+    const int grid = slb_grid((n + EMB_THREADS / lpr - 1) / (EMB_THREADS / lpr), 8);
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    DISPATCH_EMB(lpr, vec4, emb_fwd_kernel, grid, st, W, rows, dim, ids, n, hs, out, nullptr);
+    with_bool(vec4, [&](auto V) {
+        with_lpr(lpr, [&](auto L) {
+            emb_fwd_kernel<L, V><<<grid, EMB_THREADS, 0, st>>>(W, rows, dim, ids, n, hs, out, nullptr);
+        });
+    });
     SLB_LAUNCH_CHECK("emb_fwd_kernel");
     return SLB_OK;
 }
@@ -201,7 +178,7 @@ int slb_bloom_rows(const int64_t* ids, int64_t n, int32_t hash_count, const uint
     HashSpec hs;
     const int rc = make_hash(hs, hash_count, seeds, padding_idx);
     if (rc != SLB_OK) return rc;
-    bloom_rows_kernel<<<grid_for((n * hash_count + 255) / 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+    bloom_rows_kernel<<<slb_grid((n * hash_count + 255) / 256, 8), 256, 0, static_cast<cudaStream_t>(stream)>>>(
         ids, n, hs, rows, rows_out);
     SLB_LAUNCH_CHECK("bloom_rows_kernel");
     return SLB_OK;
@@ -230,7 +207,7 @@ int slb_embedding_backward(const float* dout, const int64_t* ids, int64_t n, int
         return SLB_ENOSPC;
     }
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    const int g1 = grid_for((T + 255) / 256);
+    const int g1 = slb_grid((T + 255) / 256, 8);
     emb_count_kernel<<<g1, 256, 0, st>>>(ids, T, hs, rows, l.keys, l.seg, l.flags + 4);
     SLB_LAUNCH_CHECK("emb_count_kernel");
     seg_scan_launch(l.seg, rows, st);
@@ -239,10 +216,12 @@ int slb_embedding_backward(const float* dout, const int64_t* ids, int64_t n, int
     SLB_LAUNCH_CHECK("emb_fill_kernel");
     const bool vec4 = dim % 4 == 0;
     const int lpr = pow2_lanes(vec4 ? dim / 4 : dim);
-    const int grid = grid_for((T + EMB_THREADS / lpr - 1) / (EMB_THREADS / lpr));
+    const int grid = slb_grid((T + EMB_THREADS / lpr - 1) / (EMB_THREADS / lpr), 8);
     // Bloom: the inner table is ScaledEmbedding(M, D, padding_idx=padding_idx)
     // (layers.py:162-164), so the same index is frozen in the compressed table
-    DISPATCH_EMB(lpr, vec4, emb_bwd_kernel, grid, st, dout, dim, fan, l.seg, frozen_row, dW);
+    with_bool(vec4, [&](auto V) {
+        with_lpr(lpr, [&](auto L) { emb_bwd_kernel<L, V><<<grid, EMB_THREADS, 0, st>>>(dout, dim, fan, l.seg, frozen_row, dW); });
+    });
     SLB_LAUNCH_CHECK("emb_bwd_kernel");
     return SLB_OK;
 }

@@ -8,21 +8,6 @@ namespace {
 constexpr int L_THREADS = 256;
 constexpr int L_MAX_GRID = 132 * 8;
 
-__device__ __forceinline__ void elem_loss(int loss, float p, float n, float& per, float& gp, float& gn) {
-    if (loss == SLB_LOSS_BPR) {
-        const float s = sigmoidf_(p - n);
-        per = 1.0f - s; gp = -s * (1.0f - s); gn = -gp;
-    } else if (loss == SLB_LOSS_POINTWISE) {
-        const float sp = sigmoidf_(p), sn = sigmoidf_(n);
-        per = (1.0f - sp) + sn; gp = -sp * (1.0f - sp); gn = sn * (1.0f - sn);
-    } else {
-        const float z = n - p + 1.0f;
-        per = fmaxf(z, 0.0f);
-        const float act = z >= 0.0f ? 1.0f : 0.0f;
-        gp = -act; gn = act;
-    }
-}
-
 __device__ __forceinline__ float pick_neg(int loss, const float* __restrict__ neg, int64_t i,
                                           int64_t n, int n_neg, int& kstar) {
     kstar = 0;
@@ -49,7 +34,7 @@ loss_reduce_kernel(int loss, const float* __restrict__ pos, const float* __restr
         int ks;
         const float nv = pick_neg(loss, neg, i, n, n_neg, ks);
         float per, gp, gn;
-        elem_loss(loss, pos[i], nv, per, gp, gn);
+        pair_loss(loss, pos[i], nv, per, gp, gn);
         const float m = mask ? (mask[i] ? 1.0f : 0.0f) : 1.0f;
         ls += per * m; ms += m;
     }
@@ -89,7 +74,7 @@ loss_grad_kernel(int loss, const float* __restrict__ pos, const float* __restric
         int ks;
         const float nv = pick_neg(loss, neg, i, n, n_neg, ks);
         float per, gp, gn;
-        elem_loss(loss, pos[i], nv, per, gp, gn);
+        pair_loss(loss, pos[i], nv, per, gp, gn);
         const float w = (mask ? (mask[i] ? 1.0f : 0.0f) : 1.0f) * inv;
         gpos[i] = gp * w;
         if (loss == SLB_LOSS_ADAPTIVE_HINGE) {
@@ -131,22 +116,8 @@ rating_loss_kernel(int loss, const float* __restrict__ pred, const float* __rest
         ls += per;
         if (grad) grad[i] = d * inv;
     }
-    const float bl = block_sum<L_THREADS>(ls, red);
-    if (threadIdx.x == 0) {
-        partial[blockIdx.x] = bl;
-        __threadfence();
-        is_last = atomicAdd(done, 1) == static_cast<int>(gridDim.x) - 1;
-    }
-    __syncthreads();
-    if (is_last && threadIdx.x < 32) {
-        __threadfence();
-        float a = 0.f;
-        for (int k = threadIdx.x; k < static_cast<int>(gridDim.x); k += 32)
-            a += *reinterpret_cast<volatile float*>(partial + k);
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) a += __shfl_down_sync(0xffffffffu, a, o);
-        if (threadIdx.x == 0) { *loss_out = a * inv; *done = 0; }
-    }
+    float a;
+    if (grid_fold<L_THREADS>(ls, red, is_last, partial, done, a)) { *loss_out = a * inv; *done = 0; }
 }
 
 }  // namespace
@@ -178,8 +149,7 @@ int slb_pairwise_loss(int32_t loss, const float* pos, const float* neg, const ui
     float* sums = ws.take<float>(8);
     float* partial = ws.take<float>(2 * L_MAX_GRID);
     int64_t want = (n + L_THREADS - 1) / L_THREADS;
-    const int64_t cap = static_cast<int64_t>(slb_sms()) * 8 < L_MAX_GRID ? static_cast<int64_t>(slb_sms()) * 8 : L_MAX_GRID;
-    const int grid = static_cast<int>(want < cap ? want : cap);
+    const int grid = min(slb_grid(want, 8), L_MAX_GRID);
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     loss_reduce_kernel<<<grid, L_THREADS, 0, st>>>(loss, pos, neg, mask, n, n_neg, partial, done, sums, loss_out);
     SLB_LAUNCH_CHECK("loss_reduce_kernel");
@@ -205,8 +175,7 @@ int slb_rating_loss(int32_t loss, const float* pred, const float* ratings, int64
     ws.take<float>(8);
     float* partial = ws.take<float>(2 * L_MAX_GRID);
     const int64_t want = (n + L_THREADS - 1) / L_THREADS;
-    const int64_t cap = static_cast<int64_t>(slb_sms()) * 8 < L_MAX_GRID ? static_cast<int64_t>(slb_sms()) * 8 : L_MAX_GRID;
-    const int grid = static_cast<int>(want < cap ? want : cap);
+    const int grid = min(slb_grid(want, 8), L_MAX_GRID);
     rating_loss_kernel<<<grid, L_THREADS, 0, static_cast<cudaStream_t>(stream)>>>(loss, pred, ratings, n, partial,
                                                                                   done, loss_out, grad);
     SLB_LAUNCH_CHECK("rating_loss_kernel");

@@ -70,27 +70,6 @@ __device__ __forceinline__ float row_dot(const float* __restrict__ a, const floa
     return group_sum<LPR>(acc, gmask);
 }
 
-// d loss_b / d pos and d loss_b / d neg (unscaled by 1/B), and the loss term.
-__device__ __forceinline__ void pair_loss(int loss, float p, float n, float& per, float& gp, float& gn) {
-    if (loss == SLB_LOSS_BPR) {
-        const float s = sigmoidf_(p - n);
-        per = 1.0f - s;
-        gp = -s * (1.0f - s);
-        gn = -gp;
-    } else if (loss == SLB_LOSS_POINTWISE) {
-        const float sp = sigmoidf_(p), sn = sigmoidf_(n);
-        per = (1.0f - sp) + sn;
-        gp = -sp * (1.0f - sp);
-        gn = sn * (1.0f - sn);
-    } else {  // hinge / adaptive hinge on the selected negative
-        const float z = n - p + 1.0f;
-        per = fmaxf(z, 0.0f);
-        const float act = z >= 0.0f ? 1.0f : 0.0f;  // clamp backward passes at the boundary
-        gp = -act;
-        gn = act;
-    }
-}
-
 // Rating losses on the raw score s of one interaction with observed rating r: the loss term
 // and d loss_b / d s (unscaled by 1/B).  spotlight/losses.py:169-244 with fit's exp for poisson
 // (spotlight/factorization/explicit.py:225-226): d/ds of exp(s) - r log(exp(s)) is exp(s) - r.
@@ -113,6 +92,7 @@ __device__ __forceinline__ void rating_loss(int loss, float s, float r, float& p
 template <int LPR>
 __global__ void __launch_bounds__(MF_THREADS) mf_fwd_kernel(MfDev a) {
     __shared__ float sh_red[MF_THREADS / 32];
+    __shared__ bool is_last;
     const int gl = threadIdx.x & (LPR - 1);
     const unsigned gmask = group_mask(LPR);
     constexpr int GROUPS = MF_THREADS / LPR;
@@ -182,23 +162,8 @@ __global__ void __launch_bounds__(MF_THREADS) mf_fwd_kernel(MfDev a) {
     }
 
     // deterministic loss reduction: fixed tree per block, fixed order over blocks
-    const float bsum = block_sum<MF_THREADS>(lsum, sh_red);
-    __shared__ bool is_last;
-    if (threadIdx.x == 0) {
-        a.partial[blockIdx.x] = bsum;
-        __threadfence();
-        is_last = atomicAdd(a.done, 1) == static_cast<int>(gridDim.x) - 1;
-    }
-    __syncthreads();
-    if (is_last && threadIdx.x < 32) {
-        __threadfence();
-        float v = 0.f;
-        for (int k = threadIdx.x; k < static_cast<int>(gridDim.x); k += 32)
-            v += *reinterpret_cast<volatile float*>(a.partial + k);
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) v += __shfl_down_sync(0xffffffffu, v, o);
-        if (threadIdx.x == 0) { *a.loss_out = v * invB; *a.done = 0; }
-    }
+    float v;
+    if (grid_fold<MF_THREADS>(lsum, sh_red, is_last, a.partial, a.done, v)) { *a.loss_out = v * invB; *a.done = 0; }
 }
 
 // ---------------------------------------------------------------------------
@@ -309,6 +274,8 @@ __global__ void __launch_bounds__(MF_TILE_THREADS) mf_fwd_tile_kernel(MfDev a) {
             if (gn != 0.f) atomicAdd(a.seg.cnt + a.U + j, 1);
         }
     }
+    // grid_fold written out: called through the helper, ptxas schedules this kernel's tile loop
+    // differently (more registers in some instantiations)
     const float bsum = block_sum<MF_TILE_THREADS>(lsum, sh_red);
     if (threadIdx.x == 0) {
         a.partial[blockIdx.x] = bsum;
@@ -343,10 +310,6 @@ __global__ void __launch_bounds__(MF_TILE_THREADS) mf_fwd_tile_kernel(MfDev a) {
 //         (partners are item rows, which MODE 1 no longer needs), so the user
 //         gradient is never written to memory.
 // ---------------------------------------------------------------------------
-// Adagrad step  w -= lr * g / (sqrt(s) + eps)  with MUFU-based sqrt and division
-// (rsqrt 2 ulp, fast divide 2 ulp: ~5e-7 relative, far inside the 1e-5 parity
-// budget; the IEEE sqrtf + division pair costs ~20 instructions per element and
-// made the update kernel issue-bound).
 __device__ __forceinline__ void cswap(int& x, int& y) {
     const int lo = x < y ? x : y, hi = x < y ? y : x;
     x = lo; y = hi;
@@ -999,22 +962,8 @@ __global__ void __launch_bounds__(MF_THREADS) mf_fwd_bloom_kernel(MfDev a, const
             }
         }
     }
-    const float bsum = block_sum<MF_THREADS>(lsum, sh_red);
-    if (threadIdx.x == 0) {
-        a.partial[blockIdx.x] = bsum;
-        __threadfence();
-        is_last = atomicAdd(a.done, 1) == static_cast<int>(gridDim.x) - 1;
-    }
-    __syncthreads();
-    if (is_last && threadIdx.x < 32) {
-        __threadfence();
-        float v = 0.f;
-        for (int k = threadIdx.x; k < static_cast<int>(gridDim.x); k += 32)
-            v += *reinterpret_cast<volatile float*>(a.partial + k);
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) v += __shfl_down_sync(0xffffffffu, v, o);
-        if (threadIdx.x == 0) { *a.loss_out = v * invB; *a.done = 0; }
-    }
+    float v;
+    if (grid_fold<MF_THREADS>(lsum, sh_red, is_last, a.partial, a.done, v)) { *a.loss_out = v * invB; *a.done = 0; }
 }
 
 struct MfLayout {
@@ -1040,58 +989,39 @@ MfLayout mf_layout(void* base, int64_t B, int64_t U, int64_t I, int terms_per = 
     return l;
 }
 
-int lpr_for_dim(int D) {
-    int l = D / 4;
-    if (l >= 32) return 32;
-    int p = 1;
-    while (p < l) p <<= 1;
-    return p;
+// Tile kernels: f(L, TI, EX) for L lanes per row, tiles of TI = 8 (small batches) or 32 rows, and
+// the exact-width variant EX when D == 4 * L (built for L >= 8).
+template <typename F>
+void with_tile(int lpr, bool small, int D, F&& f) {
+    with_bool(small, [&](auto SMALL) {
+        with_lpr(lpr, [&](auto L) {
+            constexpr int TI = SMALL ? 8 : 32;
+            if constexpr (L >= 8) {
+                if (D == L * 4) return f(L, std::integral_constant<int, TI>{}, std::true_type{});
+            }
+            f(L, std::integral_constant<int, TI>{}, std::false_type{});
+        });
+    });
 }
 
-#define DISPATCH_LPR(lpr, KERNEL, grid, block, stream, ...)                                   \
-    switch (lpr) {                                                                           \
-        case 1: KERNEL<1><<<grid, block, 0, stream>>>(__VA_ARGS__); break;                   \
-        case 2: KERNEL<2><<<grid, block, 0, stream>>>(__VA_ARGS__); break;                   \
-        case 4: KERNEL<4><<<grid, block, 0, stream>>>(__VA_ARGS__); break;                   \
-        case 8: KERNEL<8><<<grid, block, 0, stream>>>(__VA_ARGS__); break;                   \
-        case 16: KERNEL<16><<<grid, block, 0, stream>>>(__VA_ARGS__); break;                 \
-        default: KERNEL<32><<<grid, block, 0, stream>>>(__VA_ARGS__); break;                 \
-    }
+template <int LOSS>
+void launch_fwd_tile(const MfDev& a, int lpr, bool small, int grid, cudaStream_t st) {
+    with_tile(lpr, small, a.D, [&](auto L, auto TI, auto EX) {
+        mf_fwd_tile_kernel<L, LOSS, TI, EX><<<grid, MF_TILE_THREADS, 0, st>>>(a);
+    });
+}
 
-#define DISPATCH_LPR2(lpr, KERNEL, P2, grid, block, stream, ...)                               \
-    switch (lpr) {                                                                           \
-        case 1: KERNEL<1, P2><<<grid, block, 0, stream>>>(__VA_ARGS__); break;               \
-        case 2: KERNEL<2, P2><<<grid, block, 0, stream>>>(__VA_ARGS__); break;               \
-        case 4: KERNEL<4, P2><<<grid, block, 0, stream>>>(__VA_ARGS__); break;               \
-        case 8: KERNEL<8, P2><<<grid, block, 0, stream>>>(__VA_ARGS__); break;               \
-        case 16: KERNEL<16, P2><<<grid, block, 0, stream>>>(__VA_ARGS__); break;             \
-        default: KERNEL<32, P2><<<grid, block, 0, stream>>>(__VA_ARGS__); break;             \
-    }
-
-#define DISPATCH_LPR3_EX(L, KERNEL, P2, P3, grid, block, stream, a)                              \
-    if ((a).D == (L) * 4) KERNEL<L, P2, P3, true><<<grid, block, 0, stream>>>(a);                \
-    else KERNEL<L, P2, P3, false><<<grid, block, 0, stream>>>(a);
-#define DISPATCH_LPR3(lpr, KERNEL, P2, P3, grid, block, stream, a)                               \
-    switch (lpr) {                                                                               \
-        case 1: KERNEL<1, P2, P3, false><<<grid, block, 0, stream>>>(a); break;                  \
-        case 2: KERNEL<2, P2, P3, false><<<grid, block, 0, stream>>>(a); break;                  \
-        case 4: KERNEL<4, P2, P3, false><<<grid, block, 0, stream>>>(a); break;                  \
-        case 8: DISPATCH_LPR3_EX(8, KERNEL, P2, P3, grid, block, stream, a) break;               \
-        case 16: DISPATCH_LPR3_EX(16, KERNEL, P2, P3, grid, block, stream, a) break;             \
-        default: DISPATCH_LPR3_EX(32, KERNEL, P2, P3, grid, block, stream, a) break;             \
-    }
+template <int MODE>
+void launch_bwd_tile(const MfDev& a, int lpr, bool small, int grid, cudaStream_t st) {
+    with_tile(lpr, small, a.D, [&](auto L, auto TI, auto EX) {
+        mf_bwd_tile_kernel<L, MODE, TI, EX><<<grid, MF_TILE_THREADS, 0, st>>>(a);
+    });
+}
 
 template <int MODE>
 void launch_long(int lpr, cudaStream_t st, const MfDev& a) {
     const size_t smem = static_cast<size_t>(256 / lpr) * (a.D + 4) * sizeof(float);
-    switch (lpr) {
-        case 1: mf_bwd_long_kernel<1, MODE><<<SEG_LONG_CTAS * 4, 256, smem, st>>>(a); break;
-        case 2: mf_bwd_long_kernel<2, MODE><<<SEG_LONG_CTAS * 4, 256, smem, st>>>(a); break;
-        case 4: mf_bwd_long_kernel<4, MODE><<<SEG_LONG_CTAS * 4, 256, smem, st>>>(a); break;
-        case 8: mf_bwd_long_kernel<8, MODE><<<SEG_LONG_CTAS * 4, 256, smem, st>>>(a); break;
-        case 16: mf_bwd_long_kernel<16, MODE><<<SEG_LONG_CTAS * 4, 256, smem, st>>>(a); break;
-        default: mf_bwd_long_kernel<32, MODE><<<SEG_LONG_CTAS * 4, 256, smem, st>>>(a); break;
-    }
+    with_lpr(lpr, [&](auto L) { mf_bwd_long_kernel<L, MODE><<<SEG_LONG_CTAS * 4, 256, smem, st>>>(a); });
 }
 
 bool v2_eligible(const slb_mf_step_args* x);
@@ -1179,40 +1109,35 @@ int launch_step(const slb_mf_step_args* x, const int64_t* users, const int64_t* 
     const int lpr = lpr_for_dim(x->dim);
     const int groups = MF_THREADS / lpr;
     const int sms = slb_sms();
-    int64_t want = (B + groups - 1) / groups;
-    int grid = static_cast<int>(want < static_cast<int64_t>(sms) * 8 ? want : static_cast<int64_t>(sms) * 8);
-    if (grid < 1) grid = 1;
-    if (grid > MF_MAX_GRID) grid = MF_MAX_GRID;
+    const int grid = min(slb_grid((B + groups - 1) / groups, 8), MF_MAX_GRID);
     if ((phases & 1) && x->opt == SLB_OPT_ADAM) {
         // lazy-exact Adam: the rows this minibatch reads become current (through step t-1) first
         AdamDev o = {x->beta1, x->beta2, x->one_minus_beta1, x->one_minus_beta2, x->eps, x->weight_decay, x->adam_sched,
                      static_cast<int32_t>(x->adam_step + step_idx)};
         const int64_t refs = (2 + x->n_neg) * B;
-        const int64_t pw = (refs + groups - 1) / groups;
-        const int pgrid = static_cast<int>(pw < static_cast<int64_t>(sms) * 8 ? (pw < 1 ? 1 : pw) : static_cast<int64_t>(sms) * 8);
-        DISPATCH_LPR(lpr, mf_adam_prepass_kernel, pgrid, MF_THREADS, st, a, o, x->state2_Wu, x->state2_Wi,
-                     x->state2_bu, x->state2_bi, x->last_u, x->last_i);
+        const int pgrid = slb_grid((refs + groups - 1) / groups, 8);
+        with_lpr(lpr, [&](auto L) {
+            mf_adam_prepass_kernel<L><<<pgrid, MF_THREADS, 0, st>>>(a, o, x->state2_Wu, x->state2_Wi, x->state2_bu,
+                                                                   x->state2_bi, x->last_u, x->last_i);
+        });
         SLB_LAUNCH_CHECK("mf_adam_prepass_kernel");
     }
     if (phases & 1) {
         if (x->loss == SLB_LOSS_ADAPTIVE_HINGE) {
-            DISPATCH_LPR(lpr, mf_fwd_kernel, grid, MF_THREADS, st, a);
+            with_lpr(lpr, [&](auto L) { mf_fwd_kernel<L><<<grid, MF_THREADS, 0, st>>>(a); });
         } else {
             // small batches: 8-interaction tiles so that every SM still gets ~36 warps
             const bool small = B < static_cast<int64_t>(sms) * 36 * 32;
             const int ti = small ? 8 : 32;
             int64_t tw = ((B + ti - 1) / ti + 3) / 4;
             int tgrid = static_cast<int>(tw < MF_MAX_GRID ? tw : MF_MAX_GRID);
-#define FWD_TILE(L)                                                                             \
-    if (small) { DISPATCH_LPR3(lpr, mf_fwd_tile_kernel, L, 8, tgrid, MF_TILE_THREADS, st, a); } \
-    else { DISPATCH_LPR3(lpr, mf_fwd_tile_kernel, L, 32, tgrid, MF_TILE_THREADS, st, a); }
             switch (x->loss) {
-                case SLB_LOSS_POINTWISE: FWD_TILE(SLB_LOSS_POINTWISE); break;
-                case SLB_LOSS_BPR: FWD_TILE(SLB_LOSS_BPR); break;
-                case SLB_LOSS_REGRESSION: FWD_TILE(SLB_LOSS_REGRESSION); break;
-                case SLB_LOSS_POISSON: FWD_TILE(SLB_LOSS_POISSON); break;
-                case SLB_LOSS_LOGISTIC: FWD_TILE(SLB_LOSS_LOGISTIC); break;
-                default: FWD_TILE(SLB_LOSS_HINGE); break;
+                case SLB_LOSS_POINTWISE: launch_fwd_tile<SLB_LOSS_POINTWISE>(a, lpr, small, tgrid, st); break;
+                case SLB_LOSS_BPR: launch_fwd_tile<SLB_LOSS_BPR>(a, lpr, small, tgrid, st); break;
+                case SLB_LOSS_REGRESSION: launch_fwd_tile<SLB_LOSS_REGRESSION>(a, lpr, small, tgrid, st); break;
+                case SLB_LOSS_POISSON: launch_fwd_tile<SLB_LOSS_POISSON>(a, lpr, small, tgrid, st); break;
+                case SLB_LOSS_LOGISTIC: launch_fwd_tile<SLB_LOSS_LOGISTIC>(a, lpr, small, tgrid, st); break;
+                default: launch_fwd_tile<SLB_LOSS_HINGE>(a, lpr, small, tgrid, st); break;
             }
         }
         SLB_LAUNCH_CHECK("mf_fwd_kernel");
@@ -1221,28 +1146,21 @@ int launch_step(const slb_mf_step_args* x, const int64_t* users, const int64_t* 
         seg_scan_launch(a.seg, a.U, st);
         SLB_LAUNCH_CHECK("seg_scan_kernel");
     }
-    int fgrid = static_cast<int>((2 * B + 255) / 256);
-    if (fgrid > sms * 8) fgrid = sms * 8;
     if (phases & 4) {
-        mf_fill_kernel<<<fgrid, 256, 0, st>>>(a);
+        mf_fill_kernel<<<slb_grid((2 * B + 255) / 256, 8), 256, 0, st>>>(a);
         SLB_LAUNCH_CHECK("mf_fill_kernel");
         seg_sort_long_kernel<<<SEG_LONG_CTAS, 256, 0, st>>>(a.seg);     // no-op unless hot rows exist
         SLB_LAUNCH_CHECK("seg_sort_long_kernel");
     }
-    int64_t bwant = (2 * B + groups - 1) / groups;
-    int bgrid = static_cast<int>(bwant < static_cast<int64_t>(sms) * 8 ? bwant : static_cast<int64_t>(sms) * 8);
+    const int bgrid = slb_grid((2 * B + groups - 1) / groups, 8);
     // small batches: 8-segment tiles so that every SM still gets enough warps
     const bool bsmall = 2 * B < static_cast<int64_t>(sms) * 24 * 32;
     const int bti = bsmall ? 8 : 32;
     const int64_t tw = ((2 * B + bti - 1) / bti + 3) / 4;     // upper bound on segment tiles
-    const int tgrid = static_cast<int>(tw < static_cast<int64_t>(sms) * 16 ? tw : static_cast<int64_t>(sms) * 16);
-    const int blpr = lpr;
-#define BWD_TILE(MODE)                                                                               \
-    if (bsmall) { DISPATCH_LPR3(blpr, mf_bwd_tile_kernel, MODE, 8, tgrid, MF_TILE_THREADS, st, a); } \
-    else { DISPATCH_LPR3(blpr, mf_bwd_tile_kernel, MODE, 32, tgrid, MF_TILE_THREADS, st, a); }
+    const int tgrid = slb_grid(tw, 16);
     if (x->opt == SLB_OPT_NONE || x->opt == SLB_OPT_ADAM) {
         if (phases & 8) {
-            BWD_TILE(0);
+            launch_bwd_tile<0>(a, lpr, bsmall, tgrid, st);
             SLB_LAUNCH_CHECK("mf_bwd_tile_kernel");
             launch_long<0>(lpr, st, a);
             SLB_LAUNCH_CHECK("mf_bwd_long_kernel");
@@ -1251,15 +1169,17 @@ int launch_step(const slb_mf_step_args* x, const int64_t* users, const int64_t* 
             // lazy-exact Adam on the touched rows (mf_adam.cuh): a.sW* hold exp_avg
             AdamDev o = {x->beta1, x->beta2, x->one_minus_beta1, x->one_minus_beta2, x->eps, x->weight_decay, x->adam_sched,
                          static_cast<int32_t>(x->adam_step + step_idx)};
-            DISPATCH_LPR(lpr, mf_adam_apply_kernel, bgrid, MF_THREADS, st, a, o, x->state2_Wu, x->state2_Wi,
-                         x->state2_bu, x->state2_bi, x->last_u, x->last_i);
+            with_lpr(lpr, [&](auto L) {
+                mf_adam_apply_kernel<L><<<bgrid, MF_THREADS, 0, st>>>(a, o, x->state2_Wu, x->state2_Wi, x->state2_bu,
+                                                                     x->state2_bi, x->last_u, x->last_i);
+            });
             SLB_LAUNCH_CHECK("mf_adam_apply_kernel");
         }
     } else {
         // fused optimizer: item gradients first (they read the old user rows), then
         // the user pass updates its rows in place, then the item rows are updated
         if (phases & 8) {
-            BWD_TILE(1);
+            launch_bwd_tile<1>(a, lpr, bsmall, tgrid, st);
             SLB_LAUNCH_CHECK("mf_bwd_tile_kernel<items>");
             launch_long<1>(lpr, st, a);
             SLB_LAUNCH_CHECK("mf_bwd_long_kernel<items>");
@@ -1275,13 +1195,13 @@ int launch_step(const slb_mf_step_args* x, const int64_t* users, const int64_t* 
                 kern<<<tgrid, MF_TILE_THREADS, BULK_SMEM, st>>>(a);
             } else
 #endif
-            { BWD_TILE(2); }
+            launch_bwd_tile<2>(a, lpr, bsmall, tgrid, st);
             SLB_LAUNCH_CHECK("mf_bwd_tile_kernel<users+opt>");
             launch_long<2>(lpr, st, a);
             SLB_LAUNCH_CHECK("mf_bwd_long_kernel<users+opt>");
         }
         if ((phases & 16) && !x->opt_users_only) {
-            DISPATCH_LPR2(lpr, mf_apply_kernel, 1, bgrid, MF_THREADS, st, a);
+            with_lpr(lpr, [&](auto L) { mf_apply_kernel<L, 1><<<bgrid, MF_THREADS, 0, st>>>(a); });
             SLB_LAUNCH_CHECK("mf_apply_kernel<items>");
         }
     }
@@ -1359,17 +1279,14 @@ int v2_launch_plan(const slb_mf_step_args* x, PlanDev p, int32_t* err, const int
                    const int64_t* negs, const float* ratings, int64_t B, cudaStream_t st) {
     p.B = B; p.users = users; p.items = items; p.negs = negs; p.ratings = ratings; p.err = err;
     p.seg.long_cap = seg_sort_cap(lpr_for_dim(x->dim));
-    const int sms = slb_sms();
-    int g = static_cast<int>((B + 255) / 256);
-    if (g > sms * 8) g = sms * 8;
+    const int g = slb_grid((B + 255) / 256, 8);
     plan_count_kernel<<<g, 256, 0, st>>>(p);
     SLB_LAUNCH_CHECK("plan_count_kernel");
     seg_scan_launch(p.seg, p.U, st);
     SLB_LAUNCH_CHECK("seg_scan_kernel");
     plan_fill_kernel<<<g, 256, 0, st>>>(p);
     SLB_LAUNCH_CHECK("plan_fill_kernel");
-    int64_t tiles = ((3 * B + 31) / 32 + 3) / 4;
-    int sg = static_cast<int>(tiles < static_cast<int64_t>(sms) * 16 ? tiles : static_cast<int64_t>(sms) * 16);
+    const int sg = slb_grid(((3 * B + 31) / 32 + 3) / 4, 16);
     plan_sort_kernel<<<sg, 128, 0, st>>>(p, p.seg.long_cap);
     SLB_LAUNCH_CHECK("plan_sort_kernel");
     plan_order_long_kernel<<<1, 256, 0, st>>>(p);                      // no-op unless two or more hot rows
@@ -1442,26 +1359,14 @@ int v2_launch_step(const slb_mf_step_args* x, const V2Layout& l, int slot, int32
         const bool small = B < static_cast<int64_t>(sms) * 24 * 32;
         const int64_t tw = ((B + (small ? 8 : 32) - 1) / (small ? 8 : 32) + 3) / 4;
         const int grid = static_cast<int>(tw < MF_MAX_GRID ? (tw < 1 ? 1 : tw) : MF_MAX_GRID);
-        switch (lpr) {
-            case 2: v2_user_dispatch<2>(a, p, l.st, small, grid, st); break;
-            case 4: v2_user_dispatch<4>(a, p, l.st, small, grid, st); break;
-            case 8: v2_user_dispatch<8>(a, p, l.st, small, grid, st); break;
-            case 16: v2_user_dispatch<16>(a, p, l.st, small, grid, st); break;
-            default: v2_user_dispatch<32>(a, p, l.st, small, grid, st); break;
-        }
+        with_lpr<2>(lpr, [&](auto L) { v2_user_dispatch<L>(a, p, l.st, small, grid, st); });
         SLB_LAUNCH_CHECK("mf_user_kernel");
     }
     if (phases & 4) {
         const bool small = 2 * B < static_cast<int64_t>(sms) * 24 * 32;
         const int64_t tw = ((2 * B + (small ? 8 : 32) - 1) / (small ? 8 : 32) + 3) / 4;
-        const int grid = static_cast<int>(tw < static_cast<int64_t>(sms) * 16 ? (tw < 1 ? 1 : tw) : static_cast<int64_t>(sms) * 16);
-        switch (lpr) {
-            case 2: v2_item_launch<2>(a, p, l.st, small, grid, st); break;
-            case 4: v2_item_launch<4>(a, p, l.st, small, grid, st); break;
-            case 8: v2_item_launch<8>(a, p, l.st, small, grid, st); break;
-            case 16: v2_item_launch<16>(a, p, l.st, small, grid, st); break;
-            default: v2_item_launch<32>(a, p, l.st, small, grid, st); break;
-        }
+        const int grid = slb_grid(tw, 16);
+        with_lpr<2>(lpr, [&](auto L) { v2_item_launch<L>(a, p, l.st, small, grid, st); });
         SLB_LAUNCH_CHECK("mf_item_kernel");
     }
     return SLB_OK;
@@ -1643,12 +1548,12 @@ int slb_adam_flush(float* W, float* exp_avg, float* exp_avg_sq, float* bias, flo
     AdamDev o = {beta1, beta2, one_minus_beta1, one_minus_beta2, eps, weight_decay, sched, static_cast<int32_t>(step)};
     const int lpr = lpr_for_dim(dim);
     const int groups = MF_THREADS / lpr;
-    const int64_t want = (rows + groups - 1) / groups;
-    const int sms = slb_sms();
-    const int grid = static_cast<int>(want < static_cast<int64_t>(sms) * 16 ? want : static_cast<int64_t>(sms) * 16);
+    const int grid = slb_grid((rows + groups - 1) / groups, 16);
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    DISPATCH_LPR(lpr, adam_flush_kernel, grid, MF_THREADS, st, W, exp_avg, exp_avg_sq, bias, bias_avg, bias_avg_sq,
-                 last, rows, dim, o);
+    with_lpr(lpr, [&](auto L) {
+        adam_flush_kernel<L><<<grid, MF_THREADS, 0, st>>>(W, exp_avg, exp_avg_sq, bias, bias_avg, bias_avg_sq, last,
+                                                         rows, dim, o);
+    });
     SLB_LAUNCH_CHECK("adam_flush_kernel");
     return SLB_OK;
 }
@@ -1661,12 +1566,11 @@ int slb_mf_scores(const float* Wu, const float* Wi, const float* bu, const float
     if (n <= 0) return SLB_OK;
     const int lpr = lpr_for_dim(dim);
     const int groups = MF_THREADS / lpr;
-    const int sms = slb_sms();
-    int64_t want = (n + groups - 1) / groups;
-    int grid = static_cast<int>(want < static_cast<int64_t>(sms) * 8 ? want : static_cast<int64_t>(sms) * 8);
+    const int grid = slb_grid((n + groups - 1) / groups, 8);
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    DISPATCH_LPR(lpr, mf_scores_kernel, grid, MF_THREADS, st, Wu, Wi, bu, bi, dim, users, items, n,
-                 user_broadcast, scores);
+    with_lpr(lpr, [&](auto L) {
+        mf_scores_kernel<L><<<grid, MF_THREADS, 0, st>>>(Wu, Wi, bu, bi, dim, users, items, n, user_broadcast, scores);
+    });
     SLB_LAUNCH_CHECK("mf_scores_kernel");
     return SLB_OK;
 }
@@ -1698,9 +1602,7 @@ int slb_mf_scores_backward(const float* gscores, const int64_t* users, const int
     a.grad_mode = SLB_GRAD_DENSE;
     a.dWu = dWu; a.dWi = dWi; a.dbu = dbu; a.dbi = dbi;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    const int sms = slb_sms();
-    int g1 = static_cast<int>((n + 255) / 256);
-    if (g1 > sms * 8) g1 = sms * 8;
+    const int g1 = slb_grid((n + 255) / 256, 8);
     mf_terms_kernel<<<g1, 256, 0, st>>>(a, gscores, user_broadcast);
     SLB_LAUNCH_CHECK("mf_terms_kernel");
     seg_scan_launch(a.seg, a.U, st);
@@ -1710,9 +1612,7 @@ int slb_mf_scores_backward(const float* gscores, const int64_t* users, const int
     seg_sort_long_kernel<<<SEG_LONG_CTAS, 256, 0, st>>>(a.seg);
     SLB_LAUNCH_CHECK("seg_sort_long_kernel");
     const int lpr = lpr_for_dim(dim);
-    int64_t tw = ((n + 31) / 32 + 3) / 4;
-    int tgrid = static_cast<int>(tw < static_cast<int64_t>(sms) * 16 ? tw : static_cast<int64_t>(sms) * 16);
-    DISPATCH_LPR3(lpr, mf_bwd_tile_kernel, 0, 32, tgrid, MF_TILE_THREADS, st, a);
+    launch_bwd_tile<0>(a, lpr, false, slb_grid(((n + 31) / 32 + 3) / 4, 16), st);
     SLB_LAUNCH_CHECK("mf_bwd_tile_kernel");
     launch_long<0>(lpr, st, a);
     SLB_LAUNCH_CHECK("mf_bwd_long_kernel");
@@ -1810,9 +1710,7 @@ int bias_sparse_apply(void* wsp, const int64_t* ids, const float* g, int64_t n, 
     p.seg = seg_index_carve(ws, nb, n);
     p.ids = ids; p.g = g; p.n = n; p.mask = nb - 1; p.b = b; p.sb = sb;
     p.opt = opt; p.lr = lr; p.wd = wd; p.eps = eps; p.by_id = by_id ? 1 : 0;
-    const int sms = slb_sms();
-    int grid = static_cast<int>((n + 255) / 256);
-    if (grid > sms * 8) grid = sms * 8;
+    const int grid = slb_grid((n + 255) / 256, 8);
     bias_count_kernel<<<grid, 256, 0, st>>>(p);
     SLB_LAUNCH_CHECK("bias_count_kernel");
     seg_scan_launch(p.seg, p.seg.Rpad, st);
@@ -1938,41 +1836,27 @@ int slb_mf_bloom_train_step(const slb_mf_bloom_args* x, slb_stream_t stream) {
     if (!fused && pairs_i) { h.ids_i2 = x->pair_ids_i; h.g_i2 = x->pair_g_i; }
 
     const int groups = MF_THREADS / lpr;
-    const int sms = slb_sms();
-    int64_t want = (B + groups - 1) / groups;
-    int grid = static_cast<int>(want < static_cast<int64_t>(sms) * 8 ? want : static_cast<int64_t>(sms) * 8);
-    if (grid > MF_MAX_GRID) grid = MF_MAX_GRID;
-    switch (lpr) {
-        case 1: mf_fwd_bloom_kernel<1><<<grid, MF_THREADS, 0, st>>>(a, h); break;
-        case 2: mf_fwd_bloom_kernel<2><<<grid, MF_THREADS, 0, st>>>(a, h); break;
-        case 4: mf_fwd_bloom_kernel<4><<<grid, MF_THREADS, 0, st>>>(a, h); break;
-        case 8: mf_fwd_bloom_kernel<8><<<grid, MF_THREADS, 0, st>>>(a, h); break;
-        case 16: mf_fwd_bloom_kernel<16><<<grid, MF_THREADS, 0, st>>>(a, h); break;
-        default: mf_fwd_bloom_kernel<32><<<grid, MF_THREADS, 0, st>>>(a, h); break;
-    }
+    const int grid = min(slb_grid((B + groups - 1) / groups, 8), MF_MAX_GRID);
+    with_lpr(lpr, [&](auto L) { mf_fwd_bloom_kernel<L><<<grid, MF_THREADS, 0, st>>>(a, h); });
     SLB_LAUNCH_CHECK("mf_fwd_bloom_kernel");
     seg_scan_launch(a.seg, a.U, st);
     SLB_LAUNCH_CHECK("seg_scan_kernel");
-    int fgrid = static_cast<int>((T + 255) / 256);
-    if (fgrid > sms * 8) fgrid = sms * 8;
-    mf_fill_kernel<<<fgrid, 256, 0, st>>>(a);
+    mf_fill_kernel<<<slb_grid((T + 255) / 256, 8), 256, 0, st>>>(a);
     SLB_LAUNCH_CHECK("mf_fill_kernel");
     seg_sort_long_kernel<<<SEG_LONG_CTAS, 256, 0, st>>>(a.seg);
     SLB_LAUNCH_CHECK("seg_sort_long_kernel");
-    const int64_t tw = ((2 * T + 31) / 32 + 3) / 4;
-    const int tgrid = static_cast<int>(tw < static_cast<int64_t>(sms) * 16 ? tw : static_cast<int64_t>(sms) * 16);
+    const int tgrid = slb_grid(((2 * T + 31) / 32 + 3) / 4, 16);
     if (fused) {
         // hashed item rows first (compact gradients from the old user rows), user rows updated in
         // place, item rows updated from the compact gradients, then the id-space biases
-        DISPATCH_LPR3(lpr, mf_bwd_tile_kernel, 1, 32, tgrid, MF_TILE_THREADS, st, a);
+        launch_bwd_tile<1>(a, lpr, false, tgrid, st);
         SLB_LAUNCH_CHECK("mf_bwd_tile_kernel<items>");
         launch_long<1>(lpr, st, a);
-        DISPATCH_LPR3(lpr, mf_bwd_tile_kernel, 2, 32, tgrid, MF_TILE_THREADS, st, a);
+        launch_bwd_tile<2>(a, lpr, false, tgrid, st);
         SLB_LAUNCH_CHECK("mf_bwd_tile_kernel<users+opt>");
         launch_long<2>(lpr, st, a);
-        const int64_t aw = (2 * T + groups - 1) / groups;
-        const int agrid = static_cast<int>(aw < static_cast<int64_t>(sms) * 8 ? aw : static_cast<int64_t>(sms) * 8);
-        DISPATCH_LPR2(lpr, mf_apply_kernel, 1, agrid, MF_THREADS, st, a);
+        const int agrid = slb_grid((2 * T + groups - 1) / groups, 8);
+        with_lpr(lpr, [&](auto L) { mf_apply_kernel<L, 1><<<agrid, MF_THREADS, 0, st>>>(a); });
         SLB_LAUNCH_CHECK("mf_apply_kernel<items>");
         int rcb = bias_sparse_apply(l.bws_u, l.ids_u2, l.g_u2, 2 * B, b.bu, b.state_bu, b.opt, b.lr, b.weight_decay,
                                     b.eps, true, st);
@@ -1980,7 +1864,7 @@ int slb_mf_bloom_train_step(const slb_mf_bloom_args* x, slb_stream_t stream) {
         return bias_sparse_apply(l.bws_i, l.ids_i2, l.g_i2, 2 * B, b.bi, b.state_bi, b.opt, b.lr, b.weight_decay,
                                  b.eps, true, st);
     }
-    DISPATCH_LPR3(lpr, mf_bwd_tile_kernel, 0, 32, tgrid, MF_TILE_THREADS, st, a);
+    launch_bwd_tile<0>(a, lpr, false, tgrid, st);
     SLB_LAUNCH_CHECK("mf_bwd_tile_kernel");
     launch_long<0>(lpr, st, a);
     SLB_LAUNCH_CHECK("mf_bwd_long_kernel");

@@ -529,23 +529,10 @@ __global__ void __launch_bounds__(MF_TILE_THREADS, (VPL == 1 ? V2_UMINB : V2_UMI
     }
 
     // deterministic loss reduction: fixed tree per block, fixed order over blocks (+ hot-row partials)
-    const float bsum = block_sum<MF_TILE_THREADS>(lsum, sh_red);
-    if (threadIdx.x == 0) {
-        v.partial[blockIdx.x] = bsum;
-        __threadfence();
-        is_last = atomicAdd(v.done, 1) == static_cast<int>(gridDim.x) - 1;
-    }
-    __syncthreads();
-    if (is_last && threadIdx.x < 32) {
-        __threadfence();
-        float t = 0.f;
-        for (int k = threadIdx.x; k < static_cast<int>(gridDim.x); k += 32)
-            t += *reinterpret_cast<volatile float*>(v.partial + k);
-        for (int k = threadIdx.x; k < n_long_partials; k += 32)
-            t += *reinterpret_cast<volatile float*>(v.partial_long + k);
-#pragma unroll
-        for (int off = 16; off > 0; off >>= 1) t += __shfl_down_sync(0xffffffffu, t, off);
-        if (threadIdx.x == 0) { *a.loss_out = t * invB; *v.done = 0; }
+    float t;
+    if (grid_fold<MF_TILE_THREADS, true>(lsum, sh_red, is_last, v.partial, v.done, t, v.partial_long, n_long_partials)) {
+        *a.loss_out = t * invB;
+        *v.done = 0;
     }
 }
 

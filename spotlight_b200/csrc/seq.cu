@@ -294,42 +294,13 @@ pool_bwd_kernel(const float* __restrict__ E, const int64_t* __restrict__ seqs, i
 
 // ------------------------------------------------------------------ scoring
 // representations.py:136-144 / 444-453 + the masked loss + d loss / d r.
-__device__ __forceinline__ void seq_pair_loss(int loss, float p, float n, float& per, float& gp, float& gn) {
-    if (loss == SLB_LOSS_BPR) {
-        const float s = sigmoidf_(p - n);
-        per = 1.0f - s; gp = -s * (1.0f - s); gn = -gp;
-    } else if (loss == SLB_LOSS_POINTWISE) {
-        const float sp = sigmoidf_(p), sn = sigmoidf_(n);
-        per = (1.0f - sp) + sn; gp = -sp * (1.0f - sp); gn = sn * (1.0f - sn);
-    } else {
-        const float z = n - p + 1.0f;
-        per = fmaxf(z, 0.0f);
-        const float act = z >= 0.0f ? 1.0f : 0.0f;
-        gp = -act; gn = act;
-    }
-}
-
-// Masked loss of the step: every block writes its partial sum, the last block to finish folds the
-// partials in a fixed order (no float atomics) and writes the mean over msum positions.
+// Masked loss of the step: the grid's loss sum (grid_fold: fixed order, no float atomics) over
+// msum positions.
 __device__ __forceinline__ void seq_loss_fold(const SeqDev& a, float lsum, float msum) {
     __shared__ float sh_red[SQ_THREADS / 32];
     __shared__ bool is_last;
-    const float bsum = block_sum<SQ_THREADS>(lsum, sh_red);
-    if (threadIdx.x == 0) {
-        a.partial[blockIdx.x] = bsum;
-        __threadfence();
-        is_last = atomicAdd(a.hdr, 1) == static_cast<int>(gridDim.x) - 1;
-    }
-    __syncthreads();
-    if (is_last && threadIdx.x < 32) {
-        __threadfence();
-        float v = 0.f;
-        for (int k = threadIdx.x; k < static_cast<int>(gridDim.x); k += 32)
-            v += *reinterpret_cast<volatile float*>(a.partial + k);
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) v += __shfl_down_sync(0xffffffffu, v, o);
-        if (threadIdx.x == 0) *a.loss_out = v / msum;
-    }
+    float t;
+    if (grid_fold<SQ_THREADS>(lsum, sh_red, is_last, a.partial, a.hdr, t)) *a.loss_out = t / msum;
 }
 
 // Backward keys of one position's terms.  Plain table: the seq-role term pidx and the credited
@@ -414,7 +385,7 @@ __global__ void __launch_bounds__(SQ_THREADS) seq_score_kernel(SeqDev a) {
             if (k == 0 || nk > nbest) { nbest = nk; nid = j; }
         }
         float per, gp, gn;
-        seq_pair_loss(a.loss, p, nbest, per, gp, gn);
+        pair_loss(a.loss, p, nbest, per, gp, gn);
         const float mk = id != 0 ? 1.0f : 0.0f;      // mask = seq != PADDING_IDX
         lsum += (valid && gl == 0) ? per * mk : 0.f;
         gp *= mk * inv; gn *= mk * inv;
@@ -1012,43 +983,7 @@ int seq_validate(const slb_seq_step_args* x, bool training) {
     return SLB_OK;
 }
 
-int sq_grid(int64_t groups_needed) {
-    const int64_t cap = static_cast<int64_t>(slb_sms()) * 8 < SQ_MAX_GRID ? static_cast<int64_t>(slb_sms()) * 8 : SQ_MAX_GRID;
-    const int64_t g = groups_needed < cap ? groups_needed : cap;
-    return g < 1 ? 1 : static_cast<int>(g);
-}
-
-int lpr_of(int D) {
-    int l = D / 4, p = 1;
-    if (l >= 32) return 32;
-    while (p < l) p <<= 1;
-    return p;
-}
-
-#define SQ_DISPATCH_LPR(lpr, KERNEL, grid, stream, ...)                                  \
-    switch (lpr) {                                                                       \
-        case 1: KERNEL<1><<<grid, SQ_THREADS, 0, stream>>>(__VA_ARGS__); break;          \
-        case 2: KERNEL<2><<<grid, SQ_THREADS, 0, stream>>>(__VA_ARGS__); break;          \
-        case 4: KERNEL<4><<<grid, SQ_THREADS, 0, stream>>>(__VA_ARGS__); break;          \
-        case 8: KERNEL<8><<<grid, SQ_THREADS, 0, stream>>>(__VA_ARGS__); break;          \
-        case 16: KERNEL<16><<<grid, SQ_THREADS, 0, stream>>>(__VA_ARGS__); break;        \
-        default: KERNEL<32><<<grid, SQ_THREADS, 0, stream>>>(__VA_ARGS__); break;        \
-    }
-
-// row-source variants: HASHED is a compile-time bool of the kernel
-#define SQ_DISPATCH_LPR_T(lpr, KERNEL, HASHED, grid, stream, ...)                        \
-    switch (lpr) {                                                                       \
-        case 1: KERNEL<1, HASHED><<<grid, SQ_THREADS, 0, stream>>>(__VA_ARGS__); break;  \
-        case 2: KERNEL<2, HASHED><<<grid, SQ_THREADS, 0, stream>>>(__VA_ARGS__); break;  \
-        case 4: KERNEL<4, HASHED><<<grid, SQ_THREADS, 0, stream>>>(__VA_ARGS__); break;  \
-        case 8: KERNEL<8, HASHED><<<grid, SQ_THREADS, 0, stream>>>(__VA_ARGS__); break;  \
-        case 16: KERNEL<16, HASHED><<<grid, SQ_THREADS, 0, stream>>>(__VA_ARGS__); break; \
-        default: KERNEL<32, HASHED><<<grid, SQ_THREADS, 0, stream>>>(__VA_ARGS__); break; \
-    }
-
-#define SQ_DISPATCH_LPR_ROWS(hashed, lpr, KERNEL, grid, stream, ...)                     \
-    if (hashed) { SQ_DISPATCH_LPR_T(lpr, KERNEL, true, grid, stream, __VA_ARGS__) }      \
-    else { SQ_DISPATCH_LPR_T(lpr, KERNEL, false, grid, stream, __VA_ARGS__) }
+int sq_grid(int64_t groups_needed) { return min(slb_grid(groups_needed, 8), SQ_MAX_GRID); }
 
 #define SQ_DISPATCH_NCH_T(D, KERNEL, BYPOS, grid, smem, stream, ...)                     \
     if ((D) <= 128) KERNEL<1, BYPOS><<<grid, SQ_THREADS, smem, stream>>>(__VA_ARGS__);   \
@@ -1073,13 +1008,16 @@ SeqDev seq_dev_table(const slb_seq_step_args* x) {
 // X0 = the input rows of every position: E[seq], or the hashed sums
 int launch_gather(const slb_seq_step_args* x, const SeqLayout& l, cudaStream_t st) {
     const int64_t n = x->batch * x->seq_len;
-    const int lpr = lpr_of(x->dim);
+    const int lpr = lpr_for_dim(x->dim);
     const int grid = sq_grid((n + SQ_THREADS / lpr - 1) / (SQ_THREADS / lpr));
     if (x->item_hashes) {
-        SQ_DISPATCH_LPR(lpr, seq_gather_hashed_kernel, grid, st, seq_dev_table(x), l.X0);
+        const SeqDev a = seq_dev_table(x);
+        with_lpr(lpr, [&](auto L) { seq_gather_hashed_kernel<L><<<grid, SQ_THREADS, 0, st>>>(a, l.X0); });
         SLB_LAUNCH_CHECK("seq_gather_hashed_kernel");
     } else {
-        SQ_DISPATCH_LPR(lpr, seq_gather_kernel, grid, st, x->E, x->seqs, n, x->dim, x->num_items, l.X0);
+        with_lpr(lpr, [&](auto L) {
+            seq_gather_kernel<L><<<grid, SQ_THREADS, 0, st>>>(x->E, x->seqs, n, x->dim, x->num_items, l.X0);
+        });
         SLB_LAUNCH_CHECK("seq_gather_kernel");
     }
     return SLB_OK;
@@ -1376,7 +1314,7 @@ int slb_seq_train_step(const slb_seq_step_args* x, slb_stream_t stream) {
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     const int64_t B = x->batch;
     const int S = x->seq_len, T = S + 1, D = x->dim;
-    const int lpr = lpr_of(D);
+    const int lpr = lpr_for_dim(D);
     const int groups = SQ_THREADS / lpr;
     if (cudaMemsetAsync(l.hdr, 0, 16 * sizeof(int32_t), st) != cudaSuccess) {
         slb_set_error("seq_train_step: memset failed");
@@ -1399,14 +1337,19 @@ int slb_seq_train_step(const slb_seq_step_args* x, slb_stream_t stream) {
     // hashed rows are hot at small item_rows: sort their member lists with seg_sort_long_kernel
     if (hashed) a.seg.long_cap = seg_sort_cap(lpr);
     a.opt = x->opt; a.lr = x->lr; a.wd = x->weight_decay; a.eps = x->eps; a.sE = x->state_E; a.sbias = x->state_bias;
+    const int score_grid = sq_grid((B * T + groups - 1) / groups);
     if (x->mix_w) {
         a.M = x->num_mixtures; a.P = l.P;
-        SQ_DISPATCH_LPR_ROWS(hashed, lpr, mix::mix_score_kernel, sq_grid((B * T + groups - 1) / groups), st, a);
+        with_bool(hashed, [&](auto H) {
+            with_lpr(lpr, [&](auto L) { mix::mix_score_kernel<L, H><<<score_grid, SQ_THREADS, 0, st>>>(a); });
+        });
         SLB_LAUNCH_CHECK("mix_score_kernel");
         rc = run_mix_backward(x, l, st);
         if (rc != SLB_OK) return rc;
     } else {
-        SQ_DISPATCH_LPR_ROWS(hashed, lpr, seq_score_kernel, sq_grid((B * T + groups - 1) / groups), st, a);
+        with_bool(hashed, [&](auto H) {
+            with_lpr(lpr, [&](auto L) { seq_score_kernel<L, H><<<score_grid, SQ_THREADS, 0, st>>>(a); });
+        });
         SLB_LAUNCH_CHECK("seq_score_kernel");
     }
 
@@ -1458,7 +1401,10 @@ int slb_seq_train_step(const slb_seq_step_args* x, slb_stream_t stream) {
         seg_sort_long_kernel<<<SEG_LONG_CTAS, 256, 0, st>>>(a.seg);     // no-op unless hot rows exist
         SLB_LAUNCH_CHECK("seg_sort_long_kernel");
     }
-    SQ_DISPATCH_LPR_ROWS(hashed, lpr, seq_reduce_kernel, sq_grid((nkeys + groups - 1) / groups), st, a);
+    const int reduce_grid = sq_grid((nkeys + groups - 1) / groups);
+    with_bool(hashed, [&](auto H) {
+        with_lpr(lpr, [&](auto L) { seq_reduce_kernel<L, H><<<reduce_grid, SQ_THREADS, 0, st>>>(a); });
+    });
     SLB_LAUNCH_CHECK("seq_reduce_kernel");
     return SLB_OK;
 }

@@ -11,7 +11,7 @@
 //   dc_m = g w_m e,  dv_m = g w_m (z_m - s_bar) e,  de = g sum_m w_m (c_m + (z_m - s_bar) v_m).
 //
 // mix_score_kernel mirrors seq_score_kernel's bookkeeping: one lane group per position, the
-// loss of seq_pair_loss folded by seq_loss_fold, pos_out / neg_out, the contribution rows C (now
+// loss of pair_loss folded by seq_loss_fold, pos_out / neg_out, the contribution rows C (now
 // de of the target and of the credited negative), keys, gs and the row counts.  Instead of
 // d loss / d r it writes d loss / d P over P in place: each position's group reads its own 2M
 // rows before it overwrites them.  The row t = S is zeroed (the final step is not trained on).
@@ -114,7 +114,7 @@ __global__ void __launch_bounds__(SQ_THREADS) mix_score_kernel(SeqDev a) {
             }
         }
         float per, gp, gn;
-        seq_pair_loss(a.loss, p, nbest, per, gp, gn);
+        pair_loss(a.loss, p, nbest, per, gp, gn);
         const float mk = id != 0 ? 1.0f : 0.0f;       // mask = seq != PADDING_IDX
         lsum += (valid && gl == 0) ? per * mk : 0.f;
         gp *= mk * inv; gn *= mk * inv;
