@@ -966,6 +966,58 @@ __global__ void __launch_bounds__(MF_THREADS) mf_fwd_bloom_kernel(MfDev a, const
     if (grid_fold<MF_THREADS>(lsum, sh_red, is_last, a.partial, a.done, v)) { *a.loss_out = v * invB; *a.done = 0; }
 }
 
+// Rating losses on hashed tables (explicit.py:223-234 with Bloom layers): one scored side per
+// interaction, so Hu' * Hi' terms (term b * Hu' * Hi' + ku * Hi' + ki) and one bias pair per table
+// (pair b) per interaction.  In fused mode a pair with g == 0 gets id -1: its bias is untouched.
+template <int LPR>
+__global__ void __launch_bounds__(MF_THREADS) mf_fwd_bloom_rating_kernel(MfDev a, const __grid_constant__ BloomSpec h) {
+    __shared__ float sh_red[MF_THREADS / 32];
+    __shared__ bool is_last;
+    const int gl = threadIdx.x & (LPR - 1);
+    const unsigned gmask = group_mask(LPR);
+    constexpr int GROUPS = MF_THREADS / LPR;
+    const int64_t gid = static_cast<int64_t>(blockIdx.x) * GROUPS + threadIdx.x / LPR;
+    const int64_t gstride = static_cast<int64_t>(gridDim.x) * GROUPS;
+    const float invB = 1.0f / static_cast<float>(a.NB);
+    const int nu = h.Hu ? h.Hu : 1, ni = h.Hi ? h.Hi : 1;
+    float lsum = 0.f;
+    if (blockIdx.x == 0 && threadIdx.x == 0) a.seg.totals[3] = 0;
+    // every group runs the same number of iterations so shuffles stay converged (a stride loop
+    // over base, not an iteration count: a 64-bit division here costs a stack frame)
+    for (int64_t base = 0; base < a.B; base += gstride) {
+        const int64_t b = base + gid;
+        const bool valid = b < a.B;
+        const int64_t bb = valid ? b : 0;
+        int64_t u = a.users[bb], i = a.items[bb];
+        const bool bad = u < 0 || u >= h.num_users || i < 0 || i >= h.num_items;
+        if (bad) { u = 0; i = 0; }
+        const float p = bloom_dot<LPR>(a, h, u, i, gl, gmask) + __ldg(a.bu + u) + __ldg(a.bi + i);
+        if (valid && gl == 0) {
+            float per, g;
+            rating_loss(a.loss, p, __ldg(a.ratings + bb), per, g);
+            lsum += per;
+            g *= invB;
+            if (bad) { atomicExch(a.err, 1); g = 0.f; }
+            if (a.pos_out) a.pos_out[bb] = p;
+            const bool live = h.idle_ids == 0 || g != 0.f;
+            h.ids_u2[bb] = live ? u : -1; h.g_u2[bb] = g;
+            h.ids_i2[bb] = live ? i : -1; h.g_i2[bb] = g;
+            const int64_t t0 = bb * nu * ni;
+            for (int ku = 0; ku < nu; ++ku) {
+                const int32_t ra = static_cast<int32_t>(hashed_row(u, ku, h.Hu, h.su, a.U, h.pad_u));
+                for (int ki = 0; ki < ni; ++ki) {
+                    const int32_t rb = static_cast<int32_t>(hashed_row(i, ki, h.Hi, h.si, a.I, h.pad_i));
+                    const int64_t t = t0 + ku * ni + ki;
+                    a.t_a[t] = ra; a.t_b[t] = rb; a.t_g[t] = g;
+                    if (g != 0.f) { atomicAdd(a.seg.cnt + ra, 1); atomicAdd(a.seg.cnt + a.U + rb, 1); }
+                }
+            }
+        }
+    }
+    float v;
+    if (grid_fold<MF_THREADS>(lsum, sh_red, is_last, a.partial, a.done, v)) { *a.loss_out = v * invB; *a.done = 0; }
+}
+
 struct MfLayout {
     int32_t* t_a; int32_t* t_b; float* t_g; float* partial; int32_t* done; int32_t* err;
     SegIndex seg;
@@ -1734,9 +1786,12 @@ struct BloomLayout {
     size_t bytes;
 };
 
+// scored sides per interaction: positive + negative, or the one rated pair of a rating loss
+static int bloom_sides(const slb_mf_bloom_args* x) { return is_rating_loss(x->base.loss) ? 1 : 2; }
+
 static BloomLayout bloom_layout(void* base, const slb_mf_bloom_args* x) {
     const int nu = x->user_hashes ? x->user_hashes : 1, ni = x->item_hashes ? x->item_hashes : 1;
-    const int64_t B = x->base.batch, T = 2 * B * nu * ni;
+    const int64_t B = x->base.batch, P = bloom_sides(x) * B, T = P * nu * ni;
     WsCarver ws(base);
     BloomLayout l;
     l.done = ws.take<int32_t>(8);
@@ -1746,22 +1801,22 @@ static BloomLayout bloom_layout(void* base, const slb_mf_bloom_args* x) {
     l.t_b = ws.take<int32_t>(T);
     l.t_g = ws.take<float>(T);
     l.partial = ws.take<float>(MF_MAX_GRID);
-    l.ids_u2 = ws.take<int64_t>(2 * B);
-    l.ids_i2 = ws.take<int64_t>(2 * B);
-    l.g_u2 = ws.take<float>(2 * B);
-    l.g_i2 = ws.take<float>(2 * B);
+    l.ids_u2 = ws.take<int64_t>(P);
+    l.ids_i2 = ws.take<int64_t>(P);
+    l.g_u2 = ws.take<float>(P);
+    l.g_i2 = ws.take<float>(P);
     l.irows = nullptr; l.gWi = nullptr; l.compact_counts = nullptr; l.bws_u = nullptr; l.bws_i = nullptr;
     l.ws_u = nullptr; l.ws_i = nullptr; l.ws_u_bytes = 0; l.ws_i_bytes = 0;
     if (x->base.opt == SLB_OPT_NONE) {
-        l.ws_u_bytes = slb_embedding_backward_workspace_bytes(2 * B, x->base.num_users);
+        l.ws_u_bytes = slb_embedding_backward_workspace_bytes(P, x->base.num_users);
         l.ws_u = ws.take<char>(l.ws_u_bytes);
-        l.ws_i_bytes = slb_embedding_backward_workspace_bytes(2 * B, x->base.num_items);
+        l.ws_i_bytes = slb_embedding_backward_workspace_bytes(P, x->base.num_items);
         l.ws_i = ws.take<char>(l.ws_i_bytes);
     } else {
         // the two bias workspaces are zero-at-rest and must precede the batch-sized scratch?  No:
         // this workspace is dedicated to one (shapes, batch), so every offset is fixed.
-        l.bws_u = ws.take<char>(bias_sparse_bytes(2 * B));
-        l.bws_i = ws.take<char>(bias_sparse_bytes(2 * B));
+        l.bws_u = ws.take<char>(bias_sparse_bytes(P));
+        l.bws_i = ws.take<char>(bias_sparse_bytes(P));
         const int64_t irow_cap = T < x->item_rows ? T : x->item_rows;
         l.irows = ws.take<int64_t>(irow_cap + 1);
         l.gWi = ws.take<float>(static_cast<size_t>(irow_cap + 1) * x->base.dim);
@@ -1782,8 +1837,15 @@ int slb_mf_bloom_train_step(const slb_mf_bloom_args* x, slb_stream_t stream) {
     SLB_REQUIRE(x != nullptr, "mf_bloom_train_step: null args");
     const slb_mf_step_args& b = x->base;
     SLB_REQUIRE(b.batch > 0 && b.dim >= 4 && b.dim % 4 == 0, "mf_bloom_train_step: bad batch / dim");
-    SLB_REQUIRE(b.loss >= 0 && b.loss <= 3 && b.n_neg >= 1, "mf_bloom_train_step: bad loss / n_neg");
+    SLB_REQUIRE(b.loss >= 0 && b.loss <= SLB_LOSS_LOGISTIC && b.n_neg >= 1, "mf_bloom_train_step: bad loss / n_neg");
     SLB_REQUIRE(b.loss == SLB_LOSS_ADAPTIVE_HINGE || b.n_neg == 1, "mf_bloom_train_step: n_neg > 1 only for adaptive hinge");
+    const bool rating = is_rating_loss(b.loss);
+    const bool pairs_u = x->pair_ids_u && x->pair_g_u, pairs_i = x->pair_ids_i && x->pair_g_i;
+    if (rating) {
+        SLB_REQUIRE(b.ratings && !b.negs && !b.neg_out, "mf_bloom_train_step: rating losses need ratings and take no negatives");
+        SLB_REQUIRE(!x->pair_ids_u && !x->pair_g_u && !x->pair_ids_i && !x->pair_g_i,
+                    "mf_bloom_train_step: rating losses write no bias pairs");
+    }
     const bool fused = b.opt != SLB_OPT_NONE;
     SLB_REQUIRE(fused ? (b.opt == SLB_OPT_SGD || b.opt == SLB_OPT_ADAGRAD) : b.grad_mode == SLB_GRAD_DENSE,
                 "mf_bloom_train_step: dense gradients, or a fused SGD / Adagrad optimizer");
@@ -1794,11 +1856,10 @@ int slb_mf_bloom_train_step(const slb_mf_bloom_args* x, slb_stream_t stream) {
     SLB_REQUIRE(x->user_rows > 0 && x->item_rows > 0 && b.num_users > 0 && b.num_items > 0, "mf_bloom_train_step: empty tables");
     SLB_REQUIRE(x->user_hashes > 0 || x->user_rows == b.num_users, "mf_bloom_train_step: plain user table must have num_users rows");
     SLB_REQUIRE(x->item_hashes > 0 || x->item_rows == b.num_items, "mf_bloom_train_step: plain item table must have num_items rows");
-    const bool pairs_u = x->pair_ids_u && x->pair_g_u, pairs_i = x->pair_ids_i && x->pair_g_i;
-    SLB_REQUIRE(b.users && b.items && b.negs && b.Wu && b.Wi && b.bu && b.bi && b.loss_out && b.workspace &&
+    SLB_REQUIRE(b.users && b.items && (rating || b.negs) && b.Wu && b.Wi && b.bu && b.bi && b.loss_out && b.workspace &&
                 (fused || (b.dWu && b.dWi && (b.dbu || pairs_u) && (b.dbi || pairs_i))), "mf_bloom_train_step: null pointer");
     const int nu = x->user_hashes ? x->user_hashes : 1, ni = x->item_hashes ? x->item_hashes : 1;
-    const int64_t B = b.batch, T = 2 * B * nu * ni;
+    const int64_t B = b.batch, P = bloom_sides(x) * B, T = P * nu * ni;
     SLB_REQUIRE(x->user_rows + x->item_rows < (1ll << 31) - SEG_SCAN_TILE && 2 * T < (1ll << 31),
                 "mf_bloom_train_step: too large");
     BloomLayout l = bloom_layout(b.workspace, x);
@@ -1809,7 +1870,7 @@ int slb_mf_bloom_train_step(const slb_mf_bloom_args* x, slb_stream_t stream) {
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     MfDev a = {};
     a.B = B; a.NB = b.norm_batch > 0 ? b.norm_batch : B; a.T = T;
-    a.users = b.users; a.items = b.items; a.negs = b.negs; a.loss = b.loss; a.n_neg = b.n_neg;
+    a.users = b.users; a.items = b.items; a.negs = b.negs; a.ratings = b.ratings; a.loss = b.loss; a.n_neg = b.n_neg;
     a.U = x->user_rows; a.I = x->item_rows; a.D = b.dim;      // key spaces = table rows
     a.Wu = b.Wu; a.Wi = b.Wi; a.bu = b.bu; a.bi = b.bi;
     a.loss_out = b.loss_out; a.pos_out = b.pos_out; a.neg_out = b.neg_out;
@@ -1837,8 +1898,13 @@ int slb_mf_bloom_train_step(const slb_mf_bloom_args* x, slb_stream_t stream) {
 
     const int groups = MF_THREADS / lpr;
     const int grid = min(slb_grid((B + groups - 1) / groups, 8), MF_MAX_GRID);
-    with_lpr(lpr, [&](auto L) { mf_fwd_bloom_kernel<L><<<grid, MF_THREADS, 0, st>>>(a, h); });
-    SLB_LAUNCH_CHECK("mf_fwd_bloom_kernel");
+    if (rating) {
+        with_lpr(lpr, [&](auto L) { mf_fwd_bloom_rating_kernel<L><<<grid, MF_THREADS, 0, st>>>(a, h); });
+        SLB_LAUNCH_CHECK("mf_fwd_bloom_rating_kernel");
+    } else {
+        with_lpr(lpr, [&](auto L) { mf_fwd_bloom_kernel<L><<<grid, MF_THREADS, 0, st>>>(a, h); });
+        SLB_LAUNCH_CHECK("mf_fwd_bloom_kernel");
+    }
     seg_scan_launch(a.seg, a.U, st);
     SLB_LAUNCH_CHECK("seg_scan_kernel");
     mf_fill_kernel<<<slb_grid((T + 255) / 256, 8), 256, 0, st>>>(a);
@@ -1858,10 +1924,10 @@ int slb_mf_bloom_train_step(const slb_mf_bloom_args* x, slb_stream_t stream) {
         const int agrid = slb_grid((2 * T + groups - 1) / groups, 8);
         with_lpr(lpr, [&](auto L) { mf_apply_kernel<L, 1><<<agrid, MF_THREADS, 0, st>>>(a); });
         SLB_LAUNCH_CHECK("mf_apply_kernel<items>");
-        int rcb = bias_sparse_apply(l.bws_u, l.ids_u2, l.g_u2, 2 * B, b.bu, b.state_bu, b.opt, b.lr, b.weight_decay,
+        int rcb = bias_sparse_apply(l.bws_u, l.ids_u2, l.g_u2, P, b.bu, b.state_bu, b.opt, b.lr, b.weight_decay,
                                     b.eps, true, st);
         if (rcb != SLB_OK) return rcb;
-        return bias_sparse_apply(l.bws_i, l.ids_i2, l.g_i2, 2 * B, b.bi, b.state_bi, b.opt, b.lr, b.weight_decay,
+        return bias_sparse_apply(l.bws_i, l.ids_i2, l.g_i2, P, b.bi, b.state_bi, b.opt, b.lr, b.weight_decay,
                                  b.eps, true, st);
     }
     launch_bwd_tile<0>(a, lpr, false, tgrid, st);
@@ -1871,11 +1937,11 @@ int slb_mf_bloom_train_step(const slb_mf_bloom_args* x, slb_stream_t stream) {
     // id-space bias gradients: deterministic scalar scatter (D = 1), unless handed out as pairs
     int rc = SLB_OK;
     if (!pairs_u)
-        rc = slb_embedding_backward(l.g_u2, l.ids_u2, 2 * B, 0, nullptr, b.num_users, 1, -1, b.dbu, l.ws_u,
+        rc = slb_embedding_backward(l.g_u2, l.ids_u2, P, 0, nullptr, b.num_users, 1, -1, b.dbu, l.ws_u,
                                     l.ws_u_bytes, stream);
     if (rc != SLB_OK) return rc;
     if (!pairs_i)
-        rc = slb_embedding_backward(l.g_i2, l.ids_i2, 2 * B, 0, nullptr, b.num_items, 1, -1, b.dbi, l.ws_i,
+        rc = slb_embedding_backward(l.g_i2, l.ids_i2, P, 0, nullptr, b.num_items, 1, -1, b.dbi, l.ws_i,
                                     l.ws_i_bytes, stream);
     return rc;
 }

@@ -10,7 +10,7 @@ Losses (spotlight/losses.py:169-244), on the score ``s`` of each rated pair:
 There are no negatives: each epoch consumes the ``RandomState`` only through one
 ``shuffle`` of ``arange(n)``, exactly as the reference does.
 
-Three routes, chosen per model, as in :mod:`spotlight_b200.factorization.implicit`:
+Four routes, chosen per model, as in :mod:`spotlight_b200.factorization.implicit`:
 
 ``epoch pipeline``   BilinearNet with plain tables + a fused optimizer (including the
                      default :class:`~spotlight_b200.optim.FusedAdam`): the whole epoch is
@@ -21,8 +21,14 @@ Three routes, chosen per model, as in :mod:`spotlight_b200.factorization.implici
                      first-generation kernels.
 ``fused autograd``   BilinearNet with plain tables + any ``torch.optim`` optimizer: one
                      fused op per minibatch fills dense ``.grad``.
-``generic``          custom ``representation`` / Bloom layers: the reference's loop over
-                     ``net(...)`` and this package's rating losses.
+``bloom``            BilinearNet with ``BloomEmbedding`` user and / or item layers + fused SGD /
+                     Adagrad: one fused hashed-table step per minibatch updates the rows it
+                     touches in place (no dense gradient); the host reads the per-batch
+                     losses once per epoch.  As on the other fused routes, weight decay
+                     applies to the touched rows only.
+``generic``          custom ``representation``, sparse models, and Bloom layers under any
+                     other optimizer: the reference's loop over ``net(...)`` and this
+                     package's rating losses.
 
 Ratings go to the device once per ``fit()`` as float32.  A float64 rating array is
 therefore trained in float32 (the reference promotes the loss to float64); integer-valued
@@ -141,11 +147,15 @@ class ExplicitFactorizationModel(object):
 
     def _route(self):
         net = self._net
+        fused_kind = getattr(self._optimizer, 'fused_kind', None)
         fusable = isinstance(net, BilinearNet) and net.plain_tables()
-        if fusable and getattr(self._optimizer, 'fused_kind', None) is not None:
+        if fusable and fused_kind is not None:
             return 'epoch'
         if fusable and not self._sparse:
             return 'fused'
+        if isinstance(net, BilinearNet) and not self._sparse and net.fused_spec() is not None and \
+                fused_kind in (_lib.OPT_SGD, _lib.OPT_ADAGRAD):
+            return 'bloom'
         return 'generic'
 
     def _device(self):
@@ -228,6 +238,8 @@ class ExplicitFactorizationModel(object):
                     with torch.cuda.stream(side):
                         pending = (shuffle_begin(n, self._random_state, device), side)
                 epoch_loss = self._fit_epoch_pipeline(users_t, items_t, ratings_t)
+            elif route == 'bloom':
+                epoch_loss = self._fit_epoch_bloom_fused(users_t, items_t, ratings_t)
             else:
                 epoch_loss = self._fit_epoch_autograd(users_t, items_t, ratings_t, route)
 
@@ -300,6 +312,24 @@ class ExplicitFactorizationModel(object):
             if ops.workspace_error_flag(ws):
                 raise ValueError('ids out of range reached the device kernels')
         return float(host.sum() / n_steps)
+
+    def _fit_epoch_bloom_fused(self, users, items, ratings):
+        """Hashed-table model with fused SGD / Adagrad: one in-place step per minibatch
+        (csrc/mf.cu slb_mf_bloom_train_step with a rating loss), no dense gradient of any table;
+        returns the mean of the per-batch losses (explicit.py:231,236)."""
+        net, opt = self._net, self._optimizer
+        spec = net.fused_spec()
+        hp = opt.fused_hparams()
+        params = (spec['Wu'], spec['Wi'], net.user_biases.weight, net.item_biases.weight)
+        states = [opt.fused_state(p) for p in params] if opt.fused_kind == _lib.OPT_ADAGRAD else None
+        losses = []
+        for batch_user, batch_item, batch_ratings in minibatch(users, items, ratings, batch_size=self._batch_size):
+            losses.append(ops.mf_bloom_train_step_inplace(
+                *params, batch_user, batch_item, None, self._loss, 1, spec['user_seeds'], spec['item_seeds'],
+                spec['user_pad'], spec['item_pad'], opt.fused_kind, hp['lr'], states, hp['weight_decay'],
+                hp['eps'], ratings=batch_ratings))
+        host = torch.stack(losses).cpu().numpy().astype(np.float64)        # one sync per epoch
+        return float(host.sum() / len(host))
 
     def _fit_epoch_autograd(self, users, items, ratings, route):
         net = self._net

@@ -352,6 +352,69 @@ def mf_train_step_inplace(Wu, Wi, bu, bi, users, items, negs, loss, opt_kind, lr
     return loss_out.reshape(())
 
 
+def _bloom_args(Wu, Wi, bu, bi, users, items, negs, ratings, loss, n_neg, user_seeds, item_seeds, user_pad,
+                item_pad):
+    """A filled ``slb_mf_bloom_args`` (tables, hashes, minibatch); the caller adds outputs and the
+    optimizer, then :func:`_bloom_workspace`.  Pairwise losses pass ``negs``, rating losses
+    ``ratings`` (the other None)."""
+    x = MfBloomArgs()
+    a = x.base
+    a.batch = users.numel()
+    a.users, a.items = users.data_ptr(), items.data_ptr()
+    a.negs = negs.data_ptr() if negs is not None else None
+    a.ratings = ratings.data_ptr() if ratings is not None else None
+    a.loss = LOSS_KIND[loss] if isinstance(loss, str) else int(loss)
+    a.n_neg = int(n_neg)
+    a.num_users, a.num_items, a.dim = bu.shape[0], bi.shape[0], Wu.shape[1]
+    a.Wu, a.Wi, a.bu, a.bi = Wu.data_ptr(), Wi.data_ptr(), bu.data_ptr(), bi.data_ptr()
+    x.user_rows, x.item_rows = Wu.shape[0], Wi.shape[0]
+    x.user_hashes, x.item_hashes = len(user_seeds), len(item_seeds)
+    for k, sd in enumerate(user_seeds):
+        x.user_seeds[k] = int(sd) & 0xFFFFFFFF
+    for k, sd in enumerate(item_seeds):
+        x.item_seeds[k] = int(sd) & 0xFFFFFFFF
+    x.user_padding_idx, x.item_padding_idx = int(user_pad), int(item_pad)
+    return x
+
+
+def _bloom_workspace(kind, x, dev):
+    """Attach the workspace of ``x``: one per (kind, shapes, hash counts, loss family, batch),
+    because its zero-at-rest regions are layout dependent and a rating loss lays out one scored
+    side per interaction where a pairwise loss lays out two."""
+    a = x.base
+    family = 'rating' if a.loss >= LOSS_KIND['regression'] else 'pairwise'
+    ws = workspace('%s_%s_%d_%d_%d_%d_%d_%d_%d' % (kind, family, x.user_rows, x.item_rows, a.num_users, a.num_items,
+                                                   x.user_hashes, x.item_hashes, a.batch),
+                   _lib.load().slb_mf_bloom_workspace_bytes(ctypes.byref(x)), dev)
+    a.workspace, a.workspace_bytes = ws.data_ptr(), ws.numel()
+    return ws
+
+
+def _bloom_dense_step(Wu, Wi, bu, bi, users, items, negs, ratings, loss, n_neg, user_seeds, item_seeds,
+                      user_pad, item_pad, want_scores):
+    """The hashed-table step with dense gradients: (loss, pos, neg, dWu, dWi, dbu, dbi)."""
+    Wu, Wi, bu, bi = _f32c(Wu), _f32c(Wi), _f32c(bu), _f32c(bi)
+    B = users.numel()
+    dev = Wu.device
+    x = _bloom_args(Wu, Wi, bu, bi, users, items, negs, ratings, loss, n_neg, user_seeds, item_seeds, user_pad,
+                    item_pad)
+    a = x.base
+    loss_out = torch.empty(1, dtype=torch.float32, device=dev)
+    pos = torch.empty(B if want_scores else 0, dtype=torch.float32, device=dev)
+    neg = torch.empty(B * n_neg if want_scores and negs is not None else 0, dtype=torch.float32, device=dev)
+    dWu, dWi = torch.zeros_like(Wu), torch.zeros_like(Wi)
+    dbu, dbi = torch.zeros_like(bu), torch.zeros_like(bi)
+    a.loss_out = loss_out.data_ptr()
+    if want_scores:
+        a.pos_out = pos.data_ptr()
+        a.neg_out = neg.data_ptr() if negs is not None else None
+    a.grad_mode = _lib.GRAD_DENSE
+    a.dWu, a.dWi, a.dbu, a.dbi = dWu.data_ptr(), dWi.data_ptr(), dbu.data_ptr(), dbi.data_ptr()
+    _bloom_workspace('mfb', x, dev)
+    _lib.check(_lib.load().slb_mf_bloom_train_step(ctypes.byref(x), _stream()), 'mf_bloom_train_step')
+    return loss_out.reshape(()), pos, neg, dWu, dWi, dbu, dbi
+
+
 @torch.library.custom_op('spotlight_b200::mf_bloom_train_step', mutates_args=())
 def mf_bloom_train_step(Wu: Tensor, Wi: Tensor, bu: Tensor, bi: Tensor, users: Tensor, items: Tensor,
                         negs: Tensor, loss: int, n_neg: int, user_seeds: List[int],
@@ -361,44 +424,12 @@ def mf_bloom_train_step(Wu: Tensor, Wi: Tensor, bu: Tensor, bi: Tensor, users: T
     = plain table).  Wu / Wi are the (hashed) embedding tables, bu / bi the id-indexed
     biases.  Returns (loss, pos, neg, dWu, dWi, dbu, dbi), dense."""
     require_cuda(Wu, Wi, bu, bi, users, items, negs)
-    lib = _lib.load()
-    Wu, Wi, bu, bi = _f32c(Wu), _f32c(Wi), _f32c(bu), _f32c(bi)
     users, items, negs = _i64c(users).reshape(-1), _i64c(items).reshape(-1), _i64c(negs).reshape(-1)
     B = users.numel()
     if items.numel() != B or negs.numel() != B * n_neg:
         raise ValueError('mf_bloom_train_step: inconsistent batch sizes')
-    dev = Wu.device
-    x = MfBloomArgs()
-    a = x.base
-    a.batch = B
-    a.users, a.items, a.negs = users.data_ptr(), items.data_ptr(), negs.data_ptr()
-    a.loss, a.n_neg = loss, n_neg
-    a.num_users, a.num_items, a.dim = bu.shape[0], bi.shape[0], Wu.shape[1]
-    a.Wu, a.Wi, a.bu, a.bi = Wu.data_ptr(), Wi.data_ptr(), bu.data_ptr(), bi.data_ptr()
-    loss_out = torch.empty(1, dtype=torch.float32, device=dev)
-    pos = torch.empty(B if want_scores else 0, dtype=torch.float32, device=dev)
-    neg = torch.empty(B * n_neg if want_scores else 0, dtype=torch.float32, device=dev)
-    dWu, dWi = torch.zeros_like(Wu), torch.zeros_like(Wi)
-    dbu, dbi = torch.zeros_like(bu), torch.zeros_like(bi)
-    a.loss_out = loss_out.data_ptr()
-    if want_scores:
-        a.pos_out, a.neg_out = pos.data_ptr(), neg.data_ptr()
-    a.grad_mode = _lib.GRAD_DENSE
-    a.dWu, a.dWi, a.dbu, a.dbi = dWu.data_ptr(), dWi.data_ptr(), dbu.data_ptr(), dbi.data_ptr()
-    x.user_rows, x.item_rows = Wu.shape[0], Wi.shape[0]
-    x.user_hashes, x.item_hashes = len(user_seeds), len(item_seeds)
-    for k, sd in enumerate(user_seeds):
-        x.user_seeds[k] = int(sd) & 0xFFFFFFFF
-    for k, sd in enumerate(item_seeds):
-        x.item_seeds[k] = int(sd) & 0xFFFFFFFF
-    x.user_padding_idx, x.item_padding_idx = user_pad, item_pad
-    need = lib.slb_mf_bloom_workspace_bytes(ctypes.byref(x))
-    # one workspace per (shapes, batch): its zero-at-rest regions are layout dependent
-    ws = workspace('mfb%d_%d_%d_%d_%d_%d_%d' % (Wu.shape[0], Wi.shape[0], bu.shape[0], bi.shape[0],
-                                                len(user_seeds), len(item_seeds), B), need, dev)
-    a.workspace, a.workspace_bytes = ws.data_ptr(), ws.numel()
-    _lib.check(lib.slb_mf_bloom_train_step(ctypes.byref(x), _stream()), 'mf_bloom_train_step')
-    return loss_out.reshape(()), pos, neg, dWu, dWi, dbu, dbi
+    return _bloom_dense_step(Wu, Wi, bu, bi, users, items, negs, None, loss, n_neg, user_seeds, item_seeds,
+                             user_pad, item_pad, want_scores)
 
 
 @mf_bloom_train_step.register_fake
@@ -410,43 +441,59 @@ def _(Wu, Wi, bu, bi, users, items, negs, loss, n_neg, user_seeds, item_seeds, u
             torch.empty_like(Wu), torch.empty_like(Wi), torch.empty_like(bu), torch.empty_like(bi))
 
 
+@torch.library.custom_op('spotlight_b200::mf_bloom_rating_step', mutates_args=())
+def mf_bloom_rating_step(Wu: Tensor, Wi: Tensor, bu: Tensor, bi: Tensor, users: Tensor, items: Tensor,
+                         ratings: Tensor, loss: int, user_seeds: List[int], item_seeds: List[int], user_pad: int,
+                         item_pad: int, want_scores: bool
+                         ) -> Tuple[Tensor, Tensor, Tensor, Tensor, Tensor, Tensor]:
+    """Fused explicit-feedback step (regression / poisson / logistic) for BilinearNet with
+    BloomEmbedding user / item layers (empty seed list = plain table), dense gradients.
+    Returns (loss, scores, dWu, dWi, dbu, dbi); ``scores`` (the raw BilinearNet output) is empty
+    unless ``want_scores``."""
+    require_cuda(Wu, Wi, bu, bi, users, items, ratings)
+    users, items = _i64c(users).reshape(-1), _i64c(items).reshape(-1)
+    ratings = _f32c(ratings).reshape(-1)
+    B = users.numel()
+    if items.numel() != B or ratings.numel() != B:
+        raise ValueError('mf_bloom_rating_step: inconsistent batch sizes')
+    out = _bloom_dense_step(Wu, Wi, bu, bi, users, items, None, ratings, loss, 1, user_seeds, item_seeds,
+                            user_pad, item_pad, want_scores)
+    return out[:2] + out[3:]
+
+
+@mf_bloom_rating_step.register_fake
+def _(Wu, Wi, bu, bi, users, items, ratings, loss, user_seeds, item_seeds, user_pad, item_pad, want_scores):
+    B = users.numel()
+    return (Wu.new_empty(()), Wu.new_empty((B if want_scores else 0,)),
+            torch.empty_like(Wu), torch.empty_like(Wi), torch.empty_like(bu), torch.empty_like(bi))
+
+
 def mf_bloom_train_step_inplace(Wu, Wi, bu, bi, users, items, negs, loss, n_neg, user_seeds, item_seeds,
-                                user_pad, item_pad, opt_kind, lr, states=None, weight_decay=0.0, eps=1e-10):
+                                user_pad, item_pad, opt_kind, lr, states=None, weight_decay=0.0, eps=1e-10,
+                                ratings=None):
     """The fused hashed-table step with the row-wise optimizer applied in place: hashed / plain
     embedding rows through the compact-gradient kernels, the id-indexed bias tables through the
     hash-bucket sparse update (no dense gradient anywhere -- the item-bias table of BASELINE
-    config 4 has 50 M rows).  ``states`` = (sWu, sWi, sbu, sbi) for Adagrad.  Returns the loss."""
-    require_cuda(Wu, Wi, bu, bi, users, items, negs)
-    lib = _lib.load()
-    users, items, negs = _i64c(users).reshape(-1), _i64c(items).reshape(-1), _i64c(negs).reshape(-1)
-    B = users.numel()
+    config 4 has 50 M rows).  ``states`` = (sWu, sWi, sbu, sbi) for Adagrad.  Rating losses pass
+    ``negs=None``, ``n_neg=1`` and ``ratings`` (spotlight/factorization/explicit.py:223-234).
+    Returns the loss."""
+    require_cuda(Wu, Wi, bu, bi, users, items, negs, ratings)
+    users, items = _i64c(users).reshape(-1), _i64c(items).reshape(-1)
+    negs = _i64c(negs).reshape(-1) if negs is not None else None
+    ratings = _f32c(ratings).reshape(-1) if ratings is not None else None
     dev = Wu.device
     with torch.no_grad():
-        x = MfBloomArgs()
+        x = _bloom_args(Wu, Wi, bu, bi, users, items, negs, ratings, loss, n_neg, user_seeds, item_seeds, user_pad,
+                        item_pad)
         a = x.base
-        a.batch = B
-        a.users, a.items, a.negs = users.data_ptr(), items.data_ptr(), negs.data_ptr()
-        a.loss, a.n_neg = (LOSS_KIND[loss] if isinstance(loss, str) else int(loss)), int(n_neg)
-        a.num_users, a.num_items, a.dim = bu.shape[0], bi.shape[0], Wu.shape[1]
-        a.Wu, a.Wi, a.bu, a.bi = Wu.data_ptr(), Wi.data_ptr(), bu.data_ptr(), bi.data_ptr()
         loss_out = torch.empty(1, dtype=torch.float32, device=dev)
         a.loss_out = loss_out.data_ptr()
         a.grad_mode = _lib.GRAD_COMPACT
         a.opt, a.lr, a.weight_decay, a.eps = int(opt_kind), float(lr), float(weight_decay), float(eps)
         if opt_kind == _lib.OPT_ADAGRAD:
             a.state_Wu, a.state_Wi, a.state_bu, a.state_bi = [t.data_ptr() for t in states]
-        x.user_rows, x.item_rows = Wu.shape[0], Wi.shape[0]
-        x.user_hashes, x.item_hashes = len(user_seeds), len(item_seeds)
-        for k, sd in enumerate(user_seeds):
-            x.user_seeds[k] = int(sd) & 0xFFFFFFFF
-        for k, sd in enumerate(item_seeds):
-            x.item_seeds[k] = int(sd) & 0xFFFFFFFF
-        x.user_padding_idx, x.item_padding_idx = user_pad, item_pad
-        need = lib.slb_mf_bloom_workspace_bytes(ctypes.byref(x))
-        ws = workspace('mfbf%d_%d_%d_%d_%d_%d_%d_%d' % (Wu.shape[0], Wi.shape[0], bu.shape[0], bi.shape[0],
-                                                        len(user_seeds), len(item_seeds), B, a.n_neg), need, dev)
-        a.workspace, a.workspace_bytes = ws.data_ptr(), ws.numel()
-        _lib.check(lib.slb_mf_bloom_train_step(ctypes.byref(x), _stream()), 'mf_bloom_train_step')
+        _bloom_workspace('mfbf', x, dev)
+        _lib.check(_lib.load().slb_mf_bloom_train_step(ctypes.byref(x), _stream()), 'mf_bloom_train_step')
     return loss_out.reshape(())
 
 
