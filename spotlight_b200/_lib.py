@@ -34,6 +34,7 @@ EXPORTS = (
     'slb_embedding_backward_workspace_bytes', 'slb_embedding_backward',
     'slb_mf_scores', 'slb_mf_scores_backward', 'slb_rank_pairs', 'slb_rank_targets', 'slb_mf_step_workspace_bytes', 'slb_mf_fused_workspace_bytes', 'slb_mf_compact_rows',
     'slb_mf_train_step', 'slb_mf_train_step_phases', 'slb_mf_fit_epoch', 'slb_mf_fit_epoch_events', 'slb_adam_flush',
+    'slb_adam_flush_table',
     'slb_mf_bloom_workspace_bytes', 'slb_mf_bloom_train_step',
     'slb_bias_sparse_workspace_bytes', 'slb_bias_sparse_apply',
     'slb_unique_workspace_bytes', 'slb_unique_bucket', 'slb_shard_gather_batch', 'slb_adagrad_dense',
@@ -104,6 +105,9 @@ class SeqStepArgs(ctypes.Structure):
         ('num_mixtures', c_i32), ('mix_w', c_vp), ('mix_b', c_vp), ('dmix_w', c_vp), ('dmix_b', c_vp),
         ('item_rows', c_i64), ('item_hashes', c_i32), ('item_seeds', ctypes.c_uint32 * 24),
         ('item_padding_idx', c_i64),
+        ('beta1', c_f32), ('beta2', c_f32), ('one_minus_beta1', c_f32), ('one_minus_beta2', c_f32),
+        ('state2_E', c_vp), ('state2_bias', c_vp), ('last_E', c_vp), ('last_bias', c_vp),
+        ('adam_sched', c_vp), ('adam_step', c_i64),
     ]
 
 
@@ -163,6 +167,8 @@ def _declare(lib):
     lib.slb_mf_fit_epoch_events.argtypes = [P(MfStepArgs), c_vp, c_vp, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_i32]
     lib.slb_adam_flush.argtypes = [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_i32, c_vp, c_i64,
                                    c_f32, c_f32, c_f32, c_f32, c_f32, c_f32, c_vp]
+    lib.slb_adam_flush_table.argtypes = [c_vp, c_vp, c_vp, c_vp, c_i64, c_i32, c_vp, c_i64,
+                                         c_f32, c_f32, c_f32, c_f32, c_f32, c_f32, c_vp]
     lib.slb_unique_workspace_bytes.argtypes = [c_i64, c_i64]
     lib.slb_unique_workspace_bytes.restype = c_sz
     lib.slb_unique_bucket.argtypes = [c_vp, c_i64, c_i64, c_i64, c_i32, c_vp, c_vp, c_vp, c_vp, c_sz, c_vp]

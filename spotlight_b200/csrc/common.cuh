@@ -256,4 +256,43 @@ __device__ __forceinline__ void bias_update(const OptV2& o, float* bw, float* bs
     }
 }
 
+// ---- row-wise lazy-exact Adam shared by the MF (mf_adam.cuh) and sequence kernels -------------
+// Per-step scalars (computed by the host in double, as torch does):
+//   sched[2t] = lr / (1 - beta1^t)      sched[2t+1] = sqrt(1 - beta2^t)
+struct AdamDev {
+    float beta1, beta2, omb1, omb2, eps, wd;
+    const float* sched;       // [2 * (t_max + 1)]
+    int32_t t;                // this step (1-based)
+};
+
+// one Adam step on one element (torch/optim/adam.py, _single_tensor_adam / foreach form)
+__device__ __forceinline__ void adam_elem(const AdamDev& o, float ss, float bc2s, float g, float& w, float& m, float& v) {
+    g += o.wd * w;
+    m += (g - m) * o.omb1;                       // exp_avg.lerp_(grad, 1 - beta1)
+    v = v * o.beta2 + o.omb2 * g * g;            // mul_(beta2).addcmul_(grad, grad, 1 - beta2)
+    const float denom = sqrtf(v) / bc2s + o.eps;
+    w -= ss * (m / denom);                                  // addcdiv_(exp_avg, denom, value=-step_size)
+}
+
+// replay steps (from, to] with zero data gradient
+__device__ __forceinline__ void adam_catch_up(const AdamDev& o, int from, int to, float4& w, float4& m, float4& v) {
+    // a row that was never touched has m = v = 0: without weight decay nothing moves
+    if (from >= to) return;
+    if (o.wd == 0.f && m.x == 0.f && m.y == 0.f && m.z == 0.f && m.w == 0.f &&
+        v.x == 0.f && v.y == 0.f && v.z == 0.f && v.w == 0.f) return;
+    for (int s = from + 1; s <= to; ++s) {
+        const float ss = __ldg(o.sched + 2 * s), bc = __ldg(o.sched + 2 * s + 1);
+        adam_elem(o, ss, bc, 0.f, w.x, m.x, v.x);
+        adam_elem(o, ss, bc, 0.f, w.y, m.y, v.y);
+        adam_elem(o, ss, bc, 0.f, w.z, m.z, v.z);
+        adam_elem(o, ss, bc, 0.f, w.w, m.w, v.w);
+    }
+}
+
+__device__ __forceinline__ void adam_catch_up1(const AdamDev& o, int from, int to, float& w, float& m, float& v) {
+    if (from >= to || (o.wd == 0.f && m == 0.f && v == 0.f)) return;
+    for (int s = from + 1; s <= to; ++s)
+        adam_elem(o, __ldg(o.sched + 2 * s), __ldg(o.sched + 2 * s + 1), 0.f, w, m, v);
+}
+
 #endif  // __CUDACC__

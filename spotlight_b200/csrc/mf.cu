@@ -1610,6 +1610,25 @@ int slb_adam_flush(float* W, float* exp_avg, float* exp_avg_sq, float* bias, flo
     return SLB_OK;
 }
 
+int slb_adam_flush_table(float* W, float* exp_avg, float* exp_avg_sq, int32_t* last, int64_t rows, int32_t dim,
+                         const float* sched, int64_t step, float beta1, float beta2, float one_minus_beta1,
+                         float one_minus_beta2, float eps, float weight_decay, slb_stream_t stream) {
+    SLB_REQUIRE(W && exp_avg && exp_avg_sq && last && sched, "adam_flush_table: null pointer");
+    SLB_REQUIRE(rows > 0 && dim >= 1 && step >= 0 && step < (1ll << 31), "adam_flush_table: bad sizes");
+    if (step == 0) return SLB_OK;
+    AdamDev o = {beta1, beta2, one_minus_beta1, one_minus_beta2, eps, weight_decay, sched, static_cast<int32_t>(step)};
+    int lpr = 1;                                  // one element per lane: D lanes, a power of two, at most a warp
+    while (lpr < dim && lpr < 32) lpr <<= 1;
+    const int groups = MF_THREADS / lpr;
+    const int grid = slb_grid((rows + groups - 1) / groups, 16);
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    with_lpr(lpr, [&](auto L) {
+        adam_flush_table_kernel<L><<<grid, MF_THREADS, 0, st>>>(W, exp_avg, exp_avg_sq, last, rows, dim, o);
+    });
+    SLB_LAUNCH_CHECK("adam_flush_table_kernel");
+    return SLB_OK;
+}
+
 int slb_mf_scores(const float* Wu, const float* Wi, const float* bu, const float* bi,
                   int32_t dim, const int64_t* users, const int64_t* items, int64_t n,
                   int32_t user_broadcast, float* scores, slb_stream_t stream) {

@@ -10,46 +10,8 @@
 // replays the pending steps of every row (end of fit(), before parameters are read).  The
 // result equals dense Adam up to fp32 rounding of identical formulas; the cost per step is
 // O(touched rows x steps missed), never more arithmetic than the dense sweep did.
-//
-// Per-step scalars (computed by the host in double, as torch does):
-//   sched[2t] = lr / (1 - beta1^t)      sched[2t+1] = sqrt(1 - beta2^t)
+// The element recurrence and the catch-up (AdamDev, adam_elem, adam_catch_up) are in common.cuh.
 #pragma once
-
-struct AdamDev {
-    float beta1, beta2, omb1, omb2, eps, wd;
-    const float* sched;       // [2 * (t_max + 1)]
-    int32_t t;                // this step (1-based)
-};
-
-// one Adam step on one element (torch/optim/adam.py, _single_tensor_adam / foreach form)
-__device__ __forceinline__ void adam_elem(const AdamDev& o, float ss, float bc2s, float g, float& w, float& m, float& v) {
-    g += o.wd * w;
-    m += (g - m) * o.omb1;                       // exp_avg.lerp_(grad, 1 - beta1)
-    v = v * o.beta2 + o.omb2 * g * g;            // mul_(beta2).addcmul_(grad, grad, 1 - beta2)
-    const float denom = sqrtf(v) / bc2s + o.eps;
-    w -= ss * (m / denom);                                  // addcdiv_(exp_avg, denom, value=-step_size)
-}
-
-// replay steps (from, to] with zero data gradient
-__device__ __forceinline__ void adam_catch_up(const AdamDev& o, int from, int to, float4& w, float4& m, float4& v) {
-    // a row that was never touched has m = v = 0: without weight decay nothing moves
-    if (from >= to) return;
-    if (o.wd == 0.f && m.x == 0.f && m.y == 0.f && m.z == 0.f && m.w == 0.f &&
-        v.x == 0.f && v.y == 0.f && v.z == 0.f && v.w == 0.f) return;
-    for (int s = from + 1; s <= to; ++s) {
-        const float ss = __ldg(o.sched + 2 * s), bc = __ldg(o.sched + 2 * s + 1);
-        adam_elem(o, ss, bc, 0.f, w.x, m.x, v.x);
-        adam_elem(o, ss, bc, 0.f, w.y, m.y, v.y);
-        adam_elem(o, ss, bc, 0.f, w.z, m.z, v.z);
-        adam_elem(o, ss, bc, 0.f, w.w, m.w, v.w);
-    }
-}
-
-__device__ __forceinline__ void adam_catch_up1(const AdamDev& o, int from, int to, float& w, float& m, float& v) {
-    if (from >= to || (o.wd == 0.f && m == 0.f && v == 0.f)) return;
-    for (int s = from + 1; s <= to; ++s)
-        adam_elem(o, __ldg(o.sched + 2 * s), __ldg(o.sched + 2 * s + 1), 0.f, w, m, v);
-}
 
 // Before the forward pass of step t every row the minibatch references must be current through
 // step t-1 (dense Adam moved it at every step it missed, and the scores must see that).  One
@@ -164,5 +126,27 @@ adam_flush_kernel(float* W, float* M, float* V, float* bw, float* bm, float* bv,
             bw[row] = w; bm[row] = m; bv[row] = v;
             last[row] = o.t;
         }
+    }
+}
+
+// The same for one table with its own `last` and any width D >= 1 (a hashed table, an id-indexed
+// (rows, 1) bias): one lane group of LPR lanes per row, one element per lane at a time.
+template <int LPR>
+__global__ void __launch_bounds__(MF_THREADS)
+adam_flush_table_kernel(float* W, float* M, float* V, int32_t* last, int64_t rows, int D, AdamDev o) {
+    constexpr int GROUPS = MF_THREADS / LPR;
+    const int gl = threadIdx.x & (LPR - 1);
+    const int gib = threadIdx.x / LPR;
+    for (int64_t row = static_cast<int64_t>(blockIdx.x) * GROUPS + gib; row < rows; row += static_cast<int64_t>(gridDim.x) * GROUPS) {
+        const int lastv = last[row];
+        if (lastv >= o.t) continue;
+        for (int c = gl; c < D; c += LPR) {
+            const int64_t e = row * D + c;
+            float w = W[e], m = M[e], v = V[e];
+            adam_catch_up1(o, lastv, o.t, w, m, v);
+            W[e] = w; M[e] = m; V[e] = v;
+        }
+        __syncwarp(group_mask(LPR));          // every lane has read `last` before it moves
+        if (gl == 0) last[row] = o.t;
     }
 }

@@ -70,6 +70,9 @@ struct SeqDev {
     // Xs (B, S, D) holds the summed rows of the sequence positions, read by position
     int H; int64_t Mrows; uint32_t seeds[24];
     const float* Xs;
+    // lazy-exact Adam (SLB_OPT_ADAM): sE / sbias hold exp_avg, vE / vbias exp_avg_sq; lastE / lastb
+    // the step a table row / bias is current for (a plain table's bias shares lastE)
+    AdamDev ad; float* vE; float* vbias; int32_t* lastE; int32_t* lastb;
 };
 
 // Row source of the item reads: a plain table by id, or the hashed sum of the H rows of the
@@ -516,6 +519,147 @@ __global__ void __launch_bounds__(SQ_THREADS) seq_reduce_kernel(SeqDev a) {
         }
         if (gl == 0 && H == 0)
             bias_update(o, const_cast<float*>(a.bias) + row, a.opt == SLB_OPT_ADAGRAD ? a.sbias + row : nullptr, bacc);
+    }
+}
+
+// Lazy-exact Adam (SLB_OPT_ADAM) in place of seq_reduce_kernel's optimizers: the segment sum is
+// the same; the summed gradient of a row takes the real step t and the row's last becomes t.
+// seq_adam_prepass_kernel has made every keyed row current through t - 1.  A row whose terms are all
+// zero is skipped: a gradient-free step equals the catch-up it gets when next referenced or
+// flushed, so this stays dense Adam, weight decay included.  (A kernel of its own, so that the
+// SGD / Adagrad / gradient instantiations of seq_reduce_kernel keep their code.)
+template <int LPR, bool HASHED>
+__global__ void __launch_bounds__(SQ_THREADS) seq_reduce_adam_kernel(SeqDev a) {
+    constexpr int GROUPS = SQ_THREADS / LPR;
+    constexpr int CAP = seg_sort_cap(LPR);
+    constexpr int NCH = LPR == 32 ? 4 : 1;
+    __shared__ int32_t sh_sort[GROUPS * 2 * CAP];
+    const int gl = threadIdx.x & (LPR - 1);
+    const int gib = threadIdx.x / LPR;
+    const unsigned gmask = group_mask(LPR);
+    int32_t* sh = sh_sort + gib * 2 * CAP;
+    const int D = a.D;
+    const int H = HASHED ? a.H : 0;
+    const int64_t TH = 2 * a.B * a.S * H;
+    const int nseg = a.seg.totals[0];
+    const AdamDev o = a.ad;
+    for (int64_t s = static_cast<int64_t>(blockIdx.x) * GROUPS + gib; s < nseg;
+         s += static_cast<int64_t>(gridDim.x) * GROUPS) {
+        const int start = a.seg.seg_start[s];
+        const int len = a.seg.seg_start[s + 1] - start;
+        const int64_t row = a.seg.seg_row[s];
+        const bool bseg = H > 0 && row >= a.Mrows;
+        float4 acc[NCH];
+#pragma unroll
+        for (int q = 0; q < NCH; ++q) acc[q] = make_float4(0, 0, 0, 0);
+        float bacc = 0.f;
+        bool nz = false;
+        seg_visit_sorted<LPR>(a.seg.members, start, len, gl, gmask, sh, [&](int32_t m) {
+            const int64_t t = H == 0 ? m : (bseg ? m - TH : m / H);
+            if (!bseg) {
+                const float* src = a.C + t * D;
+#pragma unroll
+                for (int q = 0; q < NCH; ++q) {
+                    const int c = gl * 4 + q * LPR * 4;
+                    if (c < D) {
+                        const float4 v = ld4(src + c);
+                        acc[q].x += v.x; acc[q].y += v.y; acc[q].z += v.z; acc[q].w += v.w;
+                    }
+                }
+            }
+            const float g = a.gs[t];
+            bacc += g;
+            nz = nz || g != 0.f;
+        }, HASHED);
+        // the bias of a plain row (shares the row's last), or of a hashed bias segment (its own)
+        const int64_t bid = bseg ? row - a.Mrows : row;
+        float ss, bc;                         // this step's scalars, loaded where they are used
+        if (!bseg) {
+#pragma unroll
+            for (int q = 0; q < NCH; ++q)
+                nz = nz || acc[q].x != 0.f || acc[q].y != 0.f || acc[q].z != 0.f || acc[q].w != 0.f;
+            if (!__any_sync(gmask, nz)) continue;   // group-uniform
+            ss = __ldg(o.sched + 2 * o.t); bc = __ldg(o.sched + 2 * o.t + 1);
+#pragma unroll
+            for (int q = 0; q < NCH; ++q) {
+                const int c = gl * 4 + q * LPR * 4;
+                if (c < D) {
+                    float* W = const_cast<float*>(a.E) + row * D + c;
+                    float4 w = ld4(W), m = ld4(a.sE + row * D + c), v = ld4(a.vE + row * D + c);
+                    adam_elem(o, ss, bc, acc[q].x, w.x, m.x, v.x);
+                    adam_elem(o, ss, bc, acc[q].y, w.y, m.y, v.y);
+                    adam_elem(o, ss, bc, acc[q].z, w.z, m.z, v.z);
+                    adam_elem(o, ss, bc, acc[q].w, w.w, m.w, v.w);
+                    st4(W, w); st4(a.sE + row * D + c, m); st4(a.vE + row * D + c, v);
+                }
+            }
+            if (gl == 0) a.lastE[row] = o.t;
+        } else if (!nz) {
+            continue;
+        } else {
+            ss = __ldg(o.sched + 2 * o.t); bc = __ldg(o.sched + 2 * o.t + 1);
+        }
+        if (gl == 0 && (H == 0 || bseg)) {
+            float* bw = const_cast<float*>(a.bias) + bid;
+            float w = *bw, m = a.sbias[bid], v = a.vbias[bid];
+            adam_elem(o, ss, bc, bacc, w, m, v);
+            *bw = w; a.sbias[bid] = m; a.vbias[bid] = v;
+            if (bseg) a.lastb[bid] = o.t;
+        }
+    }
+}
+
+// Lazy-exact Adam, before anything in step t reads E: every row the minibatch references is
+// brought current through step t - 1 (dense Adam moved it at every step it missed, and the
+// representation and the scores must see that).  References: each sequence position (its item is
+// both an input and a target) and each negative; on a hashed table each of the id's H rows (work
+// slot k < H) and the id's bias (slot H).  The padding id is caught up like any other: dense Adam
+// with weight decay moves its row, whose gradient is zero.  atomicMax on last elects one lane group
+// per distinct row, as mf_adam_prepass_kernel does.
+template <int LPR, bool HASHED>
+__global__ void __launch_bounds__(SQ_THREADS) seq_adam_prepass_kernel(SeqDev a) {
+    constexpr int GROUPS = SQ_THREADS / LPR;
+    __shared__ uint32_t sh_seeds[24];
+    if (HASHED && threadIdx.x == 0) {
+#pragma unroll
+        for (int k = 0; k < 24; ++k) sh_seeds[k] = a.seeds[k];   // static indices: the seeds stay in the parameter bank
+    }
+    if (HASHED) __syncthreads();
+    const int gl = threadIdx.x & (LPR - 1);
+    const unsigned gmask = group_mask(LPR);
+    const int D = a.D;
+    const int upto = a.ad.t - 1;
+    const int64_t BS = a.B * a.S;
+    const int slots = HASHED ? a.H + 1 : 1;
+    const int64_t total = BS * (1 + a.n_neg) * slots;
+    for (int64_t w = static_cast<int64_t>(blockIdx.x) * GROUPS + threadIdx.x / LPR; w < total;
+         w += static_cast<int64_t>(gridDim.x) * GROUPS) {
+        const int64_t r = HASHED ? w / slots : w;
+        const int k = HASHED ? static_cast<int>(w - r * slots) : 0;
+        const int64_t id = clamp_id(r < BS ? a.seqs[r] : a.negs[r - BS], a.I);   // seq_mask_kernel flags bad ids
+        const bool bslot = HASHED && k == a.H;                                   // group-uniform
+        const int64_t row = (HASHED && !bslot) ? bloom_row(id, sh_seeds[k], a.Mrows, 0) : id;
+        int32_t* last = (bslot ? a.lastb : a.lastE) + row;
+        int old = 0;
+        if (gl == 0) old = atomicMax(last, upto);
+        old = __shfl_sync(gmask, old, (threadIdx.x & 31) & ~(LPR - 1));
+        if (old >= upto) continue;
+        if (!bslot) {
+            float* W = const_cast<float*>(a.E) + row * D;
+            float* M = a.sE + row * D;
+            float* V = a.vE + row * D;
+            for (int c = gl * 4; c < D; c += LPR * 4) {
+                float4 wv = ld4(W + c), m = ld4(M + c), v = ld4(V + c);
+                adam_catch_up(a.ad, old, upto, wv, m, v);
+                st4(W + c, wv); st4(M + c, m); st4(V + c, v);
+            }
+        }
+        if (gl == 0 && (!HASHED || bslot)) {    // the bias: with its row (plain) or in its own slot
+            float* bw = const_cast<float*>(a.bias) + id;
+            float wb = *bw, m = a.sbias[id], v = a.vbias[id];
+            adam_catch_up1(a.ad, old, upto, wb, m, v);
+            *bw = wb; a.sbias[id] = m; a.vbias[id] = v;
+        }
     }
 }
 
@@ -973,8 +1117,15 @@ int seq_validate(const slb_seq_step_args* x, bool training) {
     if (training) {
         SLB_REQUIRE(x->negs && x->bias && x->loss_out, "seq: null pointer");
         SLB_REQUIRE(x->opt != SLB_OPT_NONE || (x->dE && x->dbias), "seq: dE / dbias needed without a fused optimizer");
-        SLB_REQUIRE(x->opt == SLB_OPT_NONE || x->opt == SLB_OPT_SGD || (x->opt == SLB_OPT_ADAGRAD && x->state_E && x->state_bias),
-                    "seq: fused optimizer is SGD, or Adagrad with state_E / state_bias");
+        SLB_REQUIRE(x->opt == SLB_OPT_NONE || x->opt == SLB_OPT_SGD || (x->opt == SLB_OPT_ADAGRAD && x->state_E && x->state_bias) ||
+                    x->opt == SLB_OPT_ADAM,
+                    "seq: fused optimizer is SGD, Adagrad with state_E / state_bias, or Adam");
+        if (x->opt == SLB_OPT_ADAM)
+            SLB_REQUIRE(x->state_E && x->state_bias && x->state2_E && x->state2_bias && x->last_E &&
+                        (x->item_hashes == 0 || x->last_bias) && x->adam_sched && x->adam_step >= 1 &&
+                        x->adam_step < (1ll << 31),
+                        "seq: fused Adam needs exp_avg / exp_avg_sq / last (last_bias on a hashed table), "
+                        "the schedule and 1 <= adam_step < 2^31");
         SLB_REQUIRE(x->loss >= 0 && x->loss <= 3, "seq: bad loss kind");
         SLB_REQUIRE(x->n_neg >= 1 && (x->loss == SLB_LOSS_ADAPTIVE_HINGE || x->n_neg == 1), "seq: bad n_neg");
         if (x->n_layers > 0) SLB_REQUIRE(x->dconv_w && x->dconv_b, "seq: conv grads missing");
@@ -1323,20 +1474,38 @@ int slb_seq_train_step(const slb_seq_step_args* x, slb_stream_t stream) {
     seq_mask_kernel<<<sq_grid((B * S + 255) / 256), 256, 0, st>>>(
         x->seqs, x->negs, B * S, static_cast<int64_t>(x->n_neg) * B * S, x->num_items, l.hdr);
     SLB_LAUNCH_CHECK("seq_mask_kernel");
-    float* rep = nullptr;
-    rc = run_representation(x, l, nullptr, st, &rep);
-    if (rc != SLB_OK) return rc;
 
     const bool hashed = x->item_hashes != 0;
     SeqDev a = seq_dev_table(x);
     a.negs = x->negs; a.loss = x->loss; a.n_neg = x->n_neg; a.Xs = l.X0;
-    a.bias = x->bias; a.rep = rep; a.dR = l.dR; a.C = l.C; a.keys = l.keys; a.gs = l.gs;
+    a.bias = x->bias;
+    const bool adam = x->opt == SLB_OPT_ADAM;
+    if (adam) {
+        a.ad = {x->beta1, x->beta2, x->one_minus_beta1, x->one_minus_beta2, x->eps, x->weight_decay, x->adam_sched,
+                static_cast<int32_t>(x->adam_step)};
+        a.sE = x->state_E; a.sbias = x->state_bias; a.vE = x->state2_E; a.vbias = x->state2_bias;
+        a.lastE = x->last_E; a.lastb = hashed ? x->last_bias : x->last_E;
+        if (x->adam_step > 1) {
+            const int64_t work = B * S * (1 + x->n_neg) * (hashed ? x->item_hashes + 1 : 1);
+            with_bool(hashed, [&](auto H) {
+                with_lpr(lpr, [&](auto L) {
+                    seq_adam_prepass_kernel<L, H><<<sq_grid((work + groups - 1) / groups), SQ_THREADS, 0, st>>>(a);
+                });
+            });
+            SLB_LAUNCH_CHECK("seq_adam_prepass_kernel");
+        }
+    }
+    float* rep = nullptr;
+    rc = run_representation(x, l, nullptr, st, &rep);
+    if (rc != SLB_OK) return rc;
+    a.rep = rep; a.dR = l.dR; a.C = l.C; a.keys = l.keys; a.gs = l.gs;
     a.hdr = l.hdr; a.partial = l.partial; a.norm = x->norm_count;
     a.loss_out = x->loss_out; a.pos_out = x->pos_out; a.neg_out = x->neg_out;
     a.dE = x->dE; a.dbias = x->dbias; a.seg = l.seg;
     // hashed rows are hot at small item_rows: sort their member lists with seg_sort_long_kernel
     if (hashed) a.seg.long_cap = seg_sort_cap(lpr);
-    a.opt = x->opt; a.lr = x->lr; a.wd = x->weight_decay; a.eps = x->eps; a.sE = x->state_E; a.sbias = x->state_bias;
+    a.opt = x->opt; a.lr = x->lr; a.wd = x->weight_decay; a.eps = x->eps;
+    if (!adam) { a.sE = x->state_E; a.sbias = x->state_bias; }
     const int score_grid = sq_grid((B * T + groups - 1) / groups);
     if (x->mix_w) {
         a.M = x->num_mixtures; a.P = l.P;
@@ -1403,7 +1572,10 @@ int slb_seq_train_step(const slb_seq_step_args* x, slb_stream_t stream) {
     }
     const int reduce_grid = sq_grid((nkeys + groups - 1) / groups);
     with_bool(hashed, [&](auto H) {
-        with_lpr(lpr, [&](auto L) { seq_reduce_kernel<L, H><<<reduce_grid, SQ_THREADS, 0, st>>>(a); });
+        with_lpr(lpr, [&](auto L) {
+            if (adam) seq_reduce_adam_kernel<L, H><<<reduce_grid, SQ_THREADS, 0, st>>>(a);
+            else seq_reduce_kernel<L, H><<<reduce_grid, SQ_THREADS, 0, st>>>(a);
+        });
     });
     SLB_LAUNCH_CHECK("seq_reduce_kernel");
     return SLB_OK;

@@ -851,6 +851,28 @@ def _mixture_params(mixture, lstm, D):
     return dict(num_mixtures=M, w=w.reshape(w.shape[0], -1), b=_f32c(mixture['b']))
 
 
+def _seq_adam_args(a, fused, E, bias):
+    """The lazy-exact Adam fields of slb_seq_step_args from ``fused`` (see seq_train_step)."""
+    last_bias = fused.get('last_bias')
+    tensors = [fused['state_E'], fused['state_bias'], fused['state2_E'], fused['state2_bias'], fused['last_E'],
+               fused['sched']] + ([last_bias] if last_bias is not None else [])
+    require_cuda(*tensors)
+    for m, p in ((fused['state_E'], E), (fused['state2_E'], E), (fused['state_bias'], bias), (fused['state2_bias'], bias)):
+        if m.shape != p.shape or m.dtype != torch.float32 or not m.is_contiguous():
+            raise ValueError('seq_train_step: Adam moments must be contiguous float32 of the parameter shape')
+    for last, p in ((fused['last_E'], E), (last_bias, bias)):
+        if last is not None and (last.dtype != torch.int32 or last.shape != (p.shape[0],) or not last.is_contiguous()):
+            raise ValueError('seq_train_step: Adam `last` must be contiguous int32 with one entry per row')
+    if fused['sched'].numel() < 2 * (int(fused['step']) + 1):
+        raise ValueError('seq_train_step: the Adam schedule does not reach step %d' % int(fused['step']))
+    b1, b2 = float(fused['beta1']), float(fused['beta2'])
+    a.beta1, a.beta2, a.one_minus_beta1, a.one_minus_beta2 = b1, b2, 1.0 - b1, 1.0 - b2
+    a.state2_E, a.state2_bias = fused['state2_E'].data_ptr(), fused['state2_bias'].data_ptr()
+    a.last_E = fused['last_E'].data_ptr()
+    a.last_bias = last_bias.data_ptr() if last_bias is not None else None
+    a.adam_sched, a.adam_step = fused['sched'].data_ptr(), int(fused['step'])
+
+
 def seq_train_step(E, bias, seqs, negs, loss, n_neg, cnn=None, want_scores=False, norm_count=None, fused=None,
                    lstm=None, mixture=None, item_hash=None):
     """Fused forward + backward of one sequence minibatch, dense gradients.
@@ -864,6 +886,12 @@ def seq_train_step(E, bias, seqs, negs, loss, n_neg, cnn=None, want_scores=False
     then holds the projection gradients in the shapes given.  ``item_hash`` = dict(seeds, padding_idx)
     makes ``E`` a ``BloomEmbedding``'s compressed (M, D) table: an item is the sum of its hashed rows,
     ``bias`` stays (num_items, 1), and ``dE`` is (M, D).
+
+    Lazy-exact Adam (``optim.FusedAdam``): ``fused`` = dict(kind=OPT_ADAM, lr, weight_decay, eps, beta1,
+    beta2, state_E / state_bias (exp_avg), state2_E / state2_bias (exp_avg_sq), last_E (int32, one entry
+    per row of ``E``), last_bias (int32 (num_items,), hashed tables only; a plain table's bias shares
+    last_E), sched (``FusedAdam.schedule``), step (this step, 1-based)).  The rows the minibatch
+    references are first brought current through step - 1, then the rows with a gradient take step.
     """
     require_cuda(E, bias, seqs, negs)
     lib = _lib.load()
@@ -894,6 +922,8 @@ def seq_train_step(E, bias, seqs, negs, loss, n_neg, cnn=None, want_scores=False
         a.opt, a.lr, a.weight_decay, a.eps = int(fused['kind']), float(fused['lr']), float(fused['weight_decay']), float(fused['eps'])
         if fused.get('state_E') is not None:
             a.state_E, a.state_bias = fused['state_E'].data_ptr(), fused['state_bias'].data_ptr()
+        if a.opt == _lib.OPT_ADAM:
+            _seq_adam_args(a, fused, E, bias)
     if norm_count is not None:
         a.norm_count = norm_count.data_ptr()
     if cnn is not None:

@@ -82,6 +82,11 @@ class FusedAdam(torch.optim.Optimizer):
     parameters the caller sees are those of dense Adam (up to fp32 rounding of identical
     formulas).  State (``exp_avg``, ``exp_avg_sq``, ``step``) is kept in ``self.state`` under
     torch's names plus a per-row ``last`` step index.
+
+    Any module: the tables a fused step updates lazily (the factorization models' tables, a
+    sequence model's item table and bias) are registered through ``fused_states`` and flushed;
+    every other parameter (convolutions, LSTM, projection) takes ordinary dense Adam in
+    ``step()``, which on the fused routes runs after the kernel with the same step count.
     """
 
     fused_kind = _lib.OPT_ADAM
@@ -111,13 +116,23 @@ class FusedAdam(torch.optim.Optimizer):
         return dict(lr=float(g['lr']), weight_decay=float(g['weight_decay']), eps=float(g['eps']),
                     beta1=float(g['betas'][0]), beta2=float(g['betas'][1]))
 
-    def fused_states(self, param):
+    def _moments(self, param):
         st = self.state[param]
-        if not st:
+        if 'exp_avg' not in st:
             st['exp_avg'] = torch.zeros_like(param)
             st['exp_avg_sq'] = torch.zeros_like(param)
-            st['last'] = torch.zeros(param.shape[0], dtype=torch.int32, device=param.device)
+        if 'last' not in st:
+            st['last'] = torch.full((param.shape[0],), self._t, dtype=torch.int32, device=param.device)
         return st['exp_avg'], st['exp_avg_sq'], st['last']
+
+    def fused_states(self, param, own_last=False):
+        """``(exp_avg, exp_avg_sq, last)`` of a table a fused step updates lazily; registers it for
+        ``flush()``.  By default the table is one half of an (embedding, bias) pair that shares the
+        embedding's ``last`` (the factorization models, a plain sequence item table); ``own_last``:
+        a table flushed on its own with its own ``last`` (a hashed item table, an id-indexed bias)."""
+        states = self._moments(param)
+        self.state[param]['lazy'] = 'own' if own_last else 'pair'
+        return states
 
     def schedule(self, upto, device):
         """Device table of the per-step scalars lr / (1 - beta1^t), sqrt(1 - beta2^t), t <= upto
@@ -145,15 +160,20 @@ class FusedAdam(torch.optim.Optimizer):
         for st in self.state.values():
             st['step'] = self._t
 
+    def _lazy(self, kind):
+        return [p for g in self.param_groups for p in g['params'] if self.state.get(p, {}).get('lazy') == kind]
+
     def flush(self):
-        """Replay the pending (gradient-free) steps of every row of the embedding tables."""
-        import ctypes
+        """Replay the pending (gradient-free) steps of every row of the lazily updated tables (those
+        registered through ``fused_states``); every other parameter is always current."""
         from spotlight_b200 import ops
         if self._t == 0:
             return
         lib = _lib.load()
         hp = self.fused_hparams()
-        params = [p for g in self.param_groups for p in g['params'] if p in self.state and self.state[p]]
+        scalars = (hp['beta1'], hp['beta2'], 1.0 - hp['beta1'], 1.0 - hp['beta2'], hp['eps'], hp['weight_decay'],
+                   ops._stream())
+        params = self._lazy('pair')
         # tables come in (embedding (rows, D), bias (rows, 1)) pairs sharing `last`: the k-th
         # embedding table pairs with the k-th bias table (BilinearNet's parameter order)
         emb = [p for p in params if p.dim() == 2 and p.shape[1] > 1]
@@ -170,31 +190,51 @@ class FusedAdam(torch.optim.Optimizer):
             with torch.no_grad():
                 _lib.check(lib.slb_adam_flush(ops._ptr(W), ops._ptr(m), ops._ptr(v), ops._ptr(b), ops._ptr(bm),
                                               ops._ptr(bv), ops._ptr(last), rows, W.shape[1], ops._ptr(sched),
-                                              self._t, hp['beta1'], hp['beta2'], 1.0 - hp['beta1'], 1.0 - hp['beta2'],
-                                              hp['eps'], hp['weight_decay'], ops._stream()), 'adam_flush')
+                                              self._t, *scalars), 'adam_flush')
+        for p in self._lazy('own'):
+            if not p.is_cuda:
+                continue
+            m, v, last = self._moments(p)
+            sched = self.schedule(self._t, p.device)
+            with torch.no_grad():
+                _lib.check(lib.slb_adam_flush_table(ops._ptr(p), ops._ptr(m), ops._ptr(v), ops._ptr(last),
+                                                    p.shape[0], p[0].numel(), ops._ptr(sched), self._t, *scalars),
+                           'adam_flush_table')
 
     def step(self, closure=None):
-        """Dense fallback for callers that drive the optimizer themselves with ``.grad``:
-        flush, then one ordinary Adam step on every row (all rows become current)."""
+        """One ordinary Adam step (step count t = steps taken + 1) on every parameter that has a
+        ``.grad``.  A lazily updated table that has no ``.grad`` (a fused sequence step already
+        applied step t to it in place) is left alone.  When a lazily updated table does carry a
+        ``.grad`` (the dense fallback for callers that drive the optimizer themselves), every lazy
+        table is flushed first, so the dense step finds all rows current.  Every stepped parameter
+        keeps a ``last`` (= t after the step) so that a table a fused path registers later starts
+        current.  Sparse gradients are rejected, as torch.optim.Adam rejects them."""
         loss = closure() if closure is not None else None
-        self.flush()
+        params = [p for g in self.param_groups for p in g['params'] if p.grad is not None]
+        if any(self.state.get(p, {}).get('lazy') for p in params):
+            self.flush()
         hp = self.fused_hparams()
         self._t += 1
         t = self._t
         ss = hp['lr'] / (1.0 - hp['beta1'] ** t)
         bc2s = (1.0 - hp['beta2'] ** t) ** 0.5
+        lasts = []
         with torch.no_grad():
-            for g in self.param_groups:
-                for p in g['params']:
-                    if p.grad is None:
-                        continue
-                    m, v, last = self.fused_states(p)
-                    grad = p.grad if hp['weight_decay'] == 0 else p.grad.add(p, alpha=hp['weight_decay'])
-                    m.lerp_(grad, 1 - hp['beta1'])
-                    v.mul_(hp['beta2']).addcmul_(grad, grad, value=1 - hp['beta2'])
-                    p.addcdiv_(m, (v.sqrt() / bc2s).add_(hp['eps']), value=-ss)
-                    last.fill_(t)
-                    self.state[p]['step'] = t
+            for p in params:
+                if p.grad.is_sparse:
+                    raise RuntimeError('FusedAdam does not support sparse gradients (as torch.optim.Adam): '
+                                       'construct the model with sparse=False')
+                m, v, last = self._moments(p)
+                grad = p.grad if hp['weight_decay'] == 0 else p.grad.add(p, alpha=hp['weight_decay'])
+                m.lerp_(grad, 1 - hp['beta1'])
+                v.mul_(hp['beta2']).addcmul_(grad, grad, value=1 - hp['beta2'])
+                p.addcdiv_(m, (v.sqrt() / bc2s).add_(hp['eps']), value=-ss)
+                lasts.append(last)
+            if lasts:                  # every stepped parameter is current for t: two multi-tensor launches
+                torch._foreach_zero_(lasts)
+                torch._foreach_add_(lasts, t)
+        for st in self.state.values():
+            st['step'] = t
         return loss
 
 

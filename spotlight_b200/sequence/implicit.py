@@ -11,9 +11,14 @@
            optimizer the model holds.
   fused_hashed
            the same four nets on a ``BloomEmbedding(padding_idx=0)`` item layer (dense table,
-           within each net's fused limits) trained with ``optim.fused_sgd`` / ``fused_adagrad``:
-           the same C call, with items summed from their hashed rows, and the compressed
-           table and the biases updated in place by the row-wise optimizer.
+           within each net's fused limits) trained with ``optim.fused_sgd`` / ``fused_adagrad`` /
+           ``fused_adam``: the same C call, with items summed from their hashed rows, and the
+           compressed table and the biases updated in place by the row-wise optimizer.
+
+With ``optim.fused_adam`` (row-wise lazy-exact Adam) on either fused route the C call applies
+Adam to the item table and bias in place (no dense (num_items, D) gradient, no sweep over the
+table); ``optimizer.step()`` then takes the same Adam step on the other parameters, and ``fit()``
+flushes the pending steps of every row before it returns.
   generic  any other representation (custom, Bloom-embedded under a ``torch.optim``
            optimizer): the reference's loop shape over this package's gather and loss ops.
 """
@@ -118,7 +123,7 @@ class ImplicitSequenceModel(object):
                 return 'fused'
             # a hashed table has no dense gradient to hand to torch.optim: row-wise optimizers only
             if net.hashed_spec() is not None and \
-                    getattr(self._optimizer, 'fused_kind', None) in (_lib.OPT_SGD, _lib.OPT_ADAGRAD):
+                    getattr(self._optimizer, 'fused_kind', None) in (_lib.OPT_SGD, _lib.OPT_ADAGRAD, _lib.OPT_ADAM):
                 return 'fused_hashed'
         return 'generic'
 
@@ -184,6 +189,8 @@ class ImplicitSequenceModel(object):
 
             if np.isnan(epoch_loss) or epoch_loss == 0.0:
                 raise ValueError('Degenerate epoch loss: {}'.format(epoch_loss))
+        if hasattr(self._optimizer, 'flush'):
+            self._optimizer.flush()             # lazy-exact Adam: every row current before fit() returns
 
     def _fused_step(self, batch_sequence, batch_neg, n_neg):
         net = self._net
@@ -203,6 +210,18 @@ class ImplicitSequenceModel(object):
             fused = dict(kind=kind, lr=hp['lr'], weight_decay=hp['weight_decay'], eps=hp['eps'],
                          state_E=opt.fused_state(table),
                          state_bias=opt.fused_state(net.item_biases.weight))
+        elif kind == _lib.OPT_ADAM:
+            # lazy-exact Adam inside the step, at step t = steps taken + 1; optimizer.step() below
+            # counts t and applies it to the parameters that carry a .grad (not the item table and bias).
+            # A plain table's bias shares the rows' `last`; a hashed table and its id-indexed bias have their own.
+            hp = opt.fused_hparams()
+            hashed = item_hash is not None
+            m, v, last = opt.fused_states(table, own_last=hashed)
+            bm, bv, blast = opt.fused_states(net.item_biases.weight, own_last=hashed)
+            t = opt.steps_taken + 1
+            fused = dict(kind=kind, lr=hp['lr'], weight_decay=hp['weight_decay'], eps=hp['eps'],
+                         beta1=hp['beta1'], beta2=hp['beta2'], state_E=m, state_bias=bm, state2_E=v, state2_bias=bv,
+                         last_E=last, last_bias=blast if hashed else None, sched=opt.schedule(t, table.device), step=t)
         with torch.no_grad():
             out = ops.seq_train_step(table, net.item_biases.weight,
                                      batch_sequence, batch_neg, self._loss, n_neg, spec, fused=fused,
