@@ -81,6 +81,7 @@ class MfBloomArgs(ctypes.Structure):
         ('user_seeds', ctypes.c_uint32 * 24), ('item_seeds', ctypes.c_uint32 * 24),
         ('user_padding_idx', c_i64), ('item_padding_idx', c_i64),
         ('pair_ids_u', c_vp), ('pair_g_u', c_vp), ('pair_ids_i', c_vp), ('pair_g_i', c_vp),
+        ('last_bu', c_vp), ('last_bi', c_vp),
     ]
 
 

@@ -1018,6 +1018,107 @@ __global__ void __launch_bounds__(MF_THREADS) mf_fwd_bloom_rating_kernel(MfDev a
     if (grid_fold<MF_THREADS>(lsum, sh_red, is_last, a.partial, a.done, v)) { *a.loss_out = v * invB; *a.done = 0; }
 }
 
+// Lazy-exact Adam on hashed tables (the scheme of mf_adam.cuh): the exp_avg_sq of the four tables
+// (exp_avg are MfDev's sW* / sb*) and the step each entry is current for.  Every table has its own
+// `last`: a table row is shared by many ids, a bias belongs to one id.
+struct BloomAdamDev {
+    float* vWu; float* vWi; float* vbu; float* vbi;
+    int32_t* last_u; int32_t* last_i; int32_t* last_bu; int32_t* last_bi;
+};
+
+// Before the forward of step t: every entry the minibatch reads becomes current through step t-1 --
+// the H rows of each user, positive and negative item (its plain row when H = 0) and the bias of
+// each of those ids.  The padding row is caught up like any other: dense Adam with weight decay
+// moves it although its gradient is zero.  One lane group per id walks its rows and then its bias;
+// atomicMax on `last` elects one group per distinct entry, as in mf_adam_prepass_kernel.
+template <int LPR>
+__global__ void __launch_bounds__(MF_THREADS)
+mf_bloom_adam_prepass_kernel(MfDev a, const __grid_constant__ BloomSpec h, AdamDev o, BloomAdamDev s) {
+    constexpr int GROUPS = MF_THREADS / LPR;
+    const int gl = threadIdx.x & (LPR - 1);
+    const unsigned gmask = group_mask(LPR);
+    const int lead = (threadIdx.x & 31) & ~(LPR - 1);
+    const int D = a.D;
+    const int upto = o.t - 1;
+    if (upto <= 0) return;
+    const int64_t total = (2 + a.n_neg) * a.B;            // users, positives, negatives
+    for (int64_t r = static_cast<int64_t>(blockIdx.x) * GROUPS + threadIdx.x / LPR; r < total;
+         r += static_cast<int64_t>(gridDim.x) * GROUPS) {
+        const bool isA = r < a.B;
+        const int64_t id = isA ? a.users[r] : (r < 2 * a.B ? a.items[r - a.B] : a.negs[r - 2 * a.B]);
+        if (id < 0 || id >= (isA ? h.num_users : h.num_items)) continue;      // the forward flags bad ids
+        const int H = isA ? h.Hu : h.Hi;
+        const int nh = H ? H : 1;
+        for (int k = 0; k <= nh; ++k) {                   // k < nh: the id's table rows, k == nh: its bias
+            const bool bias = k == nh;                    // group-uniform
+            const int64_t row = bias ? id : isA ? hashed_row(id, k, H, h.su, a.U, h.pad_u)
+                                                : hashed_row(id, k, H, h.si, a.I, h.pad_i);
+            int32_t* last = (bias ? (isA ? s.last_bu : s.last_bi) : (isA ? s.last_u : s.last_i)) + row;
+            int old = 0;
+            if (gl == 0) old = atomicMax(last, upto);
+            old = __shfl_sync(gmask, old, lead);
+            if (old >= upto) continue;
+            if (bias) {
+                if (gl == 0) {
+                    float* bw = (isA ? a.bu : a.bi) + row;
+                    float* bm = (isA ? a.sbu : a.sbi) + row;
+                    float* bv = (isA ? s.vbu : s.vbi) + row;
+                    float w = *bw, m = *bm, v = *bv;
+                    adam_catch_up1(o, old, upto, w, m, v);
+                    *bw = w; *bm = m; *bv = v;
+                }
+                continue;
+            }
+            float* W = (isA ? a.Wu : a.Wi) + row * D;
+            float* M = (isA ? a.sWu : a.sWi) + row * D;
+            float* V = (isA ? s.vWu : s.vWi) + row * D;
+            for (int c = gl * 4; c < D; c += LPR * 4) {
+                float4 w = ld4(W + c), m = ld4(M + c), v = ld4(V + c);
+                adam_catch_up(o, old, upto, w, m, v);
+                st4(W + c, w); st4(M + c, m); st4(V + c, v);
+            }
+        }
+    }
+}
+
+// The real step t on the table rows with a gradient, from the compact gradients of the step (user
+// segment k: row urows[k], gradient row k of gWu; item segments likewise).  The biases are
+// id-indexed and take their step in bias_adam_apply_kernel.
+template <int LPR>
+__global__ void __launch_bounds__(MF_THREADS) mf_bloom_adam_apply_kernel(MfDev a, AdamDev o, BloomAdamDev s) {
+    constexpr int GROUPS = MF_THREADS / LPR;
+    const int gl = threadIdx.x & (LPR - 1);
+    const int gib = threadIdx.x / LPR;
+    const int D = a.D;
+    const int nseg = a.seg.totals[0];
+    const int nsegA = a.seg.totals[2];
+    const float ss = o.sched[2 * o.t], bc = o.sched[2 * o.t + 1];
+    for (int64_t sg = static_cast<int64_t>(blockIdx.x) * GROUPS + gib; sg < nseg; sg += static_cast<int64_t>(gridDim.x) * GROUPS) {
+        const bool isA = sg < nsegA;
+        const int64_t k = isA ? sg : sg - nsegA;
+        const int64_t row = isA ? a.urows[k] : a.irows[k];
+        if (row < 0) continue;                                       // frozen (padding) row: no step
+        float* W = (isA ? a.Wu : a.Wi) + row * D;
+        float* M = (isA ? a.sWu : a.sWi) + row * D;
+        float* V = (isA ? s.vWu : s.vWi) + row * D;
+        const float* G = (isA ? a.gWu : a.gWi) + k * D;
+        int32_t* lastp = (isA ? s.last_u : s.last_i) + row;
+        const int last = *lastp;
+        for (int c = gl * 4; c < D; c += LPR * 4) {
+            float4 w = ld4(W + c), m = ld4(M + c), v = ld4(V + c);
+            const float4 g = ld4(G + c);
+            adam_catch_up(o, last, o.t - 1, w, m, v);
+            adam_elem(o, ss, bc, g.x, w.x, m.x, v.x);
+            adam_elem(o, ss, bc, g.y, w.y, m.y, v.y);
+            adam_elem(o, ss, bc, g.z, w.z, m.z, v.z);
+            adam_elem(o, ss, bc, g.w, w.w, m.w, v.w);
+            st4(W + c, w); st4(M + c, m); st4(V + c, v);
+        }
+        __syncwarp(group_mask(LPR));          // every lane has read `last` before it moves
+        if (gl == 0) *lastp = o.t;
+    }
+}
+
 struct MfLayout {
     int32_t* t_a; int32_t* t_b; float* t_g; float* partial; int32_t* done; int32_t* err;
     SegIndex seg;
@@ -1772,22 +1873,31 @@ size_t bias_sparse_bytes(int64_t n) {
     return ws.bytes();
 }
 
-int bias_sparse_apply(void* wsp, const int64_t* ids, const float* g, int64_t n, float* b, float* sb,
-                      int32_t opt, float lr, float wd, float eps, bool by_id, cudaStream_t st) {
+// Groups the n (id, g) pairs by hash bucket (count -> scan -> fill) into p; the apply kernel runs next.
+int bias_sparse_index(void* wsp, const int64_t* ids, const float* g, int64_t n, float* b, float* sb,
+                      int32_t opt, float lr, float wd, float eps, bool by_id, cudaStream_t st, BiasSparse& p, int& grid) {
     int64_t nb = 4096;
     while (nb < 2 * n) nb <<= 1;
     WsCarver ws(wsp);
-    BiasSparse p;
     p.seg = seg_index_carve(ws, nb, n);
     p.ids = ids; p.g = g; p.n = n; p.mask = nb - 1; p.b = b; p.sb = sb;
     p.opt = opt; p.lr = lr; p.wd = wd; p.eps = eps; p.by_id = by_id ? 1 : 0;
-    const int grid = slb_grid((n + 255) / 256, 8);
+    grid = slb_grid((n + 255) / 256, 8);
     bias_count_kernel<<<grid, 256, 0, st>>>(p);
     SLB_LAUNCH_CHECK("bias_count_kernel");
     seg_scan_launch(p.seg, p.seg.Rpad, st);
     SLB_LAUNCH_CHECK("seg_scan_kernel");
     bias_fill_kernel<<<grid, 256, 0, st>>>(p);
     SLB_LAUNCH_CHECK("bias_fill_kernel");
+    return SLB_OK;
+}
+
+int bias_sparse_apply(void* wsp, const int64_t* ids, const float* g, int64_t n, float* b, float* sb,
+                      int32_t opt, float lr, float wd, float eps, bool by_id, cudaStream_t st) {
+    BiasSparse p;
+    int grid = 0;
+    const int rc = bias_sparse_index(wsp, ids, g, n, b, sb, opt, lr, wd, eps, by_id, st, p, grid);
+    if (rc != SLB_OK) return rc;
     bias_apply_kernel<<<grid, 256, 0, st>>>(p);
     SLB_LAUNCH_CHECK("bias_apply_kernel");
     return SLB_OK;
@@ -1802,6 +1912,8 @@ struct BloomLayout {
     void* ws_u; size_t ws_u_bytes; void* ws_i; size_t ws_i_bytes;
     // fused-optimizer mode: compact item-row gradients + hash-bucket bias workspaces
     int64_t* irows; float* gWi; int32_t* compact_counts; void* bws_u; void* bws_i;
+    // fused Adam only: compact user-row gradients (both sides' gradients precede any update)
+    int64_t* urows; float* gWu;
     size_t bytes;
 };
 
@@ -1841,9 +1953,21 @@ static BloomLayout bloom_layout(void* base, const slb_mf_bloom_args* x) {
         l.gWi = ws.take<float>(static_cast<size_t>(irow_cap + 1) * x->base.dim);
         l.compact_counts = ws.take<int32_t>(4);
     }
+    l.urows = nullptr; l.gWu = nullptr;
+    if (x->base.opt == SLB_OPT_ADAM) {
+        const int64_t urow_cap = T < x->user_rows ? T : x->user_rows;
+        l.urows = ws.take<int64_t>(urow_cap + 1);
+        l.gWu = ws.take<float>(static_cast<size_t>(urow_cap + 1) * x->base.dim);
+    }
     l.bytes = ws.bytes();
     return l;
 }
+
+// Fused Adam launches of slb_mf_bloom_train_step, defined at the end of this file (see there).
+static int bloom_adam_prepass(const MfDev& a, const BloomSpec& h, const AdamDev& o, const BloomAdamDev& s, int lpr,
+                              cudaStream_t st);
+static int bloom_adam_step(const MfDev& a, const AdamDev& o, const BloomAdamDev& s, const BloomLayout& l,
+                           const slb_mf_bloom_args* x, int lpr, int tgrid, cudaStream_t st);
 
 extern "C" {
 
@@ -1866,10 +1990,19 @@ int slb_mf_bloom_train_step(const slb_mf_bloom_args* x, slb_stream_t stream) {
                     "mf_bloom_train_step: rating losses write no bias pairs");
     }
     const bool fused = b.opt != SLB_OPT_NONE;
-    SLB_REQUIRE(fused ? (b.opt == SLB_OPT_SGD || b.opt == SLB_OPT_ADAGRAD) : b.grad_mode == SLB_GRAD_DENSE,
-                "mf_bloom_train_step: dense gradients, or a fused SGD / Adagrad optimizer");
+    const bool adam = b.opt == SLB_OPT_ADAM;
+    SLB_REQUIRE(fused ? (b.opt == SLB_OPT_SGD || b.opt == SLB_OPT_ADAGRAD || adam) : b.grad_mode == SLB_GRAD_DENSE,
+                "mf_bloom_train_step: dense gradients, or a fused SGD / Adagrad / Adam optimizer");
     SLB_REQUIRE(!fused || b.opt == SLB_OPT_SGD || (b.state_Wu && b.state_Wi && b.state_bu && b.state_bi),
-                "mf_bloom_train_step: adagrad needs state");
+                "mf_bloom_train_step: adagrad / adam need state");
+    if (adam) {
+        SLB_REQUIRE(!rating, "mf_bloom_train_step: fused Adam takes the pairwise losses only");
+        SLB_REQUIRE(b.grad_mode == SLB_GRAD_COMPACT, "mf_bloom_train_step: fused Adam needs compact mode");
+        SLB_REQUIRE(b.state2_Wu && b.state2_Wi && b.state2_bu && b.state2_bi && b.last_u && b.last_i && x->last_bu &&
+                    x->last_bi && b.adam_sched,
+                    "mf_bloom_train_step: fused Adam needs exp_avg / exp_avg_sq / last of all four tables and the schedule");
+        SLB_REQUIRE(b.adam_step >= 1 && b.adam_step < (1ll << 31), "mf_bloom_train_step: fused Adam needs adam_step >= 1");
+    }
     SLB_REQUIRE(x->user_hashes >= 0 && x->user_hashes <= 24 && x->item_hashes >= 0 && x->item_hashes <= 24,
                 "mf_bloom_train_step: at most 24 hash functions");
     SLB_REQUIRE(x->user_rows > 0 && x->item_rows > 0 && b.num_users > 0 && b.num_items > 0, "mf_bloom_train_step: empty tables");
@@ -1917,6 +2050,17 @@ int slb_mf_bloom_train_step(const slb_mf_bloom_args* x, slb_stream_t stream) {
 
     const int groups = MF_THREADS / lpr;
     const int grid = min(slb_grid((B + groups - 1) / groups, 8), MF_MAX_GRID);
+    AdamDev o = {};
+    BloomAdamDev s = {};
+    if (adam) {
+        // lazy-exact Adam: everything this minibatch reads becomes current (through step t-1) first
+        o = {b.beta1, b.beta2, b.one_minus_beta1, b.one_minus_beta2, b.eps, b.weight_decay, b.adam_sched,
+             static_cast<int32_t>(b.adam_step)};
+        s = {b.state2_Wu, b.state2_Wi, b.state2_bu, b.state2_bi, b.last_u, b.last_i, x->last_bu, x->last_bi};
+        a.urows = l.urows; a.gWu = l.gWu;
+        const int rc = bloom_adam_prepass(a, h, o, s, lpr, st);
+        if (rc != SLB_OK) return rc;
+    }
     if (rating) {
         with_lpr(lpr, [&](auto L) { mf_fwd_bloom_rating_kernel<L><<<grid, MF_THREADS, 0, st>>>(a, h); });
         SLB_LAUNCH_CHECK("mf_fwd_bloom_rating_kernel");
@@ -1931,6 +2075,11 @@ int slb_mf_bloom_train_step(const slb_mf_bloom_args* x, slb_stream_t stream) {
     seg_sort_long_kernel<<<SEG_LONG_CTAS, 256, 0, st>>>(a.seg);
     SLB_LAUNCH_CHECK("seg_sort_long_kernel");
     const int tgrid = slb_grid(((2 * T + 31) / 32 + 3) / 4, 16);
+    if (adam) {
+        // compact gradients of both sides from the tables as the forward read them, then step t on
+        // the touched rows and on the touched bias ids
+        return bloom_adam_step(a, o, s, l, x, lpr, tgrid, st);
+    }
     if (fused) {
         // hashed item rows first (compact gradients from the old user rows), user rows updated in
         // place, item rows updated from the compact gradients, then the id-space biases
@@ -1983,3 +2132,105 @@ int slb_bias_sparse_apply(const int64_t* ids, const float* g, int64_t n, float* 
 }
 
 }  // extern "C"
+
+// ---------------------------------------------------------------------------
+// Lazy-exact Adam on hashed tables: the launches of the fused Adam step.
+//
+// WHY THIS CODE SITS HERE AND IS TEMPLATED: only to keep the machine code (SASS) of every other
+// kernel in this file unchanged.  The compiler emits the non-template kernels first (in source
+// order) and then the template instantiations (in order of first use), and the basic-block labels
+// of a kernel count everything emitted ahead of it; ptxas's scheduling follows those labels, so a
+// kernel emitted earlier shifts the code of the kernels after it.  Therefore:
+//   * bias_adam_apply_kernel and bias_sparse_adam are templates (on an Index type that is always
+//     int) -- a plain __global__ here would be emitted before every template kernel of the file;
+//   * every launch of the new kernels happens in the functions below, the last uses in the file.
+// A new kernel added to this file keeps the others unchanged if it follows the same two rules.
+// ---------------------------------------------------------------------------
+namespace {
+
+// Lazy-exact Adam variant of bias_apply_kernel: the same bucket walk and per-id sum in pair order,
+// then the id's pending steps through t-1 and the real step t.  p.sb holds exp_avg, v exp_avg_sq,
+// last the step each id is current for.  One thread owns a bucket, so each id has one writer.
+// (Templated only for the emission order explained above; Index is always int.)
+template <typename Index>
+__global__ void __launch_bounds__(256) bias_adam_apply_kernel(BiasSparse p, AdamDev o, float* v, int32_t* last) {
+    const Index nseg = p.seg.totals[0];
+    const float ss = o.sched[2 * o.t], bc = o.sched[2 * o.t + 1];
+    const Index nth = gridDim.x * blockDim.x;
+    for (Index s = blockIdx.x * blockDim.x + threadIdx.x; s < nseg; s += nth) {
+        const int start = p.seg.seg_start[s], len = p.seg.seg_start[s + 1] - start;
+        // distinct ids in ascending order, each named by its first member: only 32-bit state lives
+        // across the Adam update (64-bit ids held there cost a stack frame)
+        int prev_m = -1;
+        for (;;) {
+            const int64_t last_id = prev_m < 0 ? -1 : p.ids[p.seg.members[start + prev_m]];
+            int cur_m = -1;
+            int64_t cur = INT64_MAX;
+            for (int m = 0; m < len; ++m) {
+                const int64_t id = p.ids[p.seg.members[start + m]];
+                if (id > last_id && id < cur) { cur = id; cur_m = m; }
+            }
+            if (cur_m < 0) break;
+            float acc = 0.f;                      // this id's pairs in ascending pair order
+            int prev = -1;
+            for (;;) {
+                int best = INT32_MAX;
+                for (int m = 0; m < len; ++m) {
+                    const int k = p.seg.members[start + m];
+                    if (k > prev && k < best && p.ids[k] == cur) best = k;
+                }
+                if (best == INT32_MAX) break;
+                acc += p.g[best];
+                prev = best;
+            }
+            float w = p.b[cur], m = p.sb[cur], vv = v[cur];
+            adam_catch_up1(o, last[cur], o.t - 1, w, m, vv);
+            adam_elem(o, ss, bc, acc, w, m, vv);
+            p.b[cur] = w; p.sb[cur] = m; v[cur] = vv;
+            last[cur] = o.t;
+            prev_m = cur_m;
+        }
+    }
+}
+
+template <typename Index>
+int bias_sparse_adam(void* wsp, const int64_t* ids, const float* g, int64_t n, float* b, float* m, float* v,
+                     int32_t* last, const AdamDev& o, cudaStream_t st) {
+    BiasSparse p;
+    int grid = 0;
+    const int rc = bias_sparse_index(wsp, ids, g, n, b, m, SLB_OPT_ADAM, 0.f, o.wd, o.eps, true, st, p, grid);
+    if (rc != SLB_OK) return rc;
+    bias_adam_apply_kernel<Index><<<grid, 256, 0, st>>>(p, o, v, last);
+    SLB_LAUNCH_CHECK("bias_adam_apply_kernel");
+    return SLB_OK;
+}
+
+}  // namespace
+
+static int bloom_adam_prepass(const MfDev& a, const BloomSpec& h, const AdamDev& o, const BloomAdamDev& s, int lpr,
+                              cudaStream_t st) {
+    const int groups = MF_THREADS / lpr;
+    const int pgrid = slb_grid(((2 + a.n_neg) * a.B + groups - 1) / groups, 8);
+    with_lpr(lpr, [&](auto L) { mf_bloom_adam_prepass_kernel<L><<<pgrid, MF_THREADS, 0, st>>>(a, h, o, s); });
+    SLB_LAUNCH_CHECK("mf_bloom_adam_prepass_kernel");
+    return SLB_OK;
+}
+
+// Compact gradients of both sides from the tables as the forward read them, then step t on the
+// touched rows and on the touched bias ids.
+static int bloom_adam_step(const MfDev& a, const AdamDev& o, const BloomAdamDev& s, const BloomLayout& l,
+                           const slb_mf_bloom_args* x, int lpr, int tgrid, cudaStream_t st) {
+    launch_bwd_tile<0>(a, lpr, false, tgrid, st);
+    SLB_LAUNCH_CHECK("mf_bwd_tile_kernel");
+    launch_long<0>(lpr, st, a);
+    SLB_LAUNCH_CHECK("mf_bwd_long_kernel");
+    const int groups = MF_THREADS / lpr;
+    const int agrid = slb_grid((2 * a.T + groups - 1) / groups, 8);
+    with_lpr(lpr, [&](auto L) { mf_bloom_adam_apply_kernel<L><<<agrid, MF_THREADS, 0, st>>>(a, o, s); });
+    SLB_LAUNCH_CHECK("mf_bloom_adam_apply_kernel");
+    const slb_mf_step_args& b = x->base;
+    const int64_t P = 2 * b.batch;          // Adam takes the pairwise losses: two bias pairs per interaction
+    const int rc = bias_sparse_adam<int>(l.bws_u, l.ids_u2, l.g_u2, P, b.bu, b.state_bu, b.state2_bu, x->last_bu, o, st);
+    if (rc != SLB_OK) return rc;
+    return bias_sparse_adam<int>(l.bws_i, l.ids_i2, l.g_i2, P, b.bi, b.state_bi, b.state2_bi, x->last_bi, o, st);
+}

@@ -287,7 +287,8 @@ class ImplicitFactorizationModel(object):
                             pending = (shuffle_begin(n, self._random_state, device), side)
                 epoch_loss = self._run_epoch_device(user_ids_tensor, item_ids_tensor,
                                                     after_sampling=next_permutation)
-            elif route == 'bloom' and getattr(self._optimizer, 'fused_kind', None) in (_lib.OPT_SGD, _lib.OPT_ADAGRAD):
+            elif route == 'bloom' and getattr(self._optimizer, 'fused_kind', None) in (_lib.OPT_SGD, _lib.OPT_ADAGRAD,
+                                                                                       _lib.OPT_ADAM):
                 negatives = self._epoch_negatives(len(user_ids))
                 epoch_loss = self._fit_epoch_bloom_fused(user_ids_tensor, item_ids_tensor, negatives)
             else:
@@ -436,23 +437,35 @@ class ImplicitFactorizationModel(object):
 
     def _fit_epoch_bloom_fused(self, users, items, negatives):
         """Hashed-table model with a fused row-wise optimizer: one in-place step per minibatch
-        (csrc/mf.cu slb_mf_bloom_train_step, fused mode), no dense gradient of any table."""
+        (csrc/mf.cu slb_mf_bloom_train_step, fused mode), no dense gradient of any table.  Under
+        ``FusedAdam`` the step is lazy-exact Adam: each of the four tables keeps its own ``last``,
+        and the ``flush()`` at the end of ``fit()`` brings every row current."""
         net, opt = self._net, self._optimizer
         spec = net.fused_spec()
         n_neg = self._n_neg()
         hp = opt.fused_hparams()
         params = (spec['Wu'], spec['Wi'], net.user_biases.weight, net.item_biases.weight)
-        states = [opt.fused_state(p) for p in params] if opt.fused_kind == _lib.OPT_ADAGRAD else None
+        states, adam = None, None
+        if opt.fused_kind == _lib.OPT_ADAGRAD:
+            states = [opt.fused_state(p) for p in params]
+        elif opt.fused_kind == _lib.OPT_ADAM:
+            states = [opt.fused_states(p, own_last=True) for p in params]
+            n_steps = (users.numel() + self._batch_size - 1) // self._batch_size
+            t0 = opt.steps_taken + 1
+            adam = dict(beta1=hp['beta1'], beta2=hp['beta2'], sched=opt.schedule(t0 + n_steps - 1, users.device))
+            opt.advance(n_steps)
         losses = []
         lo = 0
-        for batch_user, batch_item in minibatch(users, items, batch_size=self._batch_size):
+        for k, (batch_user, batch_item) in enumerate(minibatch(users, items, batch_size=self._batch_size)):
             B = batch_user.numel()
             batch_neg = negatives[lo * n_neg:(lo + B) * n_neg]
             lo += B
+            if adam is not None:
+                adam['step'] = t0 + k
             losses.append(ops.mf_bloom_train_step_inplace(
                 *params, batch_user, batch_item, batch_neg, self._loss, n_neg, spec['user_seeds'],
                 spec['item_seeds'], spec['user_pad'], spec['item_pad'], opt.fused_kind, hp['lr'], states,
-                hp['weight_decay'], hp['eps']))
+                hp['weight_decay'], hp['eps'], adam=adam))
         host = torch.stack(losses).cpu().numpy().astype(np.float64)        # one sync per epoch
         return float(host.sum() / len(host))
 

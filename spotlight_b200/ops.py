@@ -470,12 +470,18 @@ def _(Wu, Wi, bu, bi, users, items, ratings, loss, user_seeds, item_seeds, user_
 
 def mf_bloom_train_step_inplace(Wu, Wi, bu, bi, users, items, negs, loss, n_neg, user_seeds, item_seeds,
                                 user_pad, item_pad, opt_kind, lr, states=None, weight_decay=0.0, eps=1e-10,
-                                ratings=None):
+                                ratings=None, adam=None):
     """The fused hashed-table step with the row-wise optimizer applied in place: hashed / plain
     embedding rows through the compact-gradient kernels, the id-indexed bias tables through the
     hash-bucket sparse update (no dense gradient anywhere -- the item-bias table of BASELINE
     config 4 has 50 M rows).  ``states`` = (sWu, sWi, sbu, sbi) for Adagrad.  Rating losses pass
     ``negs=None``, ``n_neg=1`` and ``ratings`` (spotlight/factorization/explicit.py:223-234).
+
+    Lazy-exact Adam (``opt_kind = OPT_ADAM``, pairwise losses): ``states`` = four (exp_avg,
+    exp_avg_sq, last) triples of (Wu, Wi, bu, bi) (``FusedAdam.fused_states(p, own_last=True)``; each
+    ``last`` int32 with one entry per row), ``adam`` = dict(beta1, beta2, sched
+    (``FusedAdam.schedule``), step (this step, 1-based)).  Every row and bias the minibatch reads is
+    first brought current through step - 1; the entries with a gradient then take step.
     Returns the loss."""
     require_cuda(Wu, Wi, bu, bi, users, items, negs, ratings)
     users, items = _i64c(users).reshape(-1), _i64c(items).reshape(-1)
@@ -492,9 +498,36 @@ def mf_bloom_train_step_inplace(Wu, Wi, bu, bi, users, items, negs, loss, n_neg,
         a.opt, a.lr, a.weight_decay, a.eps = int(opt_kind), float(lr), float(weight_decay), float(eps)
         if opt_kind == _lib.OPT_ADAGRAD:
             a.state_Wu, a.state_Wi, a.state_bu, a.state_bi = [t.data_ptr() for t in states]
-        _bloom_workspace('mfbf', x, dev)
+        elif opt_kind == _lib.OPT_ADAM:
+            _bloom_adam_args(x, (Wu, Wi, bu, bi), states, adam)
+        # the Adam layout adds compact user-row gradients: its own workspace
+        _bloom_workspace('mfbfa' if opt_kind == _lib.OPT_ADAM else 'mfbf', x, dev)
         _lib.check(_lib.load().slb_mf_bloom_train_step(ctypes.byref(x), _stream()), 'mf_bloom_train_step')
     return loss_out.reshape(())
+
+
+def _bloom_adam_args(x, params, states, adam):
+    """The lazy-exact Adam fields of slb_mf_bloom_args (see mf_bloom_train_step_inplace)."""
+    if states is None or len(states) != 4 or adam is None:
+        raise ValueError('mf_bloom_train_step: Adam needs four (exp_avg, exp_avg_sq, last) states and adam=')
+    require_cuda(adam['sched'], *[t for st in states for t in st])
+    for p, (m, v, last) in zip(params, states):
+        for t in (m, v):
+            if t.shape != p.shape or t.dtype != torch.float32 or not t.is_contiguous():
+                raise ValueError('mf_bloom_train_step: Adam moments must be contiguous float32 of the parameter shape')
+        if last.dtype != torch.int32 or last.shape != (p.shape[0],) or not last.is_contiguous():
+            raise ValueError('mf_bloom_train_step: Adam `last` must be contiguous int32 with one entry per row')
+    step = int(adam['step'])
+    if adam['sched'].numel() < 2 * (step + 1):
+        raise ValueError('mf_bloom_train_step: the Adam schedule does not reach step %d' % step)
+    a = x.base
+    a.state_Wu, a.state_Wi, a.state_bu, a.state_bi = [st[0].data_ptr() for st in states]
+    a.state2_Wu, a.state2_Wi, a.state2_bu, a.state2_bi = [st[1].data_ptr() for st in states]
+    a.last_u, a.last_i = states[0][2].data_ptr(), states[1][2].data_ptr()
+    x.last_bu, x.last_bi = states[2][2].data_ptr(), states[3][2].data_ptr()
+    b1, b2 = float(adam['beta1']), float(adam['beta2'])
+    a.beta1, a.beta2, a.one_minus_beta1, a.one_minus_beta2 = b1, b2, 1.0 - b1, 1.0 - b2
+    a.adam_sched, a.adam_step = adam['sched'].data_ptr(), step
 
 
 def mf_bloom_step_pairs(Wu, Wi, bu, bi, users, items, negs, loss, item_seeds, item_pad, norm_batch=0):
