@@ -152,9 +152,9 @@ extern "C" {
 int slb_embedding_forward(const float* W, int64_t rows, int32_t dim, const int64_t* ids, int64_t n,
                           int32_t hash_count, const uint32_t* seeds, int64_t padding_idx,
                           float* out, slb_stream_t stream) {
-    SLB_REQUIRE(W && ids && out, "embedding_forward: null pointer");
     SLB_REQUIRE(rows > 0 && dim > 0, "embedding_forward: bad table shape");
-    if (n <= 0) return SLB_OK;
+    if (n <= 0) return SLB_OK;          // an empty lookup: its tensors may have no storage
+    SLB_REQUIRE(W && ids && out, "embedding_forward: null pointer");
     HashSpec hs;
     const int rc = make_hash(hs, hash_count, seeds, padding_idx);
     if (rc != SLB_OK) return rc;
@@ -173,8 +173,9 @@ int slb_embedding_forward(const float* W, int64_t rows, int32_t dim, const int64
 
 int slb_bloom_rows(const int64_t* ids, int64_t n, int32_t hash_count, const uint32_t* seeds,
                    int64_t rows, int64_t padding_idx, int64_t* rows_out, slb_stream_t stream) {
-    SLB_REQUIRE(ids && rows_out && hash_count > 0 && rows > 0, "bloom_rows: bad arguments");
+    SLB_REQUIRE(hash_count > 0 && rows > 0, "bloom_rows: bad arguments");
     if (n <= 0) return SLB_OK;
+    SLB_REQUIRE(ids && rows_out, "bloom_rows: null pointer");
     HashSpec hs;
     const int rc = make_hash(hs, hash_count, seeds, padding_idx);
     if (rc != SLB_OK) return rc;
@@ -191,9 +192,9 @@ size_t slb_embedding_backward_workspace_bytes(int64_t n_terms, int64_t rows) {
 int slb_embedding_backward(const float* dout, const int64_t* ids, int64_t n, int32_t hash_count,
                            const uint32_t* seeds, int64_t rows, int32_t dim, int64_t frozen_row,
                            float* dW, void* workspace, size_t workspace_bytes, slb_stream_t stream) {
-    SLB_REQUIRE(dout && ids && dW && workspace, "embedding_backward: null pointer");
     SLB_REQUIRE(rows > 0 && dim > 0, "embedding_backward: bad table shape");
-    if (n <= 0) return SLB_OK;
+    if (n <= 0) return SLB_OK;          // nothing to scatter: dW stays as the caller zeroed it
+    SLB_REQUIRE(dout && ids && dW && workspace, "embedding_backward: null pointer");
     HashSpec hs;
     const int rc = make_hash(hs, hash_count, seeds, -1);
     if (rc != SLB_OK) return rc;
