@@ -4,7 +4,8 @@
 ``sequence_precision_recall_score`` keep the reference's signatures and results, but instead
 of one ``predict`` + host ``rankdata`` / ``argsort`` per user or sequence (minutes to hours at
 1M users or 1M items) they score a block of users (sequences) against all items at once --
-one GEMM for dot-product models -- and rank every test target of the block with one pass of
+one GEMM for dot-product models, one ``slb_mixture_scores`` launch for MixtureLSTMNet's
+mixture-of-tastes head -- and rank every test target of the block with one pass of
 ``slb_rank_targets`` over each score row.  That kernel returns, per target, the average rank
 (``rankdata`` of the negated scores: the MRR) and the stable position (where the target lands in
 ``argsort(-row, kind='stable')``: a hit at k iff position < k, for every k at once).
@@ -28,7 +29,7 @@ from spotlight_b200 import _lib, ops
 from spotlight_b200.factorization.representations import BilinearNet
 from spotlight_b200.interactions import _to_host
 from spotlight_b200.layers import ScaledEmbedding
-from spotlight_b200.sequence.representations import LSTMNet, _SeqNetBase
+from spotlight_b200.sequence.representations import LSTMNet, MixtureLSTMNet, _SeqNetBase
 
 FLOAT_MAX = np.finfo(np.float32).max
 
@@ -90,7 +91,33 @@ def _score_sequences(model, sequences):
             out = final @ items.t()
             out += net.item_biases.weight.reshape(1, -1)
             return out
+        if _mixture_head(net, final):
+            return _mixture_block(net, final, num_items, sequences.device)
         return _generic_block(lambda r, t: net(r, t.reshape(-1, 1)), final, num_items, sequences.device)
+
+
+def _mixture_head(net, final):
+    """True when the block can go through slb_mixture_scores: MixtureLSTMNet's own softmax head
+    on a (n, 2M, D, 1) representation with 1 <= M <= 8 and D a multiple of 4."""
+    if not isinstance(net, MixtureLSTMNet) or type(net).forward is not MixtureLSTMNet.forward:
+        return False
+    M = net.num_mixtures
+    return (final.dim() == 4 and final.dtype == torch.float32 and 1 <= M <= MixtureLSTMNet.MAX_MIXTURES
+            and final.shape[1] == 2 * M and final.shape[3] == 1 and final.shape[2] % 4 == 0)
+
+
+def _mixture_block(net, final, num_items, dev):
+    """(n, num_items) scores of the mixture-of-tastes head for every item, in one launch."""
+    n, two_m, dim = final.shape[0], final.shape[1], final.shape[2]
+    reps = final.reshape(n, two_m, dim).contiguous()
+    items = _item_matrix(net.item_embeddings, num_items, dev).contiguous()
+    bias = net.item_biases.weight.reshape(-1).contiguous()
+    ops.require_cuda(reps, items, bias)
+    out = torch.empty(n, num_items, dtype=torch.float32, device=dev)
+    _lib.check(_lib.load().slb_mixture_scores(ops._ptr(reps), n, two_m // 2, dim, ops._ptr(items), ops._ptr(bias),
+                                              num_items, ops._ptr(out), ops._stream()),
+               'mixture_scores')
+    return out
 
 
 def _exclude(scores, rows, items):
