@@ -85,6 +85,94 @@ adagrad_dense_kernel(float* __restrict__ W, float* __restrict__ S, const float* 
     }
 }
 
+// ---- owner update: row-wise Adagrad of the received gradient rows (slb_shard_rows_adagrad) ----
+// local_ids entries outside [0, rows) are padding slots: neither counted nor placed.
+__global__ void __launch_bounds__(256)
+rows_count_kernel(const int64_t* __restrict__ ids, int64_t R, int64_t rows, SegIndex seg) {
+    if (blockIdx.x == 0 && threadIdx.x == 0) seg.totals[3] = 0;     // hot-row list of this call
+    const int64_t nth = static_cast<int64_t>(gridDim.x) * blockDim.x;
+    for (int64_t t = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x; t < R; t += nth) {
+        const int64_t r = ids[t];
+        if (r >= 0 && r < rows) atomicAdd(seg.cnt + r, 1);
+    }
+}
+
+__global__ void __launch_bounds__(256)
+rows_fill_kernel(const int64_t* __restrict__ ids, int64_t R, int64_t rows, SegIndex seg) {
+    const int64_t nth = static_cast<int64_t>(gridDim.x) * blockDim.x;
+    for (int64_t t = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x; t < R; t += nth) {
+        const int64_t r = ids[t];
+        if (r >= 0 && r < rows) seg_place(seg, r, static_cast<int32_t>(t));
+    }
+}
+
+// One group of LPR lanes per distinct row: the row's contributions in ascending position (= peer
+// rank) order, then the shared row-wise Adagrad step on the row and its bias.  Hot rows (longer
+// than the group's sort capacity: padding-heavy exchanges) were pre-sorted by seg_sort_long_kernel.
+template <int LPR, bool VEC4>
+__global__ void __launch_bounds__(256, 4)
+rows_adagrad_kernel(const float* __restrict__ g_rows, const float* __restrict__ g_bias, int D, SegIndex seg,
+                    OptV2 o, float* __restrict__ W, float* __restrict__ S, float* __restrict__ b,
+                    float* __restrict__ sb) {
+    constexpr int GROUPS = 256 / LPR;
+    constexpr int CAP = seg_sort_cap(LPR);
+    constexpr int STEP = VEC4 ? 4 : 1;
+    __shared__ int32_t sh_sort[GROUPS * 2 * CAP];
+    const int gl = threadIdx.x & (LPR - 1);
+    const int gib = threadIdx.x / LPR;
+    const unsigned gmask = group_mask(LPR);
+    int32_t* sh = sh_sort + gib * 2 * CAP;
+    const int nseg = seg.totals[0];
+    for (int64_t s = static_cast<int64_t>(blockIdx.x) * GROUPS + gib; s < nseg;
+         s += static_cast<int64_t>(gridDim.x) * GROUPS) {
+        const int start = seg.seg_start[s];
+        const int len = seg.seg_start[s + 1] - start;
+        const int64_t row = seg.seg_row[s];
+        float gb = 0.f;
+        for (int c0 = 0; c0 < D; c0 += LPR * STEP) {
+            const int c = c0 + gl * STEP;
+            float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
+            seg_visit_sorted<LPR>(seg.members, start, len, gl, gmask, sh, [&](int32_t t) {
+                const float* src = g_rows + static_cast<int64_t>(t) * D;
+                if (c0 == 0) gb += __ldg(g_bias + t);
+                if (c < D) {
+                    if (VEC4) {
+                        const float4 v = ldg4(src + c);
+                        acc.x += v.x; acc.y += v.y; acc.z += v.z; acc.w += v.w;
+                    } else {
+                        acc.x += __ldg(src + c);
+                    }
+                }
+            }, true);
+            if (c < D) {
+                float* w = W + row * D + c;
+                float* st = S + row * D + c;
+                if (VEC4) {
+                    float4 w4 = ld4(w), s4 = ld4(st);
+                    row_update(o, w4, s4, acc);
+                    st4(w, w4);
+                    st4(st, s4);
+                } else {
+                    bias_update(o, w, st, acc.x);
+                }
+            }
+        }
+        if (gl == 0) bias_update(o, b + row, sb + row, gb);
+    }
+}
+
+struct RowsLayout { SegIndex seg; size_t bytes; };
+
+RowsLayout rows_layout(void* base, int64_t R, int64_t rows) {
+    WsCarver ws(base);
+    RowsLayout l;
+    l.seg = seg_index_carve(ws, rows, R);
+    l.bytes = ws.bytes();
+    return l;
+}
+
+bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
+
 struct UqLayout { int32_t* flags; SegIndex seg; size_t bytes; };
 
 UqLayout uq_layout(void* base, int64_t n, int64_t rows) {
@@ -151,6 +239,50 @@ int slb_adagrad_dense(float* W, float* state, const float* grad, int64_t n, floa
     if (g > slb_sms() * 16) g = slb_sms() * 16;
     adagrad_dense_kernel<<<g, 256, 0, static_cast<cudaStream_t>(stream)>>>(W, state, grad, n, lr, eps);
     SLB_LAUNCH_CHECK("adagrad_dense_kernel");
+    return SLB_OK;
+}
+
+size_t slb_shard_rows_workspace_bytes(int64_t R, int64_t rows) {
+    return rows_layout(nullptr, R > 0 ? R : 0, rows > 0 ? rows : 1).bytes;
+}
+
+int slb_shard_rows_adagrad(const int64_t* local_ids, const float* g_rows, const float* g_bias, int64_t R,
+                           float* W, float* state_W, float* b, float* state_b, int64_t rows, int32_t dim,
+                           float lr, float eps, void* workspace, size_t workspace_bytes, slb_stream_t stream) {
+    SLB_REQUIRE(R >= 0 && rows >= 0 && dim >= 1, "shard_rows_adagrad: bad sizes");
+    if (R == 0) return SLB_OK;          // nothing arrived: the received tensors may have no storage
+    SLB_REQUIRE(local_ids && g_rows && g_bias && W && state_W && b && state_b && workspace,
+                "shard_rows_adagrad: null pointer");
+    SLB_REQUIRE(rows >= 1, "shard_rows_adagrad: rows arrived for an empty shard");
+    SLB_REQUIRE(R < (1ll << 31) && rows < (1ll << 31) - SEG_SCAN_TILE && dim < (1 << 28),
+                "shard_rows_adagrad: too large");
+    RowsLayout l = rows_layout(workspace, R, rows);
+    if (workspace_bytes < l.bytes) {
+        slb_set_error("shard_rows_adagrad: workspace too small (%zu < %zu)", workspace_bytes, l.bytes);
+        return SLB_ENOSPC;
+    }
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const bool vec4 = dim % 4 == 0 && aligned16(g_rows) && aligned16(W) && aligned16(state_W);
+    // lanes per row: one float4 (or one float) per lane, a power of two up to a warp
+    const int lpr = lpr_for_dim(vec4 ? dim : 4 * dim);
+    l.seg.long_cap = seg_sort_cap(lpr);
+    const int g1 = slb_grid((R + 255) / 256, 8);
+    rows_count_kernel<<<g1, 256, 0, st>>>(local_ids, R, rows, l.seg);
+    SLB_LAUNCH_CHECK("rows_count_kernel");
+    seg_scan_launch(l.seg, rows, st);
+    SLB_LAUNCH_CHECK("seg_scan_kernel");
+    rows_fill_kernel<<<g1, 256, 0, st>>>(local_ids, R, rows, l.seg);
+    SLB_LAUNCH_CHECK("rows_fill_kernel");
+    seg_sort_long_kernel<<<SEG_LONG_CTAS, 256, 0, st>>>(l.seg);     // no-op unless hot rows exist
+    SLB_LAUNCH_CHECK("seg_sort_long_kernel");
+    const OptV2 o = {SLB_OPT_ADAGRAD, lr, 0.f, eps};
+    const int grid = slb_grid((R + 256 / lpr - 1) / (256 / lpr), 8);
+    with_bool(vec4, [&](auto V) {
+        with_lpr(lpr, [&](auto L) {
+            rows_adagrad_kernel<L, V><<<grid, 256, 0, st>>>(g_rows, g_bias, dim, l.seg, o, W, state_W, b, state_b);
+        });
+    });
+    SLB_LAUNCH_CHECK("rows_adagrad_kernel");
     return SLB_OK;
 }
 

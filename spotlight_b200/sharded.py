@@ -137,14 +137,19 @@ class GpuBackend(object):
 
     def owner_update(self, st, local_ids, g_rows, g_bias):
         """Sum the peers' gradient rows per shard row (rank order, deterministic)
-        and apply Adagrad to the item shard."""
-        rows = st.Wi.shape[0]
-        if local_ids.numel() == 0:
+        and apply Adagrad to those rows of the item shard and its bias only."""
+        R = local_ids.numel()
+        if R == 0:
             return
-        dW = ops.embedding_backward(g_rows.contiguous(), local_ids, [], rows, -1)
-        db = ops.embedding_backward(g_bias.reshape(-1, 1).contiguous(), local_ids, [], rows, -1)
-        adagrad_dense_(st.Wi, st.sWi, dW, st.lr, st.eps)
-        adagrad_dense_(st.bi, st.sbi, db.reshape(-1), st.lr, st.eps)
+        lib = _lib.load()
+        rows, D = st.Wi.shape
+        ids = local_ids.contiguous().long()
+        g_rows, g_bias = g_rows.contiguous(), g_bias.reshape(-1).contiguous()
+        ws = ops.workspace('shrows%d' % rows, lib.slb_shard_rows_workspace_bytes(R, rows), self.device)
+        _lib.check(lib.slb_shard_rows_adagrad(ops._ptr(ids), ops._ptr(g_rows), ops._ptr(g_bias), R,
+                                              ops._ptr(st.Wi), ops._ptr(st.sWi), ops._ptr(st.bi), ops._ptr(st.sbi),
+                                              rows, D, st.lr, st.eps, ops._ptr(ws), ws.numel(), ops._stream()),
+                   'shard_rows_adagrad')
 
 
     # ---- hashed item table (BloomEmbedding, config 4) ----
@@ -219,13 +224,15 @@ class GpuBackend(object):
         hand-back): draw(count) -> (tensor, event the consumer stream must wait for)."""
         return _GpuEpochSampler(self.device, num_items, random_state, total)
 
-    def seq_local_step(self, E_cache, bias_cache, n_cache, seqs_idx, negs_idx, loss, cnn, norm_count):
+    def seq_local_step(self, E_cache, bias_cache, n_cache, seqs_idx, negs_idx, loss, cnn, norm_count,
+                       lstm=None, mixture=None, n_neg=1):
         """Fused sequence step on the row cache (ids already remapped onto it; cache
-        row 0 is the padding row).  Returns (loss share, dE_cache, dbias_cache, dconv_w, dconv_b)."""
-        out = ops.seq_train_step(E_cache, bias_cache.reshape(-1, 1), seqs_idx, negs_idx, loss, 1, cnn,
-                                 norm_count=norm_count)
+        row 0 is the padding row).  Returns (loss share, dE_cache, dbias_cache, dconv_w, dconv_b,
+        dlstm, dmix); ``lstm`` / ``mixture`` / ``n_neg`` as ops.seq_train_step takes them."""
+        out = ops.seq_train_step(E_cache, bias_cache.reshape(-1, 1), seqs_idx, negs_idx, loss, n_neg, cnn,
+                                 norm_count=norm_count, lstm=lstm, mixture=mixture)
         return (out['loss'], out['dE'][:n_cache], out['dbias'].reshape(-1)[:n_cache],
-                out['dconv_w'], out['dconv_b'])
+                out['dconv_w'], out['dconv_b'], out['dlstm'], out['dmix'])
 
 
 _CHUNK_VALUES = 24 << 20        # negatives per sampler chunk: within the one-round reach of the jump table
@@ -605,9 +612,13 @@ class ShardedMF(object):
 
 
 class SeqShardState(object):
-    """Item-embedding / item-bias shards (+ replicated conv weights) and Adagrad state."""
+    """Item-embedding / item-bias shards, the replicated representation parameters and their
+    Adagrad state.  ``convs``: list of (weight (D,D,k,1), bias (D,)) of CNNNet; ``lstm``:
+    dict(w_ih, w_hh, b_ih, b_hh) of LSTMNet / MixtureLSTMNet; ``mixture``: dict(num_mixtures,
+    w (2MD, D, 1), b (2MD,)), MixtureLSTMNet's projection (the forms ops.seq_train_step takes)."""
 
-    def __init__(self, plan, rank, dim, device, lr=0.05, eps=1e-10, init=None, convs=None):
+    def __init__(self, plan, rank, dim, device, lr=0.05, eps=1e-10, init=None, convs=None, lstm=None,
+                 mixture=None):
         ilo, ihi = plan.item_range(rank)
         self.ilo, self.ihi = ilo, ihi
         self.lr, self.eps = float(lr), float(eps)
@@ -625,24 +636,45 @@ class SeqShardState(object):
         # conv weights are replicated: list of (weight (D,D,k,1), bias (D,)) tensors
         self.convs = [(w.clone().to(dev), b.clone().to(dev)) for w, b in (convs or [])]
         self.sconvs = [(torch.zeros_like(w), torch.zeros_like(b)) for w, b in self.convs]
+        self.lstm = None if lstm is None else {k: lstm[k].detach().clone().to(dev).contiguous()
+                                               for k in ('w_ih', 'w_hh', 'b_ih', 'b_hh')}
+        self.slstm = None if lstm is None else {k: torch.zeros_like(v) for k, v in self.lstm.items()}
+        self.mixture = None
+        if mixture is not None:
+            self.mixture = dict(num_mixtures=int(mixture['num_mixtures']),
+                                w=mixture['w'].detach().clone().to(dev).contiguous(),
+                                b=mixture['b'].detach().clone().to(dev).contiguous())
+            self.smixture = {k: torch.zeros_like(self.mixture[k]) for k in ('w', 'b')}
+
+    def replicated(self):
+        """(parameter, Adagrad state) pairs of the replicated parameters, in a fixed order."""
+        out = [p for wb in zip(self.convs, self.sconvs) for p in zip(*wb)]
+        if self.lstm is not None:
+            out += [(self.lstm[k], self.slstm[k]) for k in ('w_ih', 'w_hh', 'b_ih', 'b_hh')]
+        if self.mixture is not None:
+            out += [(self.mixture[k], self.smixture[k]) for k in ('w', 'b')]
+        return out
 
 
 class ShardedSeq(object):
-    """PoolNet / CNNNet training step with range-sharded item rows (SURVEY §8e, config 5).
+    """PoolNet / CNNNet / LSTMNet / MixtureLSTMNet training step with range-sharded item rows
+    (SURVEY §8e, config 5).
 
     Sequences are data-parallel (each rank owns whole sequences); every item row a
     rank's batch touches -- as input, target or negative -- is fetched once per step by
     the same bucket -> all-to-all -> gather -> all-to-all exchange as the MF step, the
     fused sequence kernels run on the row cache, and the per-row gradients return to
     their owners.  The loss is normalised by the *global* number of unmasked positions
-    (one scalar all-reduce up front); conv weights are replicated and their gradients
-    all-reduced.
+    (one scalar all-reduce up front); conv, LSTM and projection weights are replicated
+    (``state``) and their gradients all-reduced.  ``n_neg`` negatives per position
+    (adaptive hinge): ``negs`` holds ``n_neg * B`` rows, row ``q * B + b`` for sequence ``b``.
     """
 
-    def __init__(self, plan, state, rank, backend, cnn=None, group=None, cache_capacity=None):
+    def __init__(self, plan, state, rank, backend, cnn=None, group=None, cache_capacity=None, n_neg=1):
         self.plan, self.st, self.rank, self.backend, self.group = plan, state, rank, backend, group
         self.cnn = cnn                      # dict(kernel_width, dilation, nonlinearity, residual) or None
         self.cache_capacity = cache_capacity
+        self.n_neg = int(n_neg)
         self.stats = {'rows_requested': 0, 'bytes_a2a': 0}
 
     _a2a = ShardedMF._a2a
@@ -677,24 +709,175 @@ class ShardedSeq(object):
             fb[:n_cache] = cache_bias
             cache_rows, cache_bias = full, fb
         self.stats['rows_requested'] += n_cache
-        cnn = None
-        if self.cnn is not None:
-            cnn = dict(self.cnn, weights=[w for w, _ in st.convs], biases=[b for _, b in st.convs])
-        n = B * S
-        loss_share, g_rows, g_bias, dws, dbs = self.backend.seq_local_step(
-            cache_rows, cache_bias, n_cache, inverse[:n].reshape(B, S), inverse[n:2 * n].reshape(B, S),
-            loss, cnn, norm)
+        n, nn = B * S, self.n_neg
+        if B:
+            cnn = None
+            if self.cnn is not None:
+                cnn = dict(self.cnn, weights=[w for w, _ in st.convs], biases=[b for _, b in st.convs])
+            # lstm / mixture / n_neg are passed only when used, so a backend that knows only
+            # PoolNet / CNNNet keeps working for those nets
+            extra = {}
+            if st.lstm is not None:
+                extra['lstm'] = st.lstm
+            if st.mixture is not None:
+                extra['mixture'] = st.mixture
+            if nn != 1:
+                extra['n_neg'] = nn
+            out = self.backend.seq_local_step(
+                cache_rows, cache_bias, n_cache, inverse[:n].reshape(B, S),
+                inverse[n:n + nn * n].reshape(nn * B, S), loss, cnn, norm, **extra)
+            loss_share, g_rows, g_bias = out[:3]
+            grads = [g for pair in zip(out[3], out[4]) for g in pair]
+            dlstm, dmix = (out[5], out[6]) if len(out) > 5 else (None, None)
+            if st.lstm is not None:
+                grads += [dlstm[k] for k in ('w_ih', 'w_hh', 'b_ih', 'b_hh')]
+            if st.mixture is not None:
+                grads += [dmix[k] for k in ('w', 'b')]
+        else:                               # no sequence of this minibatch here: serve peers, join the reductions
+            loss_share = cache_bias.new_zeros(())
+            g_rows, g_bias = cache_rows.new_zeros((n_cache, cache_rows.shape[1])), cache_bias.new_zeros(n_cache)
+            grads = [torch.zeros_like(p) for p, _ in st.replicated()]
         g_recv = self._a2a(g_rows.contiguous(), send_counts, recv_counts)
         gb_recv = self._a2a(g_bias.contiguous(), send_counts, recv_counts)
         self.backend.owner_update(st, local_req, g_recv, gb_recv)
-        for (w, b), (sw, sb), dw, db in zip(st.convs, st.sconvs, dws, dbs):
-            dist.all_reduce(dw, group=self.group)
-            dist.all_reduce(db, group=self.group)
-            adagrad_dense_(w, sw, dw, st.lr, st.eps)
-            adagrad_dense_(b, sb, db, st.lr, st.eps)
+        for (p, s), g in zip(st.replicated(), grads):
+            dist.all_reduce(g, group=self.group)
+            self.backend.adagrad_dense(p, s, g.reshape(p.shape), st.lr, st.eps)
         total = loss_share.detach().clone().reshape(1)
         dist.all_reduce(total, group=self.group)
         return total.reshape(())
+
+
+def _rank_slice(n, rank, world):
+    """[lo, hi) of this rank's near-equal contiguous share of n rows (the first n % world ranks
+    take one more)."""
+    base, extra = divmod(n, world)
+    lo = rank * base + min(rank, extra)
+    return lo, lo + base + (1 if rank < extra else 0)
+
+
+class ShardedImplicitSequenceModel(object):
+    """``ImplicitSequenceModel.fit`` on N GPUs (one process per GPU, one instance per rank), with
+    the *single-process* semantics of the reference loop (sequence/implicit.py:193-264):
+
+    * the constructor draws the torch seed from ``random_state`` and builds the net on the CPU as
+      the single-process model does, so a string ``representation`` starts from the same weights;
+      each rank then keeps only its item range of the embedding table and bias, the
+      representation's own parameters (conv, LSTM, projection) are replicated;
+    * per epoch one shuffle of the sequence rows (applied cumulatively) and one
+      ``sample_items(num_items, (n_seq * n_neg, S))`` draw, from the one global stream that every
+      rank advances identically;
+    * minibatch k is rows ``[k*B, (k+1)*B)``; each rank trains a near-equal contiguous slice of it
+      and the loss and gradients are those of the whole minibatch (:class:`ShardedSeq`);
+    * ``epoch_loss`` is the mean of the global minibatch losses.
+
+    Every rank is handed the same ``SequenceInteractions``.  Optimizer: row-wise Adagrad on the
+    item rows (``spotlight_b200.optim.fused_adagrad``'s update) and Adagrad on the replicated
+    parameters.  Nets: PoolNet, CNNNet, LSTMNet, MixtureLSTMNet on a plain
+    ``ScaledEmbedding(padding_idx=0)`` within the fused step's limits (``net.fusable()``); any
+    other net raises ``ValueError``.
+    """
+
+    def __init__(self, num_items, rank, world, device, loss='pointwise', representation='pooling',
+                 embedding_dim=32, n_iter=10, batch_size=256, learning_rate=1e-2, random_state=None,
+                 num_negative_samples=5, group=None, backend=None):
+        from spotlight_b200.sequence.representations import CNNNet, LSTMNet, MixtureLSTMNet, PoolNet
+        from spotlight_b200.torch_utils import set_seed
+        assert loss in ('pointwise', 'bpr', 'hinge', 'adaptive_hinge')
+        self._loss, self._n_iter, self._batch_size = loss, int(n_iter), int(batch_size)
+        self._n_neg = int(num_negative_samples) if loss == 'adaptive_hinge' else 1
+        self._num_items = int(num_items)
+        self._random_state = random_state or np.random.RandomState()
+        self.rank, self.world, self.device = rank, world, torch.device(device)
+        self.backend = backend or GpuBackend(device)
+        # the single-process model seeds torch from its stream at construction (implicit.py:124)
+        # and builds the net from that seed (_initialize)
+        set_seed(self._random_state.randint(-10 ** 8, 10 ** 8), cuda=self.device.type == 'cuda')
+        builders = {'pooling': PoolNet, 'cnn': CNNNet, 'lstm': LSTMNet, 'mixture': MixtureLSTMNet}
+        if isinstance(representation, str):
+            net = builders[representation](self._num_items, embedding_dim)
+        else:
+            net = representation
+        if not (isinstance(net, (PoolNet, CNNNet, LSTMNet, MixtureLSTMNet)) and net.fusable()):
+            raise ValueError('ShardedImplicitSequenceModel trains PoolNet, CNNNet, LSTMNet and MixtureLSTMNet '
+                             'on a plain ScaledEmbedding(padding_idx=0) within the fused step\'s limits '
+                             '(embedding_dim % 4 == 0); got %s' % type(net).__name__)
+        if net.item_embeddings.num_embeddings != self._num_items:
+            raise ValueError('representation has %d item rows, the model %d'
+                             % (net.item_embeddings.num_embeddings, self._num_items))
+        self._net = net
+        D = net.embedding_dim
+        self.plan = ShardPlan(1, self._num_items, world)
+        cnn = net._cnn_spec()
+        self.state = SeqShardState(
+            self.plan, rank, D, self.device, lr=learning_rate,
+            init=(net.item_embeddings.weight.detach(), net.item_biases.weight.detach()),
+            convs=[(w.detach(), b.detach()) for w, b in zip(cnn['weights'], cnn['biases'])] if cnn else None,
+            lstm=net._lstm_spec(), mixture=net._mixture_spec())
+        spec = None if cnn is None else {k: cnn[k] for k in ('kernel_width', 'dilation', 'nonlinearity', 'residual')}
+        self.seq = ShardedSeq(self.plan, self.state, rank, self.backend, cnn=spec, group=group, n_neg=self._n_neg)
+        self.epoch_losses = []
+
+    def fit(self, interactions, verbose=False):
+        """Fit the model; repeated calls resume (implicit.py:193-264)."""
+        sequences = interactions.sequences
+        if torch.is_tensor(sequences):
+            seqs = sequences.to(self.device, torch.int64).contiguous()
+        else:
+            seqs = self.backend.to_device(np.asarray(sequences).astype(np.int64))
+        n_seq = seqs.shape[0]
+        if n_seq and int(seqs.max()) >= self._num_items:
+            raise ValueError('Maximum item id greater than number of items in model.')
+        B, nn, S = self._batch_size, self._n_neg, seqs.shape[1]
+        for epoch in range(self._n_iter):
+            order = self.backend.shuffled_order(n_seq, self._random_state)
+            seqs = seqs.index_select(0, order.to(seqs.device))
+            del order
+            negatives = self.backend.sample(self._num_items, (n_seq * nn, S), self._random_state)
+            epoch_loss = torch.zeros((), dtype=torch.float64, device=seqs.device)
+            nbatch = 0
+            for lo in range(0, n_seq, B):
+                m = min(B, n_seq - lo)
+                a, c = _rank_slice(m, self.rank, self.world)
+                # the minibatch's negatives are rows q*m + b of its (nn*m, S) block; ours are b in [a, c)
+                block = negatives[lo * nn:(lo + m) * nn].reshape(nn, m, S)
+                mine = block[:, a:c].reshape(nn * (c - a), S)
+                loss = self.seq.step(seqs[lo + a:lo + c], mine, self._loss)
+                epoch_loss += loss.detach().double()
+                nbatch += 1
+            epoch_loss = float(epoch_loss.item()) / max(nbatch, 1)
+            self.epoch_losses.append(epoch_loss)
+            if verbose and self.rank == 0:
+                print('Epoch {}: loss {}'.format(epoch, epoch_loss))
+            if np.isnan(epoch_loss) or epoch_loss == 0.0:
+                raise ValueError('Degenerate epoch loss: {}'.format(epoch_loss))
+        return self
+
+    def gathered_net(self):
+        """Collective: the representation module on this rank's device with the full trained item
+        table and bias (all-gathered from the shards) and the replicated parameters."""
+        st, plan = self.state, self.plan
+        full = []
+        for shard in (st.Wi, st.bi.reshape(-1, 1)):
+            pad = shard.new_zeros((plan.ichunk,) + tuple(shard.shape[1:]))
+            pad[:shard.shape[0]] = shard
+            parts = [torch.empty_like(pad) for _ in range(self.world)]
+            dist.all_gather(parts, pad, group=self.seq.group)
+            full.append(torch.cat(parts)[:self._num_items])
+        net = self._net.to(self.device)
+        with torch.no_grad():
+            net.item_embeddings.weight.copy_(full[0])
+            net.item_biases.weight.copy_(full[1])
+            mine = []
+            for layer in (getattr(net, 'cnn_layers', None) or []):
+                mine += [layer.weight, layer.bias]
+            if st.lstm is not None:
+                mine += [net.lstm.weight_ih_l0, net.lstm.weight_hh_l0, net.lstm.bias_ih_l0, net.lstm.bias_hh_l0]
+            if st.mixture is not None:
+                mine += [net.projection.weight, net.projection.bias]
+            for prm, (val, _) in zip(mine, st.replicated()):
+                prm.copy_(val.reshape(prm.shape))
+        return net
 
 
 class ShardedImplicitFactorizationModel(object):
