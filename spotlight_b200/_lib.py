@@ -38,7 +38,8 @@ EXPORTS = (
     'slb_mf_bloom_workspace_bytes', 'slb_mf_bloom_train_step',
     'slb_bias_sparse_workspace_bytes', 'slb_bias_sparse_apply',
     'slb_unique_workspace_bytes', 'slb_unique_bucket', 'slb_shard_gather_batch', 'slb_adagrad_dense',
-    'slb_shard_rows_workspace_bytes', 'slb_shard_rows_adagrad',
+    'slb_shard_rows_workspace_bytes', 'slb_shard_rows_adagrad', 'slb_shard_rows_adam_catch_up',
+    'slb_shard_rows_adam',
     'slb_loss_workspace_bytes', 'slb_pairwise_loss', 'slb_rating_loss',
     'slb_seq_step_workspace_bytes', 'slb_seq_train_step', 'slb_seq_representation',
     'slb_sort_keys', 'slb_radix_order_workspace_bytes', 'slb_radix_order',
@@ -181,6 +182,10 @@ def _declare(lib):
     lib.slb_shard_rows_workspace_bytes.restype = c_sz
     lib.slb_shard_rows_adagrad.argtypes = [c_vp, c_vp, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_i64, c_i32,
                                            c_f32, c_f32, c_vp, c_sz, c_vp]
+    lib.slb_shard_rows_adam_catch_up.argtypes = [c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_i32,
+                                                 c_vp, c_i64, c_f32, c_f32, c_f32, c_f32, c_f32, c_f32, c_vp]
+    lib.slb_shard_rows_adam.argtypes = [c_vp, c_vp, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_i32,
+                                        c_vp, c_i64, c_f32, c_f32, c_f32, c_f32, c_f32, c_f32, c_vp, c_sz, c_vp]
     lib.slb_loss_workspace_bytes.argtypes = [c_i64]
     lib.slb_loss_workspace_bytes.restype = c_sz
     lib.slb_pairwise_loss.argtypes = [c_i32, c_vp, c_vp, c_vp, c_i64, c_i32, c_vp, c_vp, c_vp,

@@ -85,7 +85,7 @@ adagrad_dense_kernel(float* __restrict__ W, float* __restrict__ S, const float* 
     }
 }
 
-// ---- owner update: row-wise Adagrad of the received gradient rows (slb_shard_rows_adagrad) ----
+// ---- owner update of the received gradient rows (slb_shard_rows_adagrad, slb_shard_rows_adam) ----
 // local_ids entries outside [0, rows) are padding slots: neither counted nor placed.
 __global__ void __launch_bounds__(256)
 rows_count_kernel(const int64_t* __restrict__ ids, int64_t R, int64_t rows, SegIndex seg) {
@@ -161,6 +161,122 @@ rows_adagrad_kernel(const float* __restrict__ g_rows, const float* __restrict__ 
     }
 }
 
+// Lazy-exact Adam, before the owner gathers the requested rows of step t: every requested row and
+// its bias are brought current through step t - 1 (dense Adam moved them at every step they
+// missed, and the peers' forward must see that).  A row can be requested by several peers, so
+// atomicMax on last[row] elects one lane group per distinct row, as mf_adam_prepass_kernel does;
+// the others find it current and read nothing.  A kernel of its own ahead of the gather: a gather
+// fused into it would let a losing group read a row the elected group is still writing.
+template <int LPR, bool VEC4>
+__global__ void __launch_bounds__(256)
+rows_adam_catch_up_kernel(const int64_t* __restrict__ ids, int64_t R, int64_t rows, int D, AdamDev o,
+                          float* __restrict__ W, float* __restrict__ M, float* __restrict__ V, float* __restrict__ b,
+                          float* __restrict__ bm, float* __restrict__ bv, int32_t* __restrict__ last) {
+    constexpr int GROUPS = 256 / LPR;
+    constexpr int STEP = VEC4 ? 4 : 1;
+    const int gl = threadIdx.x & (LPR - 1);
+    const unsigned gmask = group_mask(LPR);
+    const int upto = o.t - 1;
+    for (int64_t k = static_cast<int64_t>(blockIdx.x) * GROUPS + threadIdx.x / LPR; k < R;
+         k += static_cast<int64_t>(gridDim.x) * GROUPS) {
+        const int64_t row = ids[k];
+        if (row < 0 || row >= rows) continue;                 // padding slot (group-uniform)
+        int old = 0;
+        if (gl == 0) old = atomicMax(last + row, upto);
+        old = __shfl_sync(gmask, old, (threadIdx.x & 31) & ~(LPR - 1));
+        if (old >= upto) continue;
+        for (int c = gl * STEP; c < D; c += LPR * STEP) {
+            const int64_t e = row * D + c;
+            if (VEC4) {
+                float4 w = ld4(W + e), m = ld4(M + e), v = ld4(V + e);
+                adam_catch_up(o, old, upto, w, m, v);
+                st4(W + e, w); st4(M + e, m); st4(V + e, v);
+            } else {
+                float w = W[e], m = M[e], v = V[e];
+                adam_catch_up1(o, old, upto, w, m, v);
+                W[e] = w; M[e] = m; V[e] = v;
+            }
+        }
+        if (gl == 0) {
+            float w = b[row], m = bm[row], v = bv[row];
+            adam_catch_up1(o, old, upto, w, m, v);
+            b[row] = w; bm[row] = m; bv[row] = v;
+        }
+    }
+}
+
+// Adam step t on each distinct received row: the segment sum of rows_adagrad_kernel (rank order, no
+// float atomics), then the step on the row and its bias, which share last[row] (= t afterwards).
+// Every received row takes the step, also one whose summed gradient is zero: that step is exactly
+// the catch-up the row would get later.  A row not yet current through t - 1 (an apply without the
+// catch-up ahead of it) is caught up first, as mf_adam_apply_kernel does.  (A kernel of its own, so
+// that rows_adagrad_kernel keeps its code.)
+template <int LPR, bool VEC4>
+__global__ void __launch_bounds__(256, 4)
+rows_adam_kernel(const float* __restrict__ g_rows, const float* __restrict__ g_bias, int D, SegIndex seg, AdamDev o,
+                 float* __restrict__ W, float* __restrict__ M, float* __restrict__ V, float* __restrict__ b,
+                 float* __restrict__ bm, float* __restrict__ bv, int32_t* __restrict__ last) {
+    constexpr int GROUPS = 256 / LPR;
+    constexpr int CAP = seg_sort_cap(LPR);
+    constexpr int STEP = VEC4 ? 4 : 1;
+    __shared__ int32_t sh_sort[GROUPS * 2 * CAP];
+    const int gl = threadIdx.x & (LPR - 1);
+    const int gib = threadIdx.x / LPR;
+    const unsigned gmask = group_mask(LPR);
+    int32_t* sh = sh_sort + gib * 2 * CAP;
+    const int nseg = seg.totals[0];
+    const float ss = __ldg(o.sched + 2 * o.t), bc = __ldg(o.sched + 2 * o.t + 1);
+    for (int64_t s = static_cast<int64_t>(blockIdx.x) * GROUPS + gib; s < nseg;
+         s += static_cast<int64_t>(gridDim.x) * GROUPS) {
+        const int start = seg.seg_start[s];
+        const int len = seg.seg_start[s + 1] - start;
+        const int64_t row = seg.seg_row[s];
+        const int lastv = last[row];
+        float gb = 0.f;
+        for (int c0 = 0; c0 < D; c0 += LPR * STEP) {
+            const int c = c0 + gl * STEP;
+            float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
+            seg_visit_sorted<LPR>(seg.members, start, len, gl, gmask, sh, [&](int32_t t) {
+                const float* src = g_rows + static_cast<int64_t>(t) * D;
+                if (c0 == 0) gb += __ldg(g_bias + t);
+                if (c < D) {
+                    if (VEC4) {
+                        const float4 v = ldg4(src + c);
+                        acc.x += v.x; acc.y += v.y; acc.z += v.z; acc.w += v.w;
+                    } else {
+                        acc.x += __ldg(src + c);
+                    }
+                }
+            }, true);
+            if (c < D) {
+                const int64_t e = row * D + c;
+                if (VEC4) {
+                    float4 w = ld4(W + e), m = ld4(M + e), v = ld4(V + e);
+                    adam_catch_up(o, lastv, o.t - 1, w, m, v);
+                    adam_elem(o, ss, bc, acc.x, w.x, m.x, v.x);
+                    adam_elem(o, ss, bc, acc.y, w.y, m.y, v.y);
+                    adam_elem(o, ss, bc, acc.z, w.z, m.z, v.z);
+                    adam_elem(o, ss, bc, acc.w, w.w, m.w, v.w);
+                    st4(W + e, w); st4(M + e, m); st4(V + e, v);
+                } else {
+                    float w = W[e], m = M[e], v = V[e];
+                    adam_catch_up1(o, lastv, o.t - 1, w, m, v);
+                    adam_elem(o, ss, bc, acc.x, w, m, v);
+                    W[e] = w; M[e] = m; V[e] = v;
+                }
+            }
+        }
+        __syncwarp(gmask);                    // every lane has read last[row] before it moves
+        if (gl == 0) {
+            float w = b[row], m = bm[row], v = bv[row];
+            adam_catch_up1(o, lastv, o.t - 1, w, m, v);
+            adam_elem(o, ss, bc, gb, w, m, v);
+            b[row] = w; bm[row] = m; bv[row] = v;
+            last[row] = o.t;
+        }
+    }
+}
+
 struct RowsLayout { SegIndex seg; size_t bytes; };
 
 RowsLayout rows_layout(void* base, int64_t R, int64_t rows) {
@@ -172,6 +288,23 @@ RowsLayout rows_layout(void* base, int64_t R, int64_t rows) {
 }
 
 bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
+
+// The segment index of the received rows (distinct shard rows ascending, each with its positions
+// in local_ids), shared by both owner updates; hot rows (more than seg_sort_cap(lpr) positions) are
+// pre-sorted.
+int rows_index(const int64_t* local_ids, int64_t R, int64_t rows, int lpr, RowsLayout& l, cudaStream_t st) {
+    l.seg.long_cap = seg_sort_cap(lpr);
+    const int g1 = slb_grid((R + 255) / 256, 8);
+    rows_count_kernel<<<g1, 256, 0, st>>>(local_ids, R, rows, l.seg);
+    SLB_LAUNCH_CHECK("rows_count_kernel");
+    seg_scan_launch(l.seg, rows, st);
+    SLB_LAUNCH_CHECK("seg_scan_kernel");
+    rows_fill_kernel<<<g1, 256, 0, st>>>(local_ids, R, rows, l.seg);
+    SLB_LAUNCH_CHECK("rows_fill_kernel");
+    seg_sort_long_kernel<<<SEG_LONG_CTAS, 256, 0, st>>>(l.seg);     // no-op unless hot rows exist
+    SLB_LAUNCH_CHECK("seg_sort_long_kernel");
+    return SLB_OK;
+}
 
 struct UqLayout { int32_t* flags; SegIndex seg; size_t bytes; };
 
@@ -265,16 +398,8 @@ int slb_shard_rows_adagrad(const int64_t* local_ids, const float* g_rows, const 
     const bool vec4 = dim % 4 == 0 && aligned16(g_rows) && aligned16(W) && aligned16(state_W);
     // lanes per row: one float4 (or one float) per lane, a power of two up to a warp
     const int lpr = lpr_for_dim(vec4 ? dim : 4 * dim);
-    l.seg.long_cap = seg_sort_cap(lpr);
-    const int g1 = slb_grid((R + 255) / 256, 8);
-    rows_count_kernel<<<g1, 256, 0, st>>>(local_ids, R, rows, l.seg);
-    SLB_LAUNCH_CHECK("rows_count_kernel");
-    seg_scan_launch(l.seg, rows, st);
-    SLB_LAUNCH_CHECK("seg_scan_kernel");
-    rows_fill_kernel<<<g1, 256, 0, st>>>(local_ids, R, rows, l.seg);
-    SLB_LAUNCH_CHECK("rows_fill_kernel");
-    seg_sort_long_kernel<<<SEG_LONG_CTAS, 256, 0, st>>>(l.seg);     // no-op unless hot rows exist
-    SLB_LAUNCH_CHECK("seg_sort_long_kernel");
+    const int rc = rows_index(local_ids, R, rows, lpr, l, st);
+    if (rc != SLB_OK) return rc;
     const OptV2 o = {SLB_OPT_ADAGRAD, lr, 0.f, eps};
     const int grid = slb_grid((R + 256 / lpr - 1) / (256 / lpr), 8);
     with_bool(vec4, [&](auto V) {
@@ -283,6 +408,70 @@ int slb_shard_rows_adagrad(const int64_t* local_ids, const float* g_rows, const 
         });
     });
     SLB_LAUNCH_CHECK("rows_adagrad_kernel");
+    return SLB_OK;
+}
+
+int slb_shard_rows_adam_catch_up(const int64_t* local_ids, int64_t R, float* W, float* exp_avg, float* exp_avg_sq,
+                                 float* b, float* b_avg, float* b_avg_sq, int32_t* last, int64_t rows, int32_t dim,
+                                 const float* sched, int64_t step, float beta1, float beta2, float one_minus_beta1,
+                                 float one_minus_beta2, float eps, float weight_decay, slb_stream_t stream) {
+    SLB_REQUIRE(R >= 0 && rows >= 0 && dim >= 1 && step >= 1 && step < (1ll << 31),
+                "shard_rows_adam_catch_up: bad sizes");
+    if (R == 0) return SLB_OK;
+    SLB_REQUIRE(local_ids && W && exp_avg && exp_avg_sq && b && b_avg && b_avg_sq && last && sched,
+                "shard_rows_adam_catch_up: null pointer");
+    SLB_REQUIRE(rows >= 1, "shard_rows_adam_catch_up: rows requested from an empty shard");
+    SLB_REQUIRE(R < (1ll << 31) && rows < (1ll << 31) && dim < (1 << 28), "shard_rows_adam_catch_up: too large");
+    if (step == 1) return SLB_OK;       // nothing pending before the first step
+    const AdamDev o = {beta1, beta2, one_minus_beta1, one_minus_beta2, eps, weight_decay, sched,
+                       static_cast<int32_t>(step)};
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const bool vec4 = dim % 4 == 0 && aligned16(W) && aligned16(exp_avg) && aligned16(exp_avg_sq);
+    const int lpr = lpr_for_dim(vec4 ? dim : 4 * dim);
+    const int grid = slb_grid((R + 256 / lpr - 1) / (256 / lpr), 8);
+    with_bool(vec4, [&](auto V) {
+        with_lpr(lpr, [&](auto L) {
+            rows_adam_catch_up_kernel<L, V><<<grid, 256, 0, st>>>(local_ids, R, rows, dim, o, W, exp_avg, exp_avg_sq,
+                                                                 b, b_avg, b_avg_sq, last);
+        });
+    });
+    SLB_LAUNCH_CHECK("rows_adam_catch_up_kernel");
+    return SLB_OK;
+}
+
+int slb_shard_rows_adam(const int64_t* local_ids, const float* g_rows, const float* g_bias, int64_t R, float* W,
+                        float* exp_avg, float* exp_avg_sq, float* b, float* b_avg, float* b_avg_sq, int32_t* last,
+                        int64_t rows, int32_t dim, const float* sched, int64_t step, float beta1, float beta2,
+                        float one_minus_beta1, float one_minus_beta2, float eps, float weight_decay, void* workspace,
+                        size_t workspace_bytes, slb_stream_t stream) {
+    SLB_REQUIRE(R >= 0 && rows >= 0 && dim >= 1 && step >= 1 && step < (1ll << 31), "shard_rows_adam: bad sizes");
+    if (R == 0) return SLB_OK;          // nothing arrived: the received tensors may have no storage
+    SLB_REQUIRE(local_ids && g_rows && g_bias && W && exp_avg && exp_avg_sq && b && b_avg && b_avg_sq && last &&
+                sched && workspace, "shard_rows_adam: null pointer");
+    SLB_REQUIRE(rows >= 1, "shard_rows_adam: rows arrived for an empty shard");
+    SLB_REQUIRE(R < (1ll << 31) && rows < (1ll << 31) - SEG_SCAN_TILE && dim < (1 << 28),
+                "shard_rows_adam: too large");
+    RowsLayout l = rows_layout(workspace, R, rows);
+    if (workspace_bytes < l.bytes) {
+        slb_set_error("shard_rows_adam: workspace too small (%zu < %zu)", workspace_bytes, l.bytes);
+        return SLB_ENOSPC;
+    }
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const bool vec4 = dim % 4 == 0 && aligned16(g_rows) && aligned16(W) && aligned16(exp_avg) &&
+                      aligned16(exp_avg_sq);
+    const int lpr = lpr_for_dim(vec4 ? dim : 4 * dim);
+    const int rc = rows_index(local_ids, R, rows, lpr, l, st);
+    if (rc != SLB_OK) return rc;
+    const AdamDev o = {beta1, beta2, one_minus_beta1, one_minus_beta2, eps, weight_decay, sched,
+                       static_cast<int32_t>(step)};
+    const int grid = slb_grid((R + 256 / lpr - 1) / (256 / lpr), 8);
+    with_bool(vec4, [&](auto V) {
+        with_lpr(lpr, [&](auto L) {
+            rows_adam_kernel<L, V><<<grid, 256, 0, st>>>(g_rows, g_bias, dim, l.seg, o, W, exp_avg, exp_avg_sq, b,
+                                                        b_avg, b_avg_sq, last);
+        });
+    });
+    SLB_LAUNCH_CHECK("rows_adam_kernel");
     return SLB_OK;
 }
 

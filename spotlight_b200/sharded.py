@@ -151,6 +151,45 @@ class GpuBackend(object):
                                               rows, D, st.lr, st.eps, ops._ptr(ws), ws.numel(), ops._stream()),
                    'shard_rows_adagrad')
 
+    def _adam_tables(self, st, t):
+        """The item shard, its bias and their lazy-exact Adam state, with step t's scalars (the
+        arguments the owner-side Adam entries share after their ids)."""
+        hp = st.opt.fused_hparams()
+        rows, D = st.Wi.shape
+        return (ops._ptr(st.Wi), ops._ptr(st.mWi), ops._ptr(st.vWi), ops._ptr(st.bi), ops._ptr(st.mbi),
+                ops._ptr(st.vbi), ops._ptr(st.last), rows, D, ops._ptr(st.opt.schedule(t, self.device)), t,
+                hp['beta1'], hp['beta2'], 1.0 - hp['beta1'], 1.0 - hp['beta2'], hp['eps'], hp['weight_decay'])
+
+    def owner_adam_catch_up(self, st, local_ids, t):
+        """Lazy-exact Adam before the gather of step t: the requested rows of the item shard and
+        their biases replay the steps they missed, through t - 1."""
+        R = local_ids.numel()
+        if R == 0:
+            return
+        ids = local_ids.contiguous().long()
+        _lib.check(_lib.load().slb_shard_rows_adam_catch_up(ops._ptr(ids), R, *self._adam_tables(st, t),
+                                                            ops._stream()), 'shard_rows_adam_catch_up')
+
+    def owner_adam_update(self, st, local_ids, g_rows, g_bias, t):
+        """Sum the peers' gradient rows per shard row (rank order, deterministic) and take Adam
+        step t on those rows of the item shard and their biases only."""
+        R = local_ids.numel()
+        if R == 0:
+            return
+        lib = _lib.load()
+        ids = local_ids.contiguous().long()
+        g_rows, g_bias = g_rows.contiguous(), g_bias.reshape(-1).contiguous()
+        ws = ops.workspace('shrows%d' % st.Wi.shape[0], lib.slb_shard_rows_workspace_bytes(R, st.Wi.shape[0]),
+                           self.device)
+        _lib.check(lib.slb_shard_rows_adam(ops._ptr(ids), ops._ptr(g_rows), ops._ptr(g_bias), R,
+                                           *self._adam_tables(st, t), ops._ptr(ws), ws.numel(), ops._stream()),
+                   'shard_rows_adam')
+
+    def owner_adam_flush(self, st):
+        """Every row of the item shard and its bias current for the steps taken (FusedAdam.flush);
+        an empty item range has nothing to flush."""
+        if st.Wi.shape[0]:
+            st.opt.flush()
 
     # ---- hashed item table (BloomEmbedding, config 4) ----
     def bloom_local_step(self, st, W_full, users_local, items, negs, loss, global_batch):
@@ -613,12 +652,19 @@ class ShardedMF(object):
 
 class SeqShardState(object):
     """Item-embedding / item-bias shards, the replicated representation parameters and their
-    Adagrad state.  ``convs``: list of (weight (D,D,k,1), bias (D,)) of CNNNet; ``lstm``:
+    optimizer state.  ``convs``: list of (weight (D,D,k,1), bias (D,)) of CNNNet; ``lstm``:
     dict(w_ih, w_hh, b_ih, b_hh) of LSTMNet / MixtureLSTMNet; ``mixture``: dict(num_mixtures,
-    w (2MD, D, 1), b (2MD,)), MixtureLSTMNet's projection (the forms ops.seq_train_step takes)."""
+    w (2MD, D, 1), b (2MD,)), MixtureLSTMNet's projection (the forms ops.seq_train_step takes).
+
+    ``optimizer_func``: None (row-wise Adagrad at ``lr``, ``eps``), ``optim.fused_adagrad`` without
+    weight decay (Adagrad with its ``lr``, ``eps``) or ``optim.fused_adam``; it is called on
+    :meth:`params`.  Under ``fused_adam``, ``opt`` is that ``FusedAdam``: the item shard and its bias
+    (``bi2``, the (rows, 1) view of ``bi``) are its lazily updated table pair, with ``mWi``, ``vWi``,
+    ``last``, ``mbi``, ``vbi`` their moments and the step each row is current for; the replicated
+    parameters take its dense ``step()``."""
 
     def __init__(self, plan, rank, dim, device, lr=0.05, eps=1e-10, init=None, convs=None, lstm=None,
-                 mixture=None):
+                 mixture=None, optimizer_func=None):
         ilo, ihi = plan.item_range(rank)
         self.ilo, self.ihi = ilo, ihi
         self.lr, self.eps = float(lr), float(eps)
@@ -632,28 +678,52 @@ class SeqShardState(object):
             self.bi = torch.zeros(ihi - ilo, device=dev)
             if ilo == 0:
                 self.Wi[0] = 0                      # padding row (PADDING_IDX = 0)
-        self.sWi, self.sbi = torch.zeros_like(self.Wi), torch.zeros_like(self.bi)
+        self.bi2 = self.bi.reshape(-1, 1)
         # conv weights are replicated: list of (weight (D,D,k,1), bias (D,)) tensors
         self.convs = [(w.clone().to(dev), b.clone().to(dev)) for w, b in (convs or [])]
-        self.sconvs = [(torch.zeros_like(w), torch.zeros_like(b)) for w, b in self.convs]
         self.lstm = None if lstm is None else {k: lstm[k].detach().clone().to(dev).contiguous()
                                                for k in ('w_ih', 'w_hh', 'b_ih', 'b_hh')}
-        self.slstm = None if lstm is None else {k: torch.zeros_like(v) for k, v in self.lstm.items()}
         self.mixture = None
         if mixture is not None:
             self.mixture = dict(num_mixtures=int(mixture['num_mixtures']),
                                 w=mixture['w'].detach().clone().to(dev).contiguous(),
                                 b=mixture['b'].detach().clone().to(dev).contiguous())
-            self.smixture = {k: torch.zeros_like(self.mixture[k]) for k in ('w', 'b')}
+        self.opt = None
+        state = torch.zeros_like                    # Adagrad's accumulators
+        if optimizer_func is not None:
+            from spotlight_b200.optim import FusedAdagrad, FusedAdam
+            opt = optimizer_func(self.params())
+            if isinstance(opt, FusedAdam):
+                self.opt = opt
+                self.mWi, self.vWi, self.last = opt.fused_states(self.Wi)
+                self.mbi, self.vbi, _ = opt.fused_states(self.bi2)
+                state = lambda p: None              # noqa: E731
+            elif isinstance(opt, FusedAdagrad) and opt.fused_hparams()['weight_decay'] == 0:
+                hp = opt.fused_hparams()
+                self.lr, self.eps = hp['lr'], hp['eps']
+            else:
+                # fused_adagrad's weight decay moves the rows a minibatch updates, which the owners
+                # do not see as the single-process step does
+                raise ValueError('the sharded sequence model trains with optimizer_func=None (row-wise Adagrad at '
+                                 'learning_rate), optim.fused_adagrad without weight decay or optim.fused_adam; '
+                                 'got %s' % type(opt).__name__)
+        self.sWi, self.sbi = state(self.Wi), state(self.bi)
+        self.srep = [state(p) for p in self.params()[2:]]
+
+    def params(self):
+        """The item shard, its bias as a (rows, 1) view and the replicated parameters, in a fixed
+        order."""
+        out = [self.Wi, self.bi2] + [p for wb in self.convs for p in wb]
+        if self.lstm is not None:
+            out += [self.lstm[k] for k in ('w_ih', 'w_hh', 'b_ih', 'b_hh')]
+        if self.mixture is not None:
+            out += [self.mixture[k] for k in ('w', 'b')]
+        return out
 
     def replicated(self):
-        """(parameter, Adagrad state) pairs of the replicated parameters, in a fixed order."""
-        out = [p for wb in zip(self.convs, self.sconvs) for p in zip(*wb)]
-        if self.lstm is not None:
-            out += [(self.lstm[k], self.slstm[k]) for k in ('w_ih', 'w_hh', 'b_ih', 'b_hh')]
-        if self.mixture is not None:
-            out += [(self.mixture[k], self.smixture[k]) for k in ('w', 'b')]
-        return out
+        """(parameter, Adagrad state) pairs of the replicated parameters, in a fixed order (state
+        None under Adam)."""
+        return list(zip(self.params()[2:], self.srep))
 
 
 class ShardedSeq(object):
@@ -696,6 +766,10 @@ class ShardedSeq(object):
         recv_counts = rc.tolist()
         req = self._a2a(uniq, send_counts, recv_counts)
         local_req = req - st.ilo
+        adam = st.opt is not None
+        if adam:                            # lazy-exact Adam: the requested rows current through t - 1
+            t = st.opt.steps_taken + 1
+            self.backend.owner_adam_catch_up(st, local_req, t)
         rows, bias = self.backend.gather(st.Wi, st.bi, local_req)
         n_cache = uniq.numel()
         # fixed capacity (a function of the batch shape only) so the fused step's workspace is reused
@@ -739,10 +813,21 @@ class ShardedSeq(object):
             grads = [torch.zeros_like(p) for p, _ in st.replicated()]
         g_recv = self._a2a(g_rows.contiguous(), send_counts, recv_counts)
         gb_recv = self._a2a(g_bias.contiguous(), send_counts, recv_counts)
-        self.backend.owner_update(st, local_req, g_recv, gb_recv)
-        for (p, s), g in zip(st.replicated(), grads):
-            dist.all_reduce(g, group=self.group)
-            self.backend.adagrad_dense(p, s, g.reshape(p.shape), st.lr, st.eps)
+        if adam:
+            # step t on the received rows, then FusedAdam.step() takes step t on the replicated
+            # parameters (the only ones carrying a .grad) and counts it, as the single-GPU route does
+            self.backend.owner_adam_update(st, local_req, g_recv, gb_recv, t)
+            for (p, _), g in zip(st.replicated(), grads):
+                dist.all_reduce(g, group=self.group)
+                p.grad = g.reshape(p.shape)
+            st.opt.step()
+            for p, _ in st.replicated():
+                p.grad = None
+        else:
+            self.backend.owner_update(st, local_req, g_recv, gb_recv)
+            for (p, s), g in zip(st.replicated(), grads):
+                dist.all_reduce(g, group=self.group)
+                self.backend.adagrad_dense(p, s, g.reshape(p.shape), st.lr, st.eps)
         total = loss_share.detach().clone().reshape(1)
         dist.all_reduce(total, group=self.group)
         return total.reshape(())
@@ -771,16 +856,26 @@ class ShardedImplicitSequenceModel(object):
       and the loss and gradients are those of the whole minibatch (:class:`ShardedSeq`);
     * ``epoch_loss`` is the mean of the global minibatch losses.
 
-    Every rank is handed the same ``SequenceInteractions``.  Optimizer: row-wise Adagrad on the
-    item rows (``spotlight_b200.optim.fused_adagrad``'s update) and Adagrad on the replicated
-    parameters.  Nets: PoolNet, CNNNet, LSTMNet, MixtureLSTMNet on a plain
+    Every rank is handed the same ``SequenceInteractions``.  Optimizer (``optimizer_func``):
+
+    * ``None``: row-wise Adagrad at ``learning_rate`` on the item rows
+      (``spotlight_b200.optim.fused_adagrad``'s update) and Adagrad on the replicated parameters;
+      ``fused_adagrad(lr, eps)`` without weight decay is the same with its hyper-parameters;
+    * ``fused_adam(lr, betas, eps, weight_decay)``: row-wise lazy-exact Adam on the item rows at
+      their owners and Adam on the replicated parameters at the same step count -- the trajectory
+      of ``ImplicitSequenceModel(optimizer_func=fused_adam(...))``, i.e. dense ``torch.optim.Adam``
+      on every parameter, weight decay included, up to fp32 rounding.  ``fit()`` brings every
+      row current before it returns, and repeated calls resume the step count and the moments;
+    * anything else raises ``ValueError``.
+
+    Nets: PoolNet, CNNNet, LSTMNet, MixtureLSTMNet on a plain
     ``ScaledEmbedding(padding_idx=0)`` within the fused step's limits (``net.fusable()``); any
     other net raises ``ValueError``.
     """
 
     def __init__(self, num_items, rank, world, device, loss='pointwise', representation='pooling',
                  embedding_dim=32, n_iter=10, batch_size=256, learning_rate=1e-2, random_state=None,
-                 num_negative_samples=5, group=None, backend=None):
+                 num_negative_samples=5, group=None, backend=None, optimizer_func=None):
         from spotlight_b200.sequence.representations import CNNNet, LSTMNet, MixtureLSTMNet, PoolNet
         from spotlight_b200.torch_utils import set_seed
         assert loss in ('pointwise', 'bpr', 'hinge', 'adaptive_hinge')
@@ -813,7 +908,7 @@ class ShardedImplicitSequenceModel(object):
             self.plan, rank, D, self.device, lr=learning_rate,
             init=(net.item_embeddings.weight.detach(), net.item_biases.weight.detach()),
             convs=[(w.detach(), b.detach()) for w, b in zip(cnn['weights'], cnn['biases'])] if cnn else None,
-            lstm=net._lstm_spec(), mixture=net._mixture_spec())
+            lstm=net._lstm_spec(), mixture=net._mixture_spec(), optimizer_func=optimizer_func)
         spec = None if cnn is None else {k: cnn[k] for k in ('kernel_width', 'dilation', 'nonlinearity', 'residual')}
         self.seq = ShardedSeq(self.plan, self.state, rank, self.backend, cnn=spec, group=group, n_neg=self._n_neg)
         self.epoch_losses = []
@@ -851,6 +946,8 @@ class ShardedImplicitSequenceModel(object):
                 print('Epoch {}: loss {}'.format(epoch, epoch_loss))
             if np.isnan(epoch_loss) or epoch_loss == 0.0:
                 raise ValueError('Degenerate epoch loss: {}'.format(epoch_loss))
+        if self.state.opt is not None:
+            self.backend.owner_adam_flush(self.state)       # lazy-exact Adam: every row current
         return self
 
     def gathered_net(self):
