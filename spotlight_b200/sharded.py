@@ -83,23 +83,6 @@ class GpuBackend(object):
         host = counts.tolist()                       # the step's one bucketing sync
         return uniq[:host[nparts + 1]], inverse, host[:nparts + 1]
 
-    def unique_bucket_dev(self, ids, rows, chunk, nparts):
-        """As unique_bucket, with nothing read back: (uniq [min(n, rows)] of which the first
-        counts[nparts + 1] entries are valid, inverse, counts = per-owner boundaries + unique count,
-        all on the device)."""
-        lib = _lib.load()
-        ids = ids.contiguous()
-        n = ids.numel()
-        uniq = torch.empty(min(n, rows), dtype=torch.int64, device=ids.device)
-        inverse = torch.empty(n, dtype=torch.int64, device=ids.device)
-        counts = torch.empty(nparts + 2, dtype=torch.int64, device=ids.device)
-        ws = ops.workspace('uq%d' % rows, lib.slb_unique_workspace_bytes(n, rows), ids.device)
-        rc = lib.slb_unique_bucket(ops._ptr(ids), n, rows, chunk, nparts, ops._ptr(uniq),
-                                   ops._ptr(inverse), ops._ptr(counts), ops._ptr(ws), ws.numel(),
-                                   ops._stream())
-        _lib.check(rc, 'unique_bucket')
-        return uniq, inverse, counts
-
     def gather(self, W, b, local_ids):
         rows = ops.embedding(W, local_ids, [], -1)
         bias = ops.embedding(b.reshape(-1, 1), local_ids, [], -1).reshape(-1)
@@ -304,24 +287,6 @@ class _GpuEpochSampler(object):
         self.out.record_stream(torch.cuda.current_stream(self.dev))
 
 
-class _Trace(object):
-    """SLB_TRACE=1: host-clock phase times of fit() with a device sync at each mark (diagnostics)."""
-
-    def __init__(self, rank):
-        import os
-        import time
-        self.on = bool(os.environ.get('SLB_TRACE')) and rank == 0
-        self.time = time
-        self.t = time.perf_counter()
-
-    def __call__(self, what):
-        if self.on:
-            torch.cuda.synchronize()
-            now = self.time.perf_counter()
-            print('[trace] %-8s %.2f ms' % (what, (now - self.t) * 1e3), flush=True)
-            self.t = now
-
-
 class _HostEpochSampler(object):
     """Backend-agnostic fallback: one synchronous draw per request (CPU / gloo tests)."""
 
@@ -370,8 +335,30 @@ class ShardState(object):
         self.sbu, self.sbi = torch.zeros_like(self.bu), torch.zeros_like(self.bi)
 
 
-class ShardedMF(object):
-    """BPR/hinge/pointwise matrix factorisation with range-sharded rows."""
+def _global_loss(loss_share, group):
+    """The global minibatch loss: the sum of the ranks' shares (one scalar all-reduce)."""
+    total = loss_share.detach().clone().reshape(1)
+    dist.all_reduce(total, group=group)
+    return total.reshape(())
+
+
+def _reduce_scatter(x, chunk, rank, group):
+    """This rank's ``chunk`` rows of the sum over ranks of ``x`` (``world * chunk`` rows)."""
+    out = x.new_empty((chunk,) + tuple(x.shape[1:]))
+    try:
+        dist.reduce_scatter_tensor(out, x, group=group)
+    except (RuntimeError, NotImplementedError):          # gloo: sum everywhere, keep our slice
+        y = x.clone()
+        dist.all_reduce(y, group=group)
+        out.copy_(y[rank * chunk:(rank + 1) * chunk])
+    return out
+
+
+class _RowExchange(object):
+    """The per-row item exchange of the MF and sequence steps (module docstring): the distinct
+    item ids of a rank's batch are bucketed by owner and requested with an all-to-all, the owners
+    gather the rows and biases from their shard and send them back, and after the local step the
+    gradient rows travel home the same way.  The owner-side update is the caller's."""
 
     def __init__(self, plan, state, rank, backend, group=None, cache_capacity=None):
         self.plan, self.st, self.rank, self.backend, self.group = plan, state, rank, backend, group
@@ -384,6 +371,53 @@ class ShardedMF(object):
                                input_split_sizes=list(send_counts), group=self.group)
         self.stats['bytes_a2a'] += out.numel() * out.element_size()
         return out
+
+    def _fetch_rows(self, ids, before_gather=None):
+        """Distinct item rows of ``ids`` from their owners: returns (cache_rows, cache_bias,
+        inverse, n_cache, route) with ``ids[k]`` living in cache row ``inverse[k]``.
+        ``before_gather(local_req)`` runs at the owner on the shard rows its peers requested,
+        before it gathers them."""
+        plan, st, P = self.plan, self.st, self.plan.world
+        dev = ids.device
+        if ids.numel():
+            uniq, inverse, bounds = self.backend.unique_bucket(ids, plan.num_items, plan.ichunk, P)
+        else:                               # nothing of this minibatch lives here: serve peers only
+            uniq, inverse, bounds = ids, ids, [0] * (P + 1)
+        send_counts = [bounds[p + 1] - bounds[p] for p in range(P)]
+        sc = torch.tensor(send_counts, dtype=torch.int64, device=dev)
+        rc = torch.empty(P, dtype=torch.int64, device=dev)
+        dist.all_to_all_single(rc, sc, group=self.group)
+        recv_counts = rc.tolist()
+        req = self._a2a(uniq, send_counts, recv_counts)
+        local_req = req - st.ilo
+        if before_gather is not None:
+            before_gather(local_req)
+        rows, bias = self.backend.gather(st.Wi, st.bi, local_req)
+        n_cache = uniq.numel()
+        # fixed capacity (a function of the batch shape only) so the fused step's workspace is reused
+        cap = self.cache_capacity or min(ids.numel(), plan.num_items)
+        cache_rows = self._a2a(rows, recv_counts, send_counts)
+        cache_bias = self._a2a(bias, recv_counts, send_counts)
+        if cap > n_cache:
+            full = cache_rows.new_zeros((cap, cache_rows.shape[1]))
+            full[:n_cache] = cache_rows
+            fb = cache_bias.new_zeros(cap)
+            fb[:n_cache] = cache_bias
+            cache_rows, cache_bias = full, fb
+        self.stats['rows_requested'] += n_cache
+        return cache_rows, cache_bias, inverse, n_cache, (send_counts, recv_counts, local_req)
+
+    def _return_grads(self, route, g_rows, g_bias):
+        """Item gradient rows go home: returns (local_req, g_recv, gb_recv), the shard rows this
+        owner served and the gradient rows and biases its peers sent for them, in rank order."""
+        send_counts, recv_counts, local_req = route
+        g_recv = self._a2a(g_rows.contiguous(), send_counts, recv_counts)
+        gb_recv = self._a2a(g_bias.contiguous(), send_counts, recv_counts)
+        return local_req, g_recv, gb_recv
+
+
+class ShardedMF(_RowExchange):
+    """BPR/hinge/pointwise matrix factorisation with range-sharded rows."""
 
     def _dense_exchange_pays(self, local_batch):
         """When a rank's 2*B item draws cover most of the table anyway, the
@@ -407,8 +441,6 @@ class ShardedMF(object):
         if exchange == 'dense' or (exchange == 'auto' and
                                    self._dense_exchange_pays(global_batch // self.plan.world)):
             return self.step_dense(users, items, negs, loss, global_batch, n_neg)
-        if exchange == 'a2a_fixed':
-            return self.step_a2a_fixed(users, items, negs, loss, global_batch, getattr(self, 'fixed_slots', None))
         return self.step_a2a(users, items, negs, loss, global_batch, n_neg)
 
     def step_dense(self, users, items, negs, loss, global_batch, n_neg=1):
@@ -430,69 +462,13 @@ class ShardedMF(object):
                 st, full_W, full_b, P * chunk, users - st.ulo, items, negs, loss, global_batch, n_neg)
         else:                               # none of this minibatch's users live here
             loss_share, g_rows, g_bias = full_b.new_zeros(()), torch.zeros_like(full_W), torch.zeros_like(full_b)
-        g_shard = self._reduce_scatter(g_rows.contiguous(), chunk)
-        gb_shard = self._reduce_scatter(g_bias.contiguous(), chunk)
+        g_shard = _reduce_scatter(g_rows.contiguous(), chunk, self.rank, self.group)
+        gb_shard = _reduce_scatter(g_bias.contiguous(), chunk, self.rank, self.group)
         self.stats['bytes_a2a'] += (g_rows.numel() + g_bias.numel()) * 4
         n = st.Wi.shape[0]
         adagrad_dense_(st.Wi, st.sWi, g_shard[:n], st.lr, st.eps)
         adagrad_dense_(st.bi, st.sbi, gb_shard[:n], st.lr, st.eps)
-        total = loss_share.detach().clone().reshape(1)
-        dist.all_reduce(total, group=self.group)
-        return total.reshape(())
-
-    def _reduce_scatter(self, x, chunk):
-        out = x.new_empty((chunk,) + tuple(x.shape[1:]))
-        try:
-            dist.reduce_scatter_tensor(out, x, group=self.group)
-        except (RuntimeError, NotImplementedError):          # gloo: sum everywhere, keep our slice
-            y = x.clone()
-            dist.all_reduce(y, group=self.group)
-            out.copy_(y[self.rank * chunk:(self.rank + 1) * chunk])
-        return out
-
-    def _fetch_rows(self, ids):
-        """Distinct item rows of ``ids`` from their owners (steps 1-3 of the exchange):
-        returns (cache_rows, cache_bias, inverse, n_cache, route) with ``ids[k]`` living
-        in cache row ``inverse[k]``."""
-        plan, st, P = self.plan, self.st, self.plan.world
-        dev = ids.device
-        if ids.numel():
-            uniq, inverse, bounds = self.backend.unique_bucket(ids, plan.num_items, plan.ichunk, P)
-        else:                               # nothing of this minibatch lives here: serve peers only
-            uniq, inverse, bounds = ids, ids, [0] * (P + 1)
-        send_counts = [bounds[p + 1] - bounds[p] for p in range(P)]
-        sc = torch.tensor(send_counts, dtype=torch.int64, device=dev)
-        rc = torch.empty(P, dtype=torch.int64, device=dev)
-        dist.all_to_all_single(rc, sc, group=self.group)
-        recv_counts = rc.tolist()
-        req = self._a2a(uniq, send_counts, recv_counts)
-        local_req = req - st.ilo
-        rows, bias = self.backend.gather(st.Wi, st.bi, local_req)
-        n_cache = uniq.numel()
-        # fixed capacity (a function of the batch shape only) so the fused step's workspace is reused
-        cap = self.cache_capacity or min(ids.numel(), plan.num_items)
-        cache_rows = self._a2a(rows, recv_counts, send_counts)
-        cache_bias = self._a2a(bias, recv_counts, send_counts)
-        if cap > n_cache:                  # fixed-capacity cache keeps the kernel workspace layout stable
-            full = cache_rows.new_zeros((cap, cache_rows.shape[1]))
-            full[:n_cache] = cache_rows
-            fb = cache_bias.new_zeros(cap)
-            fb[:n_cache] = cache_bias
-            cache_rows, cache_bias = full, fb
-        self.stats['rows_requested'] += n_cache
-        return cache_rows, cache_bias, inverse, n_cache, (send_counts, recv_counts, local_req)
-
-    def _return_grads(self, route, g_rows, g_bias):
-        """Item gradients go home; owners reduce in rank order and update their shard."""
-        send_counts, recv_counts, local_req = route
-        g_recv = self._a2a(g_rows.contiguous(), send_counts, recv_counts)
-        gb_recv = self._a2a(g_bias.contiguous(), send_counts, recv_counts)
-        self.backend.owner_update(self.st, local_req, g_recv, gb_recv)
-
-    def _global_loss(self, loss_share):
-        total = loss_share.detach().clone().reshape(1)
-        dist.all_reduce(total, group=self.group)
-        return total.reshape(())
+        return _global_loss(loss_share, self.group)
 
     def step_a2a(self, users, items, negs, loss, global_batch, n_neg=1):
         """Per-row routing (the north-star exchange).
@@ -510,75 +486,8 @@ class ShardedMF(object):
                 global_batch, n_neg)
         else:
             loss_share, g_rows, g_bias = st.bi.new_zeros(()), cache_rows[:0], cache_bias[:0]
-        self._return_grads(route, g_rows, g_bias)
-        return self._global_loss(loss_share)
-
-    def step_a2a_fixed(self, users, items, negs, loss, global_batch, slots=None):
-        """Per-row routing WITHOUT host synchronisation: every rank sends every peer a fixed
-        number of request slots (``slots`` per peer; unused slots carry -1), so the all-to-alls
-        have equal, host-known splits and the bucket sizes never leave the device.  Traffic is
-        padded to the slot capacity; a bucket that does not fit raises ``self.overflow`` (a device
-        flag the caller reads once per epoch -- the step's result is then invalid and the epoch
-        must be rerun with more slots or the synchronising ``step_a2a``).
-
-        CPU-verified against the float64 oracle (tests/test_sharded_cpu.py, gloo); not yet run or
-        measured on GPUs (DESIGN.md section 8)."""
-        plan, st, P, be = self.plan, self.st, self.plan.world, self.backend
-        dev = users.device
-        B = users.numel()
-        ids = torch.cat([items, negs])
-        n = ids.numel()
-        C = int(slots or min(plan.ichunk, (3 * max(n, 1)) // (2 * P) + 1024))
-        D = st.Wi.shape[1]
-        if not hasattr(self, 'overflow'):
-            self.overflow = torch.zeros((), dtype=torch.int64, device=dev)
-        if n:
-            uniq, inverse, counts = be.unique_bucket_dev(ids, plan.num_items, plan.ichunk, P)
-            cap = uniq.numel()
-            pos = torch.arange(cap, device=dev)
-            valid = pos < counts[P + 1]
-            owner = torch.where(valid, torch.div(uniq, plan.ichunk, rounding_mode='floor'), torch.zeros_like(uniq))
-            owner = owner.clamp_(0, P - 1)
-            rel = pos - counts[:P + 1][owner]
-            ok = valid & (rel < C) & (rel >= 0)
-            self.overflow += (valid & ~ok).sum()
-            slot = torch.where(ok, owner * C + rel, torch.full_like(rel, P * C))      # P*C = a dump slot
-            req = torch.full((P * C + 1,), -1, dtype=torch.int64, device=dev)
-            req[slot] = torch.where(ok, uniq, torch.full_like(uniq, -1))
-            req = req[:P * C].contiguous()
-        else:
-            cap, inverse = 0, ids
-            req = torch.full((P * C,), -1, dtype=torch.int64, device=dev)
-        got = torch.empty_like(req)
-        dist.all_to_all_single(got, req, group=self.group)
-        live = got >= 0
-        local = torch.where(live, got - st.ilo, torch.zeros_like(got))
-        rows, bias = be.gather(st.Wi, st.bi, local)
-        back_rows, back_bias = torch.empty_like(rows), torch.empty_like(bias)
-        dist.all_to_all_single(back_rows, rows.contiguous(), group=self.group)
-        dist.all_to_all_single(back_bias, bias.contiguous(), group=self.group)
-        self.stats['bytes_a2a'] += 2 * (rows.numel() + bias.numel()) * 4 + 8 * req.numel()
-        if B:
-            take = slot.clamp(max=P * C - 1)
-            okf = ok.to(back_rows.dtype)
-            cache_rows = back_rows[take] * okf[:, None]
-            cache_bias = back_bias[take] * okf
-            loss_share, g_rows, g_bias = be.local_step(st, cache_rows, cache_bias, cap, users - st.ulo,
-                                                       inverse[:B], inverse[B:], loss, global_batch, 1)
-            send_g = g_rows.new_zeros((P * C + 1, D))
-            send_gb = g_bias.new_zeros(P * C + 1)
-            send_g[slot] = g_rows * okf[:, None]
-            send_gb[slot] = g_bias * okf
-            send_g, send_gb = send_g[:P * C].contiguous(), send_gb[:P * C].contiguous()
-        else:
-            loss_share = st.bi.new_zeros(())
-            send_g, send_gb = st.Wi.new_zeros((P * C, D)), st.bi.new_zeros(P * C)
-        g_recv, gb_recv = torch.empty_like(send_g), torch.empty_like(send_gb)
-        dist.all_to_all_single(g_recv, send_g, group=self.group)
-        dist.all_to_all_single(gb_recv, send_gb, group=self.group)
-        # unused slots carry local row 0 with a zero gradient: they add nothing
-        be.owner_update(st, local, g_recv, gb_recv)
-        return self._global_loss(loss_share)
+        self.backend.owner_update(st, *self._return_grads(route, g_rows, g_bias))
+        return _global_loss(loss_share, self.group)
 
     def step_adaptive(self, users, items, negs_block, bpos, batch_users, n_neg):
         """Adaptive hinge on a sharded minibatch, with the reference's pairing.
@@ -646,8 +555,8 @@ class ShardedMF(object):
             g_rows, g_bias = dcache[:n_cache], dbcache.reshape(-1)[:n_cache]
         else:
             g_rows, g_bias = cache_rows[:0], cache_bias[:0]
-        self._return_grads(route, g_rows, g_bias)
-        return self._global_loss(loss_share)
+        self.backend.owner_update(st, *self._return_grads(route, g_rows, g_bias))
+        return _global_loss(loss_share, self.group)
 
 
 class SeqShardState(object):
@@ -726,7 +635,7 @@ class SeqShardState(object):
         return list(zip(self.params()[2:], self.srep))
 
 
-class ShardedSeq(object):
+class ShardedSeq(_RowExchange):
     """PoolNet / CNNNet / LSTMNet / MixtureLSTMNet training step with range-sharded item rows
     (SURVEY §8e, config 5).
 
@@ -741,48 +650,24 @@ class ShardedSeq(object):
     """
 
     def __init__(self, plan, state, rank, backend, cnn=None, group=None, cache_capacity=None, n_neg=1):
-        self.plan, self.st, self.rank, self.backend, self.group = plan, state, rank, backend, group
+        _RowExchange.__init__(self, plan, state, rank, backend, group, cache_capacity)
         self.cnn = cnn                      # dict(kernel_width, dilation, nonlinearity, residual) or None
-        self.cache_capacity = cache_capacity
         self.n_neg = int(n_neg)
-        self.stats = {'rows_requested': 0, 'bytes_a2a': 0}
-
-    _a2a = ShardedMF._a2a
 
     def step(self, seqs, negs, loss):
-        plan, st, P = self.plan, self.st, self.plan.world
+        st = self.st
         B, S = seqs.shape
-        dev = seqs.device
         # global mask count first (device scalar; no host sync)
         norm = (seqs != 0).sum().to(torch.int32).reshape(1)
         dist.all_reduce(norm, group=self.group)
         # distinct ids, with the padding id forced in so that it maps to cache row 0
         ids = torch.cat([seqs.reshape(-1), negs.reshape(-1), seqs.new_zeros(1)])
-        uniq, inverse, bounds = self.backend.unique_bucket(ids, plan.num_items, plan.ichunk, P)
-        send_counts = [bounds[p + 1] - bounds[p] for p in range(P)]
-        sc = torch.tensor(send_counts, dtype=torch.int64, device=dev)
-        rc = torch.empty(P, dtype=torch.int64, device=dev)
-        dist.all_to_all_single(rc, sc, group=self.group)
-        recv_counts = rc.tolist()
-        req = self._a2a(uniq, send_counts, recv_counts)
-        local_req = req - st.ilo
         adam = st.opt is not None
+        catch_up = None
         if adam:                            # lazy-exact Adam: the requested rows current through t - 1
             t = st.opt.steps_taken + 1
-            self.backend.owner_adam_catch_up(st, local_req, t)
-        rows, bias = self.backend.gather(st.Wi, st.bi, local_req)
-        n_cache = uniq.numel()
-        # fixed capacity (a function of the batch shape only) so the fused step's workspace is reused
-        cap = self.cache_capacity or min(ids.numel(), plan.num_items)
-        cache_rows = self._a2a(rows, recv_counts, send_counts)
-        cache_bias = self._a2a(bias, recv_counts, send_counts)
-        if cap != n_cache:
-            full = cache_rows.new_zeros((cap, cache_rows.shape[1]))
-            full[:n_cache] = cache_rows
-            fb = cache_bias.new_zeros(cap)
-            fb[:n_cache] = cache_bias
-            cache_rows, cache_bias = full, fb
-        self.stats['rows_requested'] += n_cache
+            catch_up = lambda local_req: self.backend.owner_adam_catch_up(st, local_req, t)    # noqa: E731
+        cache_rows, cache_bias, inverse, n_cache, route = self._fetch_rows(ids, catch_up)
         n, nn = B * S, self.n_neg
         if B:
             cnn = None
@@ -811,12 +696,11 @@ class ShardedSeq(object):
             loss_share = cache_bias.new_zeros(())
             g_rows, g_bias = cache_rows.new_zeros((n_cache, cache_rows.shape[1])), cache_bias.new_zeros(n_cache)
             grads = [torch.zeros_like(p) for p, _ in st.replicated()]
-        g_recv = self._a2a(g_rows.contiguous(), send_counts, recv_counts)
-        gb_recv = self._a2a(g_bias.contiguous(), send_counts, recv_counts)
+        returned = self._return_grads(route, g_rows, g_bias)
         if adam:
             # step t on the received rows, then FusedAdam.step() takes step t on the replicated
             # parameters (the only ones carrying a .grad) and counts it, as the single-GPU route does
-            self.backend.owner_adam_update(st, local_req, g_recv, gb_recv, t)
+            self.backend.owner_adam_update(st, *returned, t)
             for (p, _), g in zip(st.replicated(), grads):
                 dist.all_reduce(g, group=self.group)
                 p.grad = g.reshape(p.shape)
@@ -824,13 +708,11 @@ class ShardedSeq(object):
             for p, _ in st.replicated():
                 p.grad = None
         else:
-            self.backend.owner_update(st, local_req, g_recv, gb_recv)
+            self.backend.owner_update(st, *returned)
             for (p, s), g in zip(st.replicated(), grads):
                 dist.all_reduce(g, group=self.group)
                 self.backend.adagrad_dense(p, s, g.reshape(p.shape), st.lr, st.eps)
-        total = loss_share.detach().clone().reshape(1)
-        dist.all_reduce(total, group=self.group)
-        return total.reshape(())
+        return _global_loss(loss_share, self.group)
 
 
 def _rank_slice(n, rank, world):
@@ -1019,7 +901,6 @@ class ShardedImplicitFactorizationModel(object):
     def fit(self, interactions, verbose=False):
         be = self.backend
         n = len(interactions.user_ids)
-        trace = _Trace(self.rank)
         if hasattr(be, 'upload_sharded'):
             users_dev = be.upload_sharded(interactions.user_ids, self.rank, self.world, self.mf.group)
             items_dev = be.upload_sharded(interactions.item_ids, self.rank, self.world, self.mf.group)
@@ -1028,7 +909,6 @@ class ShardedImplicitFactorizationModel(object):
             items_dev = be.to_device(interactions.item_ids)
         if users_dev.dtype != items_dev.dtype:
             users_dev, items_dev = users_dev.long(), items_dev.long()
-        trace('upload')
         if n:
             umax, imax = torch.stack([users_dev.max(), items_dev.max()]).tolist()      # one sync
             if umax >= self._num_users:
@@ -1036,15 +916,11 @@ class ShardedImplicitFactorizationModel(object):
             if imax >= self._num_items:
                 raise ValueError('Maximum item id greater than number of items in model.')
         for epoch in range(self._n_iter):
-            trace('check')
             order = be.shuffled_order(n, self._random_state)
-            trace('shuffle')
             u, i = be.permute(order, users_dev, items_dev)
             del order
-            trace('permute')
             epoch_loss = self._run_epoch_device(u, i)
             del u, i
-            trace('epoch')
             self.epoch_losses.append(epoch_loss)
             if verbose and self.rank == 0:
                 print('Epoch {}: loss {}'.format(epoch, epoch_loss))
@@ -1154,12 +1030,6 @@ class ShardedImplicitFactorizationModel(object):
             _, ev = sampler.draw(min(hi_k * B, n) - k * B)
             waits.append((k, ev))
             k = hi_k
-        import os
-        if os.environ.get('SLB_SAMPLER_UPFRONT'):
-            # experiment switch (DESIGN.md section 8.3): every chunk becomes a dependency of step 0,
-            # i.e. the whole epoch's negatives are drawn before the first step and nothing of the
-            # generator overlaps the training kernels
-            waits = [(0, ev) for _, ev in waits]
         negs_all = sampler.out
         plan_ev = [torch.cuda.Event(), torch.cuda.Event()]
         done_ev = [torch.cuda.Event(), torch.cuda.Event()]
@@ -1201,59 +1071,30 @@ class ShardedImplicitFactorizationModel(object):
                                                             ops._stream()), 'plan')
                 plan_ev[slot].record(pstream)
 
-        import os
-        import time
-        trace = bool(os.environ.get('SLB_TRACE_STEP'))      # diagnostics: device time per phase (events), host time per step
-        marks, host_t = [], []
-
-        def mark():
-            if trace:
-                e = torch.cuda.Event(enable_timing=True)
-                e.record(main)
-                marks.append(e)
-
         prep(0)
         for k in range(nsteps):
-            t_host = time.perf_counter()
             if k + 1 < nsteps:
                 prep(k + 1)
             slot = k & 1
             m = bounds[k + 1] - bounds[k]
-            mark()
             dist.all_gather_into_tensor(buf['full_W'], st.Wi, group=self.mf.group)
             dist.all_gather_into_tensor(buf['full_b'], st.bi, group=self.mf.group)
-            mark()
             buf['dW'].zero_()
             buf['db'].zero_()
             main.wait_event(plan_ev[slot])
-            mark()
             if m:
                 _lib.check(lib.slb_mf_train_step_phases(ctypes.byref(args[slot]), 6 | (slot << 8),
                                                         ops._stream()), 'step')
             done_ev[slot].record(main)
-            mark()
             dist.reduce_scatter_tensor(buf['gW'], buf['dW'], group=self.mf.group)
             dist.reduce_scatter_tensor(buf['gb'], buf['db'], group=self.mf.group)
-            mark()
             _lib.check(lib.slb_adagrad_dense(ops._ptr(st.Wi), ops._ptr(st.sWi), ops._ptr(buf['gW']), chunk * D,
                                              st.lr, st.eps, ops._stream()), 'adagrad')
             _lib.check(lib.slb_adagrad_dense(ops._ptr(st.bi), ops._ptr(st.sbi), ops._ptr(buf['gb']), chunk,
                                              st.lr, st.eps, ops._stream()), 'adagrad')
-            mark()
-            host_t.append(time.perf_counter() - t_host)
-        if trace and self.rank == 0 and nsteps > 4:
-            torch.cuda.synchronize()
-            names = ['all_gather', 'zero+wait_plan', 'user+item', 'reduce_scatter', 'adagrad', 'gap_to_next']
-            acc = [0.0] * 6
-            for k in range(2, nsteps - 1):
-                ev = marks[6 * k:6 * k + 7]
-                for j in range(6):
-                    acc[j] += ev[j].elapsed_time(ev[j + 1])
-            print('[trace-step] world %d device ms per step:' % self.world,
-                  {nm: round(v / (nsteps - 3), 4) for nm, v in zip(names, acc)},
-                  'host ms per step %.3f' % (1e3 * sum(host_t[2:]) / len(host_t[2:])), flush=True)
-            self.mf.stats['bytes_a2a'] += 2 * (buf['full_W'].numel() + buf['full_b'].numel()) * 4
-            self.mf.stats['rows_requested'] += P * chunk
+        # each step moved what ShardedMF.step_dense counts: the whole table there and its gradient back
+        self.mf.stats['rows_requested'] += nsteps * P * chunk
+        self.mf.stats['bytes_a2a'] += nsteps * 2 * (buf['full_W'].numel() + buf['full_b'].numel()) * 4
         pstream.wait_stream(main)                              # later plan-stream work follows this epoch
         dist.all_reduce(losses, group=self.mf.group)           # one reduction per epoch: global minibatch losses
         sampler.finish()
@@ -1338,13 +1179,7 @@ class ShardedBloomMF(object):
         else:
             loss_share = st.bu.new_zeros(())
             dW_pad = st.Wi.new_zeros((P * st.mchunk, D))
-        g_shard = st.Wi.new_empty((st.mchunk, D))
-        try:
-            dist.reduce_scatter_tensor(g_shard, dW_pad, group=self.group)
-        except (RuntimeError, NotImplementedError):          # gloo: sum everywhere, keep our slice
-            y = dW_pad.clone()
-            dist.all_reduce(y, group=self.group)
-            g_shard.copy_(y[self.rank * st.mchunk:(self.rank + 1) * st.mchunk])
+        g_shard = _reduce_scatter(dW_pad, st.mchunk, self.rank, self.group)
         be.adagrad_dense(st.Wi, st.sWi, g_shard, st.lr, st.eps)
         ids_all = torch.empty(P * cap, dtype=torch.int64, device=dev)
         g_all = torch.empty(P * cap, dtype=torch.float32, device=dev)
@@ -1352,7 +1187,5 @@ class ShardedBloomMF(object):
         dist.all_gather_into_tensor(g_all, g_pad, group=self.group)
         be.bias_sparse_adagrad(ids_all, g_all, st.bi, st.sbi, st.lr, st.eps)
         self.stats['bytes_exchanged'] += (W_full.numel() + dW_pad.numel()) * 4 + P * cap * 12
-        total = loss_share.detach().clone().reshape(1)
-        dist.all_reduce(total, group=self.group)
-        return total.reshape(())
+        return _global_loss(loss_share, self.group)
 

@@ -1,13 +1,83 @@
 """Shared driver for the sharded-step tests (CPU/gloo with a NumPy backend,
-GPU/NCCL with the product backend): runs a few global steps on `world` ranks
-and on a single-process oracle, and returns both parameter sets."""
+GPU/NCCL with the product backend): spawns a process group of `world` ranks, runs a
+few global steps on it and on a single-process oracle, and returns both parameter sets."""
+
+import os
+import shutil
+import tempfile
 
 import numpy as np
 import torch
 import torch.distributed as dist
+import torch.multiprocessing as mp
 
 from oracle import mf as omf
 from oracle import seq as oseq
+
+
+def _rank_main(rank, world, store, q, backend, job, args):
+    try:
+        if backend == 'nccl':
+            torch.cuda.set_device(rank)
+            dev = torch.device('cuda', rank)
+            dist.init_process_group('nccl', init_method=store, rank=rank, world_size=world, device_id=dev)
+        else:
+            dev = torch.device('cpu')
+            dist.init_process_group('gloo', init_method=store, rank=rank, world_size=world)
+        out = job(rank, world, dev, *args)
+        if backend == 'nccl':
+            torch.cuda.synchronize()
+        q.put((rank, out, None))
+    except Exception:                        # surface the traceback in the parent
+        import traceback
+        q.put((rank, None, traceback.format_exc()))
+    finally:
+        if dist.is_initialized():
+            dist.destroy_process_group()
+
+
+def run_world(job, world, args=(), backend='gloo', timeout=300):
+    """Runs ``job(rank, world, device, *args)`` (a module-level function) on ``world`` spawned
+    ranks of one process group -- ``gloo`` on the CPU, or ``nccl`` with rank r on GPU r.  Returns
+    {rank: result}; a rank that raises fails the caller with its traceback.
+
+    The ranks meet through a file in a fresh temporary directory rather than on a TCP port, so
+    a port some other socket holds cannot stall or fail the group; ranks still running when the
+    call fails are terminated, so none outlives it."""
+    ctx = mp.get_context('spawn')
+    q = ctx.Queue()
+    rendezvous = tempfile.mkdtemp(prefix='sharded_world_')
+    store = 'file://' + os.path.join(rendezvous, 'store')
+    procs = [ctx.Process(target=_rank_main, args=(r, world, store, q, backend, job, tuple(args)))
+             for r in range(world)]
+    try:
+        for p in procs:
+            p.start()
+        res = {}
+        for _ in range(world):
+            rank, out, err = q.get(timeout=timeout)
+            assert err is None, 'rank %d failed:\n%s' % (rank, err)
+            res[rank] = out
+        for p in procs:
+            p.join(timeout=120)
+            assert p.exitcode == 0
+        return res
+    finally:
+        for p in procs:
+            if p.is_alive():
+                p.terminate()
+                p.join()
+        shutil.rmtree(rendezvous, ignore_errors=True)
+
+
+def gather_rows(shard, chunk, n):
+    """The first ``n`` rows of a range-sharded table, as NumPy, from every rank's ``shard`` of at
+    most ``chunk`` rows: each padded to ``chunk`` rows, all-gathered and concatenated in rank order."""
+    pad = shard.new_zeros((chunk,) + tuple(shard.shape[1:]))
+    pad[:shard.shape[0]] = shard
+    parts = [torch.empty_like(pad) for _ in range(dist.get_world_size())]
+    dist.all_gather(parts, pad)
+    return torch.cat(parts)[:n].cpu().numpy()
 
 
 class NumpyBackend(object):
@@ -18,12 +88,6 @@ class NumpyBackend(object):
         uniq, inverse = np.unique(x, return_inverse=True)
         bounds = [int(np.searchsorted(uniq, p * chunk)) for p in range(nparts)] + [len(uniq)]
         return torch.from_numpy(uniq), torch.from_numpy(inverse.astype(np.int64)), bounds
-
-    def unique_bucket_dev(self, ids, rows, chunk, nparts):
-        uniq, inverse, bounds = self.unique_bucket(ids, rows, chunk, nparts)
-        pad = torch.full((min(ids.numel(), rows),), 123456789, dtype=torch.int64)     # garbage beyond the count
-        pad[:uniq.numel()] = uniq
-        return pad, inverse, torch.tensor(bounds + [uniq.numel()], dtype=torch.int64)
 
     def gather(self, W, b, local_ids):
         i = local_ids.numpy()
@@ -181,30 +245,20 @@ def oracle_run(params, batches, loss, lr, eps=1e-10, n_neg=1):
 
 
 def sharded_run(rank, world, params, batches, loss, lr, device, backend, cache_capacity=None,
-                exchange='a2a', fixed_slots=None):
-    """Runs the steps on this rank; returns (all-gathered full tables, losses)."""
+                exchange='a2a'):
+    """Runs the steps on this rank; returns (all-gathered full tables, losses, exchange stats)."""
     from spotlight_b200.sharded import ShardedMF, ShardPlan, ShardState
     U, D = params[0].shape
     I = params[1].shape[0]
     plan = ShardPlan(U, I, world)
     st = ShardState(plan, rank, D, device, lr=lr, init=[torch.from_numpy(p) for p in params])
     model = ShardedMF(plan, st, rank, backend, cache_capacity=cache_capacity)
-    model.fixed_slots = fixed_slots
     losses = []
     for users, items, negs in batches:
         mine = plan.user_owner(users) == rank
         t = lambda x: torch.from_numpy(x[mine]).to(device)        # noqa: E731
         losses.append(float(model.step(t(users), t(items), t(negs), loss, len(users), exchange)))
-    out = []
-    for shard, n, chunk in ((st.Wu, U, plan.uchunk), (st.Wi, I, plan.ichunk),
-                            (st.bu.reshape(-1, 1), U, plan.uchunk), (st.bi.reshape(-1, 1), I, plan.ichunk)):
-        pad = torch.zeros((chunk,) + tuple(shard.shape[1:]), dtype=shard.dtype, device=shard.device)
-        pad[:shard.shape[0]] = shard
-        parts = [torch.empty_like(pad) for _ in range(world)]
-        dist.all_gather(parts, pad)
-        out.append(torch.cat(parts)[:n].cpu().numpy())
-    stats = dict(model.stats, overflow=int(getattr(model, 'overflow', 0)))
-    return out, losses, stats
+    return gather_tables(st, plan, U, I), losses, model.stats
 
 
 def make_seq_problem(seed, I, D, B, S, steps, layers=0, k=3):
@@ -259,13 +313,7 @@ def seq_sharded_run(rank, world, params, batches, loss, lr, device, backend, cnn
     for seqs, negs in batches:
         t = lambda x: torch.from_numpy(np.ascontiguousarray(x[rank::world])).to(device)   # noqa: E731
         losses.append(float(model.step(t(seqs), t(negs), loss)))
-    out = []
-    for shard in (st.Wi, st.bi.reshape(-1, 1)):
-        pad = torch.zeros((plan.ichunk,) + tuple(shard.shape[1:]), dtype=shard.dtype, device=shard.device)
-        pad[:shard.shape[0]] = shard
-        parts = [torch.empty_like(pad) for _ in range(world)]
-        dist.all_gather(parts, pad)
-        out.append(torch.cat(parts)[:I].cpu().numpy())
+    out = [gather_rows(st.Wi, plan.ichunk, I), gather_rows(st.bi.reshape(-1, 1), plan.ichunk, I)]
     out += [x.cpu().numpy() for wb in st.convs for x in wb]
     return out, losses, model.stats
 
@@ -288,16 +336,11 @@ def reference_epochs(seed, users, items, num_items, B, n_iter, n_neg=1):
     return epochs, rs
 
 
-def gather_tables(st, plan, U, I, world):
-    out = []
-    for shard, n, chunk in ((st.Wu, U, plan.uchunk), (st.Wi, I, plan.ichunk),
-                            (st.bu.reshape(-1, 1), U, plan.uchunk), (st.bi.reshape(-1, 1), I, plan.ichunk)):
-        pad = torch.zeros((chunk,) + tuple(shard.shape[1:]), dtype=shard.dtype, device=shard.device)
-        pad[:shard.shape[0]] = shard
-        parts = [torch.empty_like(pad) for _ in range(world)]
-        dist.all_gather(parts, pad)
-        out.append(torch.cat(parts)[:n].cpu().numpy())
-    return out
+def gather_tables(st, plan, U, I):
+    """The full Wu, Wi, bu and bi (biases as columns) of a ShardState on every rank."""
+    return [gather_rows(shard, chunk, n) for shard, n, chunk in
+            ((st.Wu, U, plan.uchunk), (st.Wi, I, plan.ichunk),
+             (st.bu.reshape(-1, 1), U, plan.uchunk), (st.bi.reshape(-1, 1), I, plan.ichunk))]
 
 
 def sharded_fit_run(rank, world, params, users, items, loss, device, backend, seed, B, n_iter, exchange,
@@ -313,7 +356,7 @@ def sharded_fit_run(rank, world, params, users, items, loss, device, backend, se
                                               init=[torch.from_numpy(p) for p in params],
                                               num_negative_samples=n_neg)
     model.fit(Interactions(users, items, num_users=U, num_items=I))
-    return gather_tables(model.state, model.plan, U, I, world), model.epoch_losses, rs.get_state()
+    return gather_tables(model.state, model.plan, U, I), model.epoch_losses, rs.get_state()
 
 
 # ---------------------------------------------------------------- hashed item table (config 4)
@@ -355,13 +398,8 @@ def bloom_sharded_run(rank, world, params, batches, loss, lr, device, backend, H
         mine = plan.user_owner(users) == rank
         t = lambda x: torch.from_numpy(x[mine]).to(device)        # noqa: E731
         losses.append(float(model.step(t(users), t(items), t(negs), loss, len(users))))
-    out = []
-    for shard, n, chunk in ((st.Wu, U, plan.uchunk), (st.Wi, M, st.mchunk), (st.bu.reshape(-1, 1), U, plan.uchunk)):
-        pad = torch.zeros((chunk,) + tuple(shard.shape[1:]), dtype=shard.dtype, device=shard.device)
-        pad[:shard.shape[0]] = shard
-        parts = [torch.empty_like(pad) for _ in range(world)]
-        dist.all_gather(parts, pad)
-        out.append(torch.cat(parts)[:n].cpu().numpy())
+    out = [gather_rows(shard, chunk, n) for shard, n, chunk in
+           ((st.Wu, U, plan.uchunk), (st.Wi, M, st.mchunk), (st.bu.reshape(-1, 1), U, plan.uchunk))]
     out.append(st.bi.reshape(-1, 1).cpu().numpy())           # replicated
     return out, losses
 

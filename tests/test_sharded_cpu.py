@@ -15,45 +15,24 @@ import sys
 import numpy as np
 import pytest
 import torch
-import torch.distributed as dist
-import torch.multiprocessing as mp
 
 from conftest import ROOT, assert_close
 
 sys.path.insert(0, os.path.join(ROOT, 'tests'))
 
+import sharded_common as sc            # noqa: E402
 
-def _worker(rank, world, port, loss, q, exchange='a2a', fixed_slots=None):
-    import sharded_common as sc
-    os.environ['MASTER_ADDR'] = '127.0.0.1'
-    os.environ['MASTER_PORT'] = str(port)
-    dist.init_process_group('gloo', rank=rank, world_size=world)
-    try:
-        params, batches = sc.make_problem(5, 101, 57, 8, 96, 3)
-        got, losses, stats = sc.sharded_run(rank, world, params, batches, loss, 0.05, 'cpu',
-                                            sc.NumpyBackend(), exchange=exchange, fixed_slots=fixed_slots)
-        if rank == 0:
-            q.put((got, losses, stats))
-    finally:
-        dist.destroy_process_group()
+
+def _step_job(rank, world, dev, loss, exchange):
+    params, batches = sc.make_problem(5, 101, 57, 8, 96, 3)
+    return sc.sharded_run(rank, world, params, batches, loss, 0.05, dev, sc.NumpyBackend(), exchange=exchange)
 
 
 @pytest.mark.parametrize('world,loss,exchange', [(2, 'bpr', 'a2a'), (3, 'bpr', 'a2a'),
                                                  (2, 'pointwise', 'a2a'), (2, 'bpr', 'dense'),
-                                                 (3, 'pointwise', 'dense'), (2, 'bpr', 'a2a_fixed'),
-                                                 (3, 'pointwise', 'a2a_fixed')])
+                                                 (3, 'pointwise', 'dense')])
 def test_sharded_step_matches_single_process(world, loss, exchange):
-    import sharded_common as sc
-    ctx = mp.get_context('spawn')
-    q = ctx.Queue()
-    port = 29500 + (os.getpid() + world * 7) % 2000
-    procs = [ctx.Process(target=_worker, args=(r, world, port, loss, q, exchange)) for r in range(world)]
-    for p in procs:
-        p.start()
-    got, losses, stats = q.get(timeout=240)
-    for p in procs:
-        p.join(timeout=60)
-        assert p.exitcode == 0
+    got, losses, stats = sc.run_world(_step_job, world, (loss, exchange))[0]
     params, batches = sc.make_problem(5, 101, 57, 8, 96, 3)
     ref, ref_losses = sc.oracle_run(params, batches, loss, 0.05)
     assert_close(np.array(losses), np.array(ref_losses), 1e-5, what='losses')
@@ -62,43 +41,15 @@ def test_sharded_step_matches_single_process(world, loss, exchange):
     # each distinct row crosses the wire once per rank per step, never per use
     if exchange == 'a2a':
         assert stats['rows_requested'] <= 3 * 57
-    if exchange == 'a2a_fixed':
-        assert stats['overflow'] == 0
-
-
-def test_fixed_slot_exchange_reports_overflow():
-    """Too few request slots per peer: the no-sync exchange must say so (device flag), not
-    silently train on a truncated row cache."""
-    ctx = mp.get_context('spawn')
-    q = ctx.Queue()
-    port = 26500 + os.getpid() % 2000
-    procs = [ctx.Process(target=_worker, args=(r, 2, port, 'bpr', q, 'a2a_fixed', 3)) for r in range(2)]
-    for p in procs:
-        p.start()
-    got, losses, stats = q.get(timeout=240)
-    for p in procs:
-        p.join(timeout=60)
-        assert p.exitcode == 0
-    assert stats['overflow'] > 0
 
 
 _CNN = dict(kernel_width=[3, 3], dilation=[1, 2], nonlinearity='tanh', residual=True)
 
 
-def _seq_worker(rank, world, port, loss, net, q):
-    import sharded_common as sc
-    os.environ['MASTER_ADDR'] = '127.0.0.1'
-    os.environ['MASTER_PORT'] = str(port)
-    dist.init_process_group('gloo', rank=rank, world_size=world)
-    try:
-        cnn = _CNN if net == 'cnn' else None
-        params, batches = sc.make_seq_problem(9, 41, 8, 10, 7, 3, layers=2 if cnn else 0)
-        got, losses, stats = sc.seq_sharded_run(rank, world, params, batches, loss, 0.05, 'cpu',
-                                                sc.NumpyBackend(), cnn=cnn)
-        if rank == 0:
-            q.put((got, losses, stats))
-    finally:
-        dist.destroy_process_group()
+def _seq_job(rank, world, dev, loss, net):
+    cnn = _CNN if net == 'cnn' else None
+    params, batches = sc.make_seq_problem(9, 41, 8, 10, 7, 3, layers=2 if cnn else 0)
+    return sc.seq_sharded_run(rank, world, params, batches, loss, 0.05, dev, sc.NumpyBackend(), cnn=cnn)
 
 
 @pytest.mark.parametrize('world,loss,net', [(2, 'bpr', 'pool'), (3, 'pointwise', 'pool'),
@@ -107,17 +58,7 @@ def test_sharded_sequence_step_matches_single_process(world, loss, net):
     """Sequence models (SURVEY §8e, config 5): sequences are data-parallel, item rows
     range-sharded and fetched once per step, conv weights replicated + all-reduced,
     loss normalised by the global unmasked count."""
-    import sharded_common as sc
-    ctx = mp.get_context('spawn')
-    q = ctx.Queue()
-    port = 31500 + (os.getpid() + world * 11) % 2000
-    procs = [ctx.Process(target=_seq_worker, args=(r, world, port, loss, net, q)) for r in range(world)]
-    for p in procs:
-        p.start()
-    got, losses, stats = q.get(timeout=240)
-    for p in procs:
-        p.join(timeout=60)
-        assert p.exitcode == 0
+    got, losses, stats = sc.run_world(_seq_job, world, (loss, net))[0]
     cnn = _CNN if net == 'cnn' else None
     params, batches = sc.make_seq_problem(9, 41, 8, 10, 7, 3, layers=2 if cnn else 0)
     ref, ref_losses = sc.seq_oracle_run(params, batches, loss, 0.05, cnn=cnn)
@@ -134,25 +75,16 @@ FIT = dict(seed=21, U=61, I=37, D=8, n=500, B=64, n_iter=2)
 
 def _fit_problem():
     rs = np.random.RandomState(4)
-    params, _ = __import__('sharded_common').make_problem(5, FIT['U'], FIT['I'], FIT['D'], 8, 0)
+    params, _ = sc.make_problem(5, FIT['U'], FIT['I'], FIT['D'], 8, 0)
     users = rs.randint(0, 40, FIT['n']).astype(np.int32)          # world 3: rank 2 owns users >= 42, always empty
     items = rs.randint(0, FIT['I'], FIT['n']).astype(np.int32)
     return params, users, items
 
 
-def _fit_worker(rank, world, port, loss, exchange, q):
-    import sharded_common as sc
-    os.environ['MASTER_ADDR'] = '127.0.0.1'
-    os.environ['MASTER_PORT'] = str(port)
-    dist.init_process_group('gloo', rank=rank, world_size=world)
-    try:
-        params, users, items = _fit_problem()
-        out = sc.sharded_fit_run(rank, world, params, users, items, loss, 'cpu', sc.NumpyBackend(),
-                                 FIT['seed'], FIT['B'], FIT['n_iter'], exchange, n_neg=3)
-        if rank == 0:
-            q.put(out)
-    finally:
-        dist.destroy_process_group()
+def _fit_job(rank, world, dev, loss, exchange):
+    params, users, items = _fit_problem()
+    return sc.sharded_fit_run(rank, world, params, users, items, loss, dev, sc.NumpyBackend(),
+                              FIT['seed'], FIT['B'], FIT['n_iter'], exchange, n_neg=3)
 
 
 @pytest.mark.parametrize('world,loss,exchange', [(2, 'bpr', 'a2a'), (3, 'pointwise', 'dense'),
@@ -162,17 +94,7 @@ def test_sharded_fit_is_the_single_process_fit(world, loss, exchange):
     stream (global shuffle, one randint per minibatch), so its trajectory is the
     single-process one; with 500 interactions in minibatches of 64 over 3 ranks some ranks
     get empty shares, which must not stall the collectives."""
-    import sharded_common as sc
-    ctx = mp.get_context('spawn')
-    q = ctx.Queue()
-    port = 33500 + (os.getpid() + world * 13) % 2000
-    procs = [ctx.Process(target=_fit_worker, args=(r, world, port, loss, exchange, q)) for r in range(world)]
-    for p in procs:
-        p.start()
-    got, losses, state = q.get(timeout=240)
-    for p in procs:
-        p.join(timeout=60)
-        assert p.exitcode == 0
+    got, losses, state = sc.run_world(_fit_job, world, (loss, exchange))[0]
     params, users, items = _fit_problem()
     n_neg = 3 if loss == 'adaptive_hinge' else 1
     epochs, rs = sc.reference_epochs(FIT['seed'], users, items, FIT['I'], FIT['B'], FIT['n_iter'], n_neg)
@@ -197,19 +119,10 @@ def test_shard_plan_ranges():
 BLOOM = (9, 120, 700, 64, 8, 128, 3, 3)         # seed, U, N ids, M hashed rows, D, B, steps, H
 
 
-def _bloom_worker(rank, world, port, loss, q):
-    import sharded_common as sc
-    os.environ['MASTER_ADDR'] = '127.0.0.1'
-    os.environ['MASTER_PORT'] = str(port)
-    dist.init_process_group('gloo', rank=rank, world_size=world)
-    try:
-        seed, U, N, M, D, B, steps, H = BLOOM
-        params, batches = sc.make_bloom_problem(seed, U, N, M, D, B, steps)
-        got, losses = sc.bloom_sharded_run(rank, world, params, batches, loss, 0.05, 'cpu', sc.NumpyBackend(), H)
-        if rank == 0:
-            q.put((got, losses))
-    finally:
-        dist.destroy_process_group()
+def _bloom_job(rank, world, dev, loss):
+    seed, U, N, M, D, B, steps, H = BLOOM
+    params, batches = sc.make_bloom_problem(seed, U, N, M, D, B, steps)
+    return sc.bloom_sharded_run(rank, world, params, batches, loss, 0.05, dev, sc.NumpyBackend(), H)
 
 
 @pytest.mark.parametrize('world,loss', [(2, 'bpr'), (3, 'pointwise'), (4, 'bpr')])
@@ -217,17 +130,7 @@ def test_sharded_bloom_step_matches_single_process(world, loss):
     """BASELINE config 4's partitioning (hashed item rows range-sharded, users owner-routed,
     id-space item bias replicated through all-gathered sparse updates) against the
     single-process float64 oracle of BilinearNet + BloomEmbedding."""
-    import sharded_common as sc
-    ctx = mp.get_context('spawn')
-    q = ctx.Queue()
-    port = 27500 + (os.getpid() + world * 11) % 2000
-    procs = [ctx.Process(target=_bloom_worker, args=(r, world, port, loss, q)) for r in range(world)]
-    for p in procs:
-        p.start()
-    got, losses = q.get(timeout=240)
-    for p in procs:
-        p.join(timeout=60)
-        assert p.exitcode == 0
+    got, losses = sc.run_world(_bloom_job, world, (loss,))[0]
     seed, U, N, M, D, B, steps, H = BLOOM
     params, batches = sc.make_bloom_problem(seed, U, N, M, D, B, steps)
     ref, ref_losses = sc.bloom_oracle_run(params, batches, loss, 0.05, H)

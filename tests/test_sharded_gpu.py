@@ -12,13 +12,13 @@ import sys
 import numpy as np
 import pytest
 import torch
-import torch.distributed as dist
-import torch.multiprocessing as mp
 
 from conftest import ROOT, assert_close
 
 sys.path.insert(0, os.path.join(ROOT, 'tests'))
 pytestmark = pytest.mark.gpu
+
+import sharded_common as sc            # noqa: E402
 
 SHAPE = (7, 2000, 500, 32, 1024, 3)     # seed, U, I, D, B, steps
 MF_JOBS = [('bpr', 'a2a'), ('pointwise', 'a2a'), ('bpr', 'dense')]
@@ -38,7 +38,6 @@ BLOOM = (9, 3000, 40000, 1500, 32, 2048, 3, 4)            # seed, U, N ids, M ha
 
 
 def _fit_problem():
-    import sharded_common as sc
     rs = np.random.RandomState(8)
     params, _ = sc.make_problem(6, FIT['U'], FIT['I'], FIT['D'], 8, 0)
     params = tuple(p * 0.3 for p in params)
@@ -49,7 +48,6 @@ def _adaptive_grad_job(rank, world, dev):
     """One ShardedMF.step_adaptive on the product kernels with the gradients tapped where
     the step hands them to the optimizer (user side: scores_backward; item side: the rows
     each owner receives)."""
-    import sharded_common as sc
     from spotlight_b200.sharded import GpuBackend, ShardedMF, ShardPlan, ShardState
 
     class Tap(GpuBackend):
@@ -85,45 +83,50 @@ def _adaptive_grad_job(rank, world, dev):
     return rec
 
 
-def _worker(rank, world, port, q):
-    import sharded_common as sc
+def _dense_stats_job(rank, world, dev):
+    """fit() on the dense exchange (B = 16384 covers the 800 items twice over, so 'auto' picks it
+    too), and one ShardedMF.step_dense on the same shards: the exchange stats of each."""
+    from spotlight_b200.interactions import Interactions
+    from spotlight_b200.sharded import GpuBackend, ShardedImplicitFactorizationModel, ShardedMF
+    params, users, items = _fit_problem()
+    model = ShardedImplicitFactorizationModel(FIT['U'], FIT['I'], rank, world, dev, loss='bpr',
+                                              embedding_dim=FIT['D'], n_iter=FIT['n_iter'], batch_size=FIT['B'],
+                                              random_state=np.random.RandomState(FIT['seed']), exchange='dense',
+                                              init=[torch.from_numpy(p) for p in params])
+    model.fit(Interactions(users, items, num_users=FIT['U'], num_items=FIT['I']))
+    one = ShardedMF(model.plan, model.state, rank, GpuBackend(dev))
+    empty = torch.zeros(0, dtype=torch.int64, device=dev)
+    one.step_dense(empty, empty, empty, 'bpr', FIT['B'])
+    return dict(model.mf.stats), dict(one.stats), model.plan.ichunk
+
+
+def _jobs(rank, world, dev):
     from spotlight_b200.sharded import GpuBackend
-    os.environ['MASTER_ADDR'] = '127.0.0.1'
-    os.environ['MASTER_PORT'] = str(port)
-    torch.cuda.set_device(rank)
-    dev = torch.device('cuda', rank)
-    dist.init_process_group('nccl', rank=rank, world_size=world, device_id=dev)
     res = {}
-    try:
-        for loss, exchange in MF_JOBS:
-            params, batches = sc.make_problem(*SHAPE)
-            got, losses, stats = sc.sharded_run(rank, world, params, batches, loss, 0.05, dev,
-                                                GpuBackend(dev), cache_capacity=min(2 * SHAPE[4], SHAPE[2]),
-                                                exchange=exchange)
-            res['mf', loss, exchange] = (got, losses)
-        for loss, net in SEQ_JOBS:
-            cnn = _CNN if net == 'cnn' else None
-            params, batches = sc.make_seq_problem(*SEQ_SHAPE[net], layers=2 if cnn else 0)
-            got, losses, stats = sc.seq_sharded_run(rank, world, params, batches, loss, 0.05, dev,
-                                                    GpuBackend(dev), cnn=cnn)
-            res['seq', loss, net] = (got, losses)
-        for loss, exchange in FIT_JOBS:
-            params, users, items = _fit_problem()
-            res['fit', loss, exchange] = sc.sharded_fit_run(rank, world, params, users, items, loss, dev,
-                                                           GpuBackend(dev), FIT['seed'], FIT['B'],
-                                                           FIT['n_iter'], exchange, n_neg=4)
-        seed, U, N, M, D, B, steps, H = BLOOM
-        params, batches = sc.make_bloom_problem(seed, U, N, M, D, B, steps)
-        for loss in ('bpr', 'hinge'):
-            res['bloom', loss] = sc.bloom_sharded_run(rank, world, params, batches, loss, 0.05, dev, GpuBackend(dev), H)
-        res['ada', rank] = _adaptive_grad_job(rank, world, dev)
-        torch.cuda.synchronize()
-        q.put((rank, res, None))
-    except Exception:                        # surface the traceback in the parent
-        import traceback
-        q.put((rank, None, traceback.format_exc()))
-    finally:
-        dist.destroy_process_group()
+    for loss, exchange in MF_JOBS:
+        params, batches = sc.make_problem(*SHAPE)
+        got, losses, stats = sc.sharded_run(rank, world, params, batches, loss, 0.05, dev,
+                                            GpuBackend(dev), cache_capacity=min(2 * SHAPE[4], SHAPE[2]),
+                                            exchange=exchange)
+        res['mf', loss, exchange] = (got, losses)
+    for loss, net in SEQ_JOBS:
+        cnn = _CNN if net == 'cnn' else None
+        params, batches = sc.make_seq_problem(*SEQ_SHAPE[net], layers=2 if cnn else 0)
+        got, losses, stats = sc.seq_sharded_run(rank, world, params, batches, loss, 0.05, dev,
+                                                GpuBackend(dev), cnn=cnn)
+        res['seq', loss, net] = (got, losses)
+    for loss, exchange in FIT_JOBS:
+        params, users, items = _fit_problem()
+        res['fit', loss, exchange] = sc.sharded_fit_run(rank, world, params, users, items, loss, dev,
+                                                       GpuBackend(dev), FIT['seed'], FIT['B'],
+                                                       FIT['n_iter'], exchange, n_neg=4)
+    seed, U, N, M, D, B, steps, H = BLOOM
+    params, batches = sc.make_bloom_problem(seed, U, N, M, D, B, steps)
+    for loss in ('bpr', 'hinge'):
+        res['bloom', loss] = sc.bloom_sharded_run(rank, world, params, batches, loss, 0.05, dev, GpuBackend(dev), H)
+    res['ada', rank] = _adaptive_grad_job(rank, world, dev)
+    res['dense_stats'] = _dense_stats_job(rank, world, dev)
+    return res
 
 
 _CACHE = {}
@@ -133,21 +136,7 @@ def _results(world):
     if torch.cuda.device_count() < world:
         pytest.skip('needs %d GPUs' % world)
     if world not in _CACHE:
-        ctx = mp.get_context('spawn')
-        q = ctx.Queue()
-        port = 29500 + (os.getpid() * 3 + world) % 2000
-        procs = [ctx.Process(target=_worker, args=(r, world, port, q)) for r in range(world)]
-        for p in procs:
-            p.start()
-        per_rank = {}
-        for _ in range(world):
-            rank, res, err = q.get(timeout=900)
-            assert err is None, 'rank %d failed:\n%s' % (rank, err)
-            per_rank[rank] = res
-        for p in procs:
-            p.join(timeout=120)
-            assert p.exitcode == 0
-        _CACHE[world] = per_rank
+        _CACHE[world] = sc.run_world(_jobs, world, backend='nccl', timeout=900)
     return _CACHE[world]
 
 
@@ -157,7 +146,6 @@ WORLDS = [1, 2]
 @pytest.mark.parametrize('world', WORLDS)
 @pytest.mark.parametrize('loss,exchange', MF_JOBS)
 def test_sharded_gpu_matches_oracle(world, loss, exchange):
-    import sharded_common as sc
     got, losses = _results(world)[0]['mf', loss, exchange]
     params, batches = sc.make_problem(*SHAPE)
     ref, ref_losses = sc.oracle_run(params, batches, loss, 0.05)
@@ -171,7 +159,6 @@ def test_sharded_gpu_matches_oracle(world, loss, exchange):
 @pytest.mark.parametrize('world', WORLDS)
 @pytest.mark.parametrize('loss,net', SEQ_JOBS)
 def test_sharded_sequence_gpu_matches_oracle(world, loss, net):
-    import sharded_common as sc
     got, losses = _results(world)[0]['seq', loss, net]
     cnn = _CNN if net == 'cnn' else None
     params, batches = sc.make_seq_problem(*SEQ_SHAPE[net], layers=2 if cnn else 0)
@@ -187,7 +174,6 @@ def test_sharded_adaptive_hinge_step_gradients(world):
     f scored with users[f // n], consumed as element (f // B, f % B)) against the float64
     oracle: loss and all four gradients at the north star's 1e-5.  No trajectory, so none of
     the chaos that limits the fit() comparison below."""
-    import sharded_common as sc
     from oracle import mf as omf
     res = _results(world)
     n = ADA['n']
@@ -220,7 +206,6 @@ def test_sharded_bloom_gpu_matches_oracle(world, loss):
     """BASELINE config 4's partitioning on the product kernels (hashed item table range-sharded and
     exchanged whole, fused hashed step with in-register murmur3, sparse bias updates) against the
     single-process float64 oracle of BilinearNet + BloomEmbedding."""
-    import sharded_common as sc
     got, losses = _results(world)[0]['bloom', loss]
     seed, U, N, M, D, B, steps, H = BLOOM
     params, batches = sc.make_bloom_problem(seed, U, N, M, D, B, steps)
@@ -298,3 +283,16 @@ def test_sharded_fit_equals_single_gpu_fit(world, loss, exchange):
             assert_close(a, b.reshape(a.shape), 5e-3, what=nm)   # Adagrad trajectory tolerance, as above
     assert np.array_equal(state[1], want[1]) and state[2] == want[2]
     assert len(losses) == FIT['n_iter'] and all(0.0 < v < 1.5 for v in losses)
+
+
+@pytest.mark.parametrize('world', WORLDS)
+def test_sharded_dense_epoch_counts_the_exchange(world):
+    """The dense-exchange epoch counts, on every rank and for every step, what ShardedMF.step_dense
+    counts: the whole padded item table (world * ichunk rows) requested, and the table, its bias and
+    their gradients moved as float32."""
+    steps = FIT['n_iter'] * -(-FIT['n'] // FIT['B'])
+    for r in range(world):
+        fit_stats, step_stats, chunk = _results(world)[r]['dense_stats']
+        assert step_stats == {'rows_requested': world * chunk,
+                              'bytes_a2a': 2 * (world * chunk * FIT['D'] + world * chunk) * 4}
+        assert fit_stats == {k: steps * v for k, v in step_stats.items()}

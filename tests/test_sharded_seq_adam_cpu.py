@@ -11,12 +11,12 @@ import sys
 import numpy as np
 import pytest
 import torch
-import torch.distributed as dist
 
 from conftest import ROOT, assert_close
 
 sys.path.insert(0, os.path.join(ROOT, 'tests'))
 
+import sharded_common as sc            # noqa: E402
 import test_sharded_seq_cpu as tsc     # noqa: E402
 from oracle.adam import LazyAdamTable  # noqa: E402
 
@@ -200,19 +200,11 @@ def _step_job(rank, world, net, loss, wd, I):
         mine = negs.reshape(n_neg, B, S)[:, a:c].reshape(-1, S)
         losses.append(float(model.step(torch.from_numpy(seqs[a:c].copy()), torch.from_numpy(mine.copy()), loss)))
     be.owner_adam_flush(st)
-    return tsc.gather_state(st, plan, I, world), losses, st.last.numpy().copy(), st.opt.steps_taken
+    return tsc.gather_state(st, plan, I), losses, st.last.numpy().copy(), st.opt.steps_taken
 
 
-def _step_worker(rank, world, port, q):
-    tsc._init(rank, world, port)
-    try:
-        res = {job: _step_job(rank, world, *job) for job in STEP_JOBS}
-        q.put((rank, res, None))
-    except Exception:
-        import traceback
-        q.put((rank, None, traceback.format_exc()))
-    finally:
-        dist.destroy_process_group()
+def _step_jobs(rank, world, dev):
+    return {job: _step_job(rank, world, *job) for job in STEP_JOBS}
 
 
 _CACHE = {}
@@ -220,7 +212,7 @@ _CACHE = {}
 
 def _step_results(world):
     if world not in _CACHE:
-        _CACHE[world] = tsc._run(_step_worker, world, (), 39500)
+        _CACHE[world] = sc.run_world(_step_jobs, world)
     return _CACHE[world]
 
 
@@ -288,17 +280,9 @@ def _fit_job(rank, world, rep, loss, splits):
     return params, model.epoch_losses, rs.get_state(), model.state.opt.steps_taken
 
 
-def _fit_worker(rank, world, port, q):
-    tsc._init(rank, world, port)
-    try:
-        res = {(rep, loss, splits): _fit_job(rank, world, rep, loss, splits)
-               for rep, loss in FIT_JOBS for splits in (1, 2)}
-        q.put((rank, res, None))
-    except Exception:
-        import traceback
-        q.put((rank, None, traceback.format_exc()))
-    finally:
-        dist.destroy_process_group()
+def _fit_jobs(rank, world, dev):
+    return {(rep, loss, splits): _fit_job(rank, world, rep, loss, splits)
+            for rep, loss in FIT_JOBS for splits in (1, 2)}
 
 
 _FIT = {}
@@ -306,7 +290,7 @@ _FIT = {}
 
 def _fit_results():
     if not _FIT:
-        _FIT.update(tsc._run(_fit_worker, 2, (), 41500))
+        _FIT.update(sc.run_world(_fit_jobs, 2))
     return _FIT
 
 

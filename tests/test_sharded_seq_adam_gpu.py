@@ -12,18 +12,17 @@ import sys
 import numpy as np
 import pytest
 import torch
-import torch.distributed as dist
-import torch.multiprocessing as mp
 
 from conftest import ROOT, assert_close
 
 sys.path.insert(0, os.path.join(ROOT, 'tests'))
 pytestmark = pytest.mark.gpu
 
+import sharded_common as sc                  # noqa: E402
 import test_sharded_seq_adam_cpu as tac      # noqa: E402
 import test_sharded_seq_gpu as tsg           # noqa: E402
 from oracle.adam import LazyAdamTable        # noqa: E402
-from test_sharded_seq_cpu import owner_case  # noqa: E402
+from test_sharded_seq_cpu import gather_state, owner_case  # noqa: E402
 
 DEV = torch.device('cuda', 0)
 T = 6                # the step the kernel tests take; rows start current for earlier steps
@@ -196,7 +195,6 @@ FIT_OPT = dict(lr=1e-2, weight_decay=1e-3)
 def _step_job(rank, world, dev, net, loss, wd):
     from spotlight_b200.optim import fused_adam
     from spotlight_b200.sharded import GpuBackend, SeqShardState, ShardedSeq, ShardPlan, _rank_slice
-    from test_sharded_seq_cpu import gather_state
     I, D, S = tac.STEP['I'], tac.STEP['D'], tac.STEP['S']
     n_neg = tac._n_neg(loss)
     E, bias, lstm, mix, convs = tac.step_params(net, I)
@@ -216,7 +214,7 @@ def _step_job(rank, world, dev, net, loss, wd):
         d = lambda x: torch.from_numpy(np.ascontiguousarray(x)).to(dev)      # noqa: E731
         losses.append(float(model.step(d(seqs[a:c]), d(mine), loss)))
     be.owner_adam_flush(st)
-    return gather_state(st, plan, I, world), losses, st.last.cpu().numpy(), st.opt.steps_taken
+    return gather_state(st, plan, I), losses, st.last.cpu().numpy(), st.opt.steps_taken
 
 
 def _fit_job(rank, world, dev, rep, loss):
@@ -235,26 +233,14 @@ def _fit_job(rank, world, dev, rep, loss):
     return sd, model.epoch_losses, rs.get_state(), (int(last.min()), int(last.max())), model.state.opt.steps_taken
 
 
-def _worker(rank, world, port, q):
-    os.environ['MASTER_ADDR'] = '127.0.0.1'
-    os.environ['MASTER_PORT'] = str(port)
-    torch.cuda.set_device(rank)
-    dev = torch.device('cuda', rank)
-    dist.init_process_group('nccl', rank=rank, world_size=world, device_id=dev)
+def _jobs(rank, world, dev):
     res = {}
-    try:
-        for job in STEP_JOBS:
-            res['step', job] = _step_job(rank, world, dev, *job)
-        if world == 1:
-            for rep, loss in FIT_JOBS:
-                res['fit', rep, loss] = _fit_job(rank, world, dev, rep, loss)
-        torch.cuda.synchronize()
-        q.put((rank, res, None))
-    except Exception:                        # surface the traceback in the parent
-        import traceback
-        q.put((rank, None, traceback.format_exc()))
-    finally:
-        dist.destroy_process_group()
+    for job in STEP_JOBS:
+        res['step', job] = _step_job(rank, world, dev, *job)
+    if world == 1:
+        for rep, loss in FIT_JOBS:
+            res['fit', rep, loss] = _fit_job(rank, world, dev, rep, loss)
+    return res
 
 
 _CACHE = {}
@@ -264,21 +250,7 @@ def _results(world):
     if torch.cuda.device_count() < world:
         pytest.skip('needs %d GPUs' % world)
     if world not in _CACHE:
-        ctx = mp.get_context('spawn')
-        q = ctx.Queue()
-        port = 33500 + (os.getpid() * 5 + world) % 2000
-        procs = [ctx.Process(target=_worker, args=(r, world, port, q)) for r in range(world)]
-        for p in procs:
-            p.start()
-        per_rank = {}
-        for _ in range(world):
-            rank, res, err = q.get(timeout=900)
-            assert err is None, 'rank %d failed:\n%s' % (rank, err)
-            per_rank[rank] = res
-        for p in procs:
-            p.join(timeout=120)
-            assert p.exitcode == 0
-        _CACHE[world] = per_rank
+        _CACHE[world] = sc.run_world(_jobs, world, backend='nccl', timeout=900)
     return _CACHE[world]
 
 

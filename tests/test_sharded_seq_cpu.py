@@ -9,8 +9,6 @@ import sys
 import numpy as np
 import pytest
 import torch
-import torch.distributed as dist
-import torch.multiprocessing as mp
 
 from conftest import ROOT, assert_close
 
@@ -124,39 +122,10 @@ def oracle_trajectory(params, batches, loss, lr, n_neg):
     return P, losses
 
 
-def gather_state(st, plan, I, world):
-    out = []
-    for shard in (st.Wi, st.bi.reshape(-1, 1)):
-        pad = shard.new_zeros((plan.ichunk,) + tuple(shard.shape[1:]))
-        pad[:shard.shape[0]] = shard
-        parts = [torch.empty_like(pad) for _ in range(world)]
-        dist.all_gather(parts, pad)
-        out.append(torch.cat(parts)[:I].cpu().numpy())
+def gather_state(st, plan, I):
+    """The full item table and bias of a SeqShardState, then its replicated parameters."""
+    out = [sc.gather_rows(st.Wi, plan.ichunk, I), sc.gather_rows(st.bi.reshape(-1, 1), plan.ichunk, I)]
     return out + [p.cpu().numpy() for p, _ in st.replicated()]
-
-
-def _init(rank, world, port):
-    os.environ['MASTER_ADDR'] = '127.0.0.1'
-    os.environ['MASTER_PORT'] = str(port)
-    dist.init_process_group('gloo', rank=rank, world_size=world)
-
-
-def _run(target, world, args, base):
-    ctx = mp.get_context('spawn')
-    q = ctx.Queue()
-    port = base + (os.getpid() * 7 + world) % 2000
-    procs = [ctx.Process(target=target, args=(r, world, port, q) + tuple(args)) for r in range(world)]
-    for p in procs:
-        p.start()
-    res = {}
-    for _ in range(world):
-        rank, out, err = q.get(timeout=300)
-        assert err is None, 'rank %d failed:\n%s' % (rank, err)
-        res[rank] = out
-    for p in procs:
-        p.join(timeout=60)
-        assert p.exitcode == 0
-    return res
 
 
 # ------------------------------------------------------------------ ShardedSeq steps
@@ -166,31 +135,23 @@ STEP_CASES = [(2, 'lstm', 'bpr', 1), (3, 'lstm', 'pointwise', 1), (2, 'mixture',
               (3, 'mixture', 'bpr', 1), (2, 'pool', 'adaptive_hinge', 3), (3, 'lstm', 'adaptive_hinge', 2)]
 
 
-def _step_worker(rank, world, port, q, net, loss, n_neg):
-    _init(rank, world, port)
-    try:
-        from spotlight_b200.sharded import SeqShardState, ShardedSeq, ShardPlan
-        E, bias, lstm, mix = make_params(STEP['seed'], STEP['I'], STEP['D'], net)
-        batches = make_batches(STEP['seed'] + 2, STEP['I'], STEP['B'], STEP['S'], STEP['steps'], n_neg)
-        t = lambda d: None if d is None else {k: (torch.from_numpy(v) if isinstance(v, np.ndarray) else v)   # noqa: E731
-                                             for k, v in d.items()}
-        plan = ShardPlan(1, STEP['I'], world)
-        st = SeqShardState(plan, rank, STEP['D'], 'cpu', lr=0.05, init=(torch.from_numpy(E), torch.from_numpy(bias)),
-                           lstm=t(lstm), mixture=t(mix))
-        model = ShardedSeq(plan, st, rank, SeqBackend(), n_neg=n_neg)
-        from spotlight_b200.sharded import _rank_slice
-        losses = []
-        for seqs, negs in batches:
-            B, S = seqs.shape
-            a, c = _rank_slice(B, rank, world)
-            mine = negs.reshape(n_neg, B, S)[:, a:c].reshape(-1, S)
-            losses.append(float(model.step(torch.from_numpy(seqs[a:c].copy()), torch.from_numpy(mine.copy()), loss)))
-        q.put((rank, (gather_state(st, plan, STEP['I'], world), losses), None))
-    except Exception:
-        import traceback
-        q.put((rank, None, traceback.format_exc()))
-    finally:
-        dist.destroy_process_group()
+def _step_job(rank, world, dev, net, loss, n_neg):
+    from spotlight_b200.sharded import SeqShardState, ShardedSeq, ShardPlan, _rank_slice
+    E, bias, lstm, mix = make_params(STEP['seed'], STEP['I'], STEP['D'], net)
+    batches = make_batches(STEP['seed'] + 2, STEP['I'], STEP['B'], STEP['S'], STEP['steps'], n_neg)
+    t = lambda d: None if d is None else {k: (torch.from_numpy(v) if isinstance(v, np.ndarray) else v)   # noqa: E731
+                                         for k, v in d.items()}
+    plan = ShardPlan(1, STEP['I'], world)
+    st = SeqShardState(plan, rank, STEP['D'], dev, lr=0.05, init=(torch.from_numpy(E), torch.from_numpy(bias)),
+                       lstm=t(lstm), mixture=t(mix))
+    model = ShardedSeq(plan, st, rank, SeqBackend(), n_neg=n_neg)
+    losses = []
+    for seqs, negs in batches:
+        B, S = seqs.shape
+        a, c = _rank_slice(B, rank, world)
+        mine = negs.reshape(n_neg, B, S)[:, a:c].reshape(-1, S)
+        losses.append(float(model.step(torch.from_numpy(seqs[a:c].copy()), torch.from_numpy(mine.copy()), loss)))
+    return gather_state(st, plan, STEP['I']), losses
 
 
 @pytest.mark.parametrize('world,net,loss,n_neg', STEP_CASES)
@@ -198,7 +159,7 @@ def test_sharded_seq_step_matches_single_process(world, net, loss, n_neg):
     """LSTMNet, MixtureLSTMNet (M = 2) and adaptive hinge: the sharded steps (each rank a
     contiguous slice of every minibatch, its negatives rows q*B + b of the minibatch's block,
     replicated LSTM / projection weights all-reduced) reproduce the whole-minibatch oracle."""
-    res = _run(_step_worker, world, (net, loss, n_neg), 35500)
+    res = sc.run_world(_step_job, world, (net, loss, n_neg))
     got, losses = res[0]
     params = make_params(STEP['seed'], STEP['I'], STEP['D'], net)
     batches = make_batches(STEP['seed'] + 2, STEP['I'], STEP['B'], STEP['S'], STEP['steps'], n_neg)
@@ -227,25 +188,18 @@ def _fit_data():
     return seqs
 
 
-def _fit_worker(rank, world, port, q, rep, loss):
-    _init(rank, world, port)
-    try:
-        from spotlight_b200.interactions import SequenceInteractions
-        from spotlight_b200.sharded import ShardedImplicitSequenceModel
-        rs = np.random.RandomState(FIT['seed'])
-        model = ShardedImplicitSequenceModel(FIT['I'], rank, world, 'cpu', loss=loss, representation=rep,
-                                             embedding_dim=FIT['D'], n_iter=FIT['n_iter'], batch_size=FIT['B'],
-                                             learning_rate=0.05, random_state=rs, num_negative_samples=3,
-                                             backend=SeqBackend())
-        model.fit(SequenceInteractions(_fit_data(), num_items=FIT['I']))
-        net = model.gathered_net()
-        params = [p.detach().numpy().copy() for p in net.parameters()]
-        q.put((rank, (params, model.epoch_losses, rs.get_state()), None))
-    except Exception:
-        import traceback
-        q.put((rank, None, traceback.format_exc()))
-    finally:
-        dist.destroy_process_group()
+def _fit_job(rank, world, dev, rep, loss):
+    from spotlight_b200.interactions import SequenceInteractions
+    from spotlight_b200.sharded import ShardedImplicitSequenceModel
+    rs = np.random.RandomState(FIT['seed'])
+    model = ShardedImplicitSequenceModel(FIT['I'], rank, world, dev, loss=loss, representation=rep,
+                                         embedding_dim=FIT['D'], n_iter=FIT['n_iter'], batch_size=FIT['B'],
+                                         learning_rate=0.05, random_state=rs, num_negative_samples=3,
+                                         backend=SeqBackend())
+    model.fit(SequenceInteractions(_fit_data(), num_items=FIT['I']))
+    net = model.gathered_net()
+    params = [p.detach().numpy().copy() for p in net.parameters()]
+    return params, model.epoch_losses, rs.get_state()
 
 
 def _reference_fit(rep, loss, n_neg, store=None):
@@ -308,7 +262,7 @@ def test_sharded_sequence_fit_is_the_single_process_fit(world, rep, loss):
     replay: epoch losses, item table, bias and replicated parameters, and every rank's final
     RandomState."""
     n_neg = 3 if loss == 'adaptive_hinge' else 1
-    res = _run(_fit_worker, world, (rep, loss), 37500)
+    res = sc.run_world(_fit_job, world, (rep, loss))
     # float32 parameter storage, as the model keeps: the hinge's kink and its argmax over negatives
     # turn the 1e-8 gap between float64 and float32 storage into different active terms within an
     # epoch, so a float64-stored replay is a different (equally valid) trajectory

@@ -13,16 +13,15 @@ import types
 import numpy as np
 import pytest
 import torch
-import torch.distributed as dist
-import torch.multiprocessing as mp
 
 from conftest import ROOT, assert_close
 
 sys.path.insert(0, os.path.join(ROOT, 'tests'))
 pytestmark = pytest.mark.gpu
 
-from test_sharded_seq_cpu import (make_batches, make_params, oracle_trajectory,  # noqa: E402
-                                  owner_case, owner_update_reference)
+import sharded_common as sc                                                       # noqa: E402
+from test_sharded_seq_cpu import (gather_state, make_batches, make_params,          # noqa: E402
+                                  oracle_trajectory, owner_case, owner_update_reference)
 
 # ------------------------------------------------------------------ owner update kernel
 
@@ -43,8 +42,7 @@ def _run_owner(case, dev):
 
 
 def _hot_case(seed, rows, D):
-    """One row requested at 300 positions (more than any lane group's in-register sort holds), as
-    a fixed-slot exchange's unused slots all map to one row."""
+    """One row requested at 300 positions (more than any lane group's in-register sort holds)."""
     ids, g_rows, g_bias, W, S, b, sb = owner_case(seed, rows, D)
     rs = np.random.RandomState(seed + 1)
     hot = np.full(300, 7, dtype=np.int64)
@@ -140,7 +138,6 @@ def _fit_data():
 
 def _step_job(rank, world, dev, net, loss):
     from spotlight_b200.sharded import GpuBackend, SeqShardState, ShardedSeq, ShardPlan, _rank_slice
-    from test_sharded_seq_cpu import gather_state
     E, bias, lstm, mix = make_params(STEP['seed'], STEP['I'], STEP['D'], net)
     batches = make_batches(STEP['seed'] + 2, STEP['I'], STEP['B'], STEP['S'], STEP['steps'], 1)
     t = lambda d: None if d is None else {k: (torch.from_numpy(v) if isinstance(v, np.ndarray) else v)   # noqa: E731
@@ -154,7 +151,7 @@ def _step_job(rank, world, dev, net, loss):
         a, c = _rank_slice(seqs.shape[0], rank, world)
         d = lambda x: torch.from_numpy(np.ascontiguousarray(x[a:c])).to(dev)      # noqa: E731
         losses.append(float(model.step(d(seqs), d(negs), loss)))
-    return gather_state(st, plan, STEP['I'], world), losses
+    return gather_state(st, plan, STEP['I']), losses
 
 
 def _fit_job(rank, world, dev, rep, loss):
@@ -170,26 +167,14 @@ def _fit_job(rank, world, dev, rep, loss):
     return sd, model.epoch_losses, rs.get_state()
 
 
-def _worker(rank, world, port, q):
-    os.environ['MASTER_ADDR'] = '127.0.0.1'
-    os.environ['MASTER_PORT'] = str(port)
-    torch.cuda.set_device(rank)
-    dev = torch.device('cuda', rank)
-    dist.init_process_group('nccl', rank=rank, world_size=world, device_id=dev)
+def _jobs(rank, world, dev):
     res = {}
-    try:
-        for net, loss in STEP_JOBS:
-            res['step', net, loss] = _step_job(rank, world, dev, net, loss)
-        if world == 1:
-            for rep, loss in FIT_JOBS:
-                res['fit', rep, loss] = _fit_job(rank, world, dev, rep, loss)
-        torch.cuda.synchronize()
-        q.put((rank, res, None))
-    except Exception:                        # surface the traceback in the parent
-        import traceback
-        q.put((rank, None, traceback.format_exc()))
-    finally:
-        dist.destroy_process_group()
+    for net, loss in STEP_JOBS:
+        res['step', net, loss] = _step_job(rank, world, dev, net, loss)
+    if world == 1:
+        for rep, loss in FIT_JOBS:
+            res['fit', rep, loss] = _fit_job(rank, world, dev, rep, loss)
+    return res
 
 
 _CACHE = {}
@@ -199,21 +184,7 @@ def _results(world):
     if torch.cuda.device_count() < world:
         pytest.skip('needs %d GPUs' % world)
     if world not in _CACHE:
-        ctx = mp.get_context('spawn')
-        q = ctx.Queue()
-        port = 31500 + (os.getpid() * 5 + world) % 2000
-        procs = [ctx.Process(target=_worker, args=(r, world, port, q)) for r in range(world)]
-        for p in procs:
-            p.start()
-        per_rank = {}
-        for _ in range(world):
-            rank, res, err = q.get(timeout=900)
-            assert err is None, 'rank %d failed:\n%s' % (rank, err)
-            per_rank[rank] = res
-        for p in procs:
-            p.join(timeout=120)
-            assert p.exitcode == 0
-        _CACHE[world] = per_rank
+        _CACHE[world] = sc.run_world(_jobs, world, backend='nccl', timeout=900)
     return _CACHE[world]
 
 
