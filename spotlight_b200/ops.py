@@ -79,10 +79,17 @@ def workspace(kind: str, nbytes: int, device) -> Tensor:
     return ws
 
 
+def workspace_error_word(ws: Tensor) -> Tensor:
+    """The device-side id-range error word of an MF or row-bucketing workspace (int32 word 4 of
+    the flags the library carves first), as a one-element view: nonzero once a kernel met an id
+    outside its table."""
+    return ws[:32].view(torch.int32)[4:5]
+
+
 def workspace_error_flag(ws: Tensor) -> int:
-    """Device-side id-range error flag of an MF workspace (int32 word 4); reading clears
+    """Device-side id-range error flag of an MF workspace (workspace_error_word); reading clears
     it, so one bad batch does not poison later calls that share the cached workspace."""
-    word = ws[:32].view(torch.int32)[4:5]
+    word = workspace_error_word(ws)
     flag = int(word.item())
     if flag:
         word.zero_()

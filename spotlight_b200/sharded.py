@@ -68,19 +68,26 @@ class GpuBackend(object):
         self.device = torch.device(device)
 
     def unique_bucket(self, ids, rows, chunk, nparts):
-        """distinct ids ascending, inverse map, and per-owner boundaries (host list)."""
+        """distinct ids ascending, inverse map, and per-owner boundaries (host list).  An id
+        outside [0, rows) raises ValueError (the kernels would count and train it as row 0)."""
         lib = _lib.load()
         ids = ids.contiguous()
         n = ids.numel()
         uniq = torch.empty(min(n, rows), dtype=torch.int64, device=ids.device)
         inverse = torch.empty(n, dtype=torch.int64, device=ids.device)
-        counts = torch.empty(nparts + 2, dtype=torch.int64, device=ids.device)
+        # nparts + 1 owner boundaries, the distinct count, then the workspace's id-range error word
+        counts = torch.empty(nparts + 3, dtype=torch.int64, device=ids.device)
         ws = ops.workspace('uq%d' % rows, lib.slb_unique_workspace_bytes(n, rows), ids.device)
         rc = lib.slb_unique_bucket(ops._ptr(ids), n, rows, chunk, nparts, ops._ptr(uniq),
                                    ops._ptr(inverse), ops._ptr(counts), ops._ptr(ws), ws.numel(),
                                    ops._stream())
         _lib.check(rc, 'unique_bucket')
+        err = ops.workspace_error_word(ws)
+        counts[nparts + 2:].copy_(err)
         host = counts.tolist()                       # the step's one bucketing sync
+        if host[nparts + 2]:
+            err.zero_()                              # the cached workspace serves the next call clean
+            raise ValueError('unique_bucket: an id outside [0, %d) reached the row exchange' % rows)
         return uniq[:host[nparts + 1]], inverse, host[:nparts + 1]
 
     def gather(self, W, b, local_ids):

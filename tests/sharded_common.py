@@ -230,18 +230,128 @@ def make_problem(seed, U, I, D, B, steps, n_neg=1):
     return (Wu, Wi, bu, bi), batches
 
 
-def oracle_run(params, batches, loss, lr, eps=1e-10, n_neg=1):
-    """Single-process reference: full-batch oracle step + dense Adagrad (float64)."""
+def make_margin_params(seed, U, I, D):
+    """(Wu, Wi, bu, bi) whose hinge margins stay far from the kink: small embeddings (dot products
+    of a few hundredths) and item biases on levels 1.5 apart, so that neg - pos + 1 sits near
+    1 + {0, +-1.5, +-3} and a step or a few of training cannot carry it to 0."""
+    rs = np.random.RandomState(seed)
+    Wu = (rs.randn(U, D) * 0.05).astype(np.float32)
+    Wi = (rs.randn(I, D) * 0.05).astype(np.float32)
+    bu = (rs.randn(U, 1) * 0.1).astype(np.float32)
+    bi = (1.5 * rs.randint(0, 3, (I, 1)) + rs.randn(I, 1) * 0.02).astype(np.float32)
+    return Wu, Wi, bu, bi
+
+
+def accumulator_scales(B):
+    """Squared typical gradient elements of (Wu, Wi, bu, bi) at make_margin_params' scale for
+    one hit in a minibatch of B: score gradients of about 0.2 / B, times a 0.05 row element for
+    the embeddings."""
+    return [(0.01 / B) ** 2, (0.01 / B) ** 2, (0.2 / B) ** 2, (0.2 / B) ** 2]
+
+
+def hinge_margin(r):
+    """The smallest |neg - pos + 1| of one oracle step: how close the hinge came to its kink."""
+    return float(np.abs(r['neg'] - r['pos'] + 1.0).min())
+
+
+def oracle_run(params, batches, loss, lr, eps=1e-10, n_neg=1, S0=None, each=None):
+    """Single-process reference: full-batch oracle step + dense Adagrad (float64).
+
+    ``S0``: initial Adagrad accumulators of (Wu, Wi, bu, bi) instead of zeros; then the final
+    accumulators are returned as a third value.  ``each(r)`` sees every step's oracle result."""
     P = [p.astype(np.float64) for p in params]
-    S = [np.zeros_like(p) for p in P]
+    S = [np.zeros_like(p) for p in P] if S0 is None else [s.astype(np.float64).reshape(p.shape)
+                                                          for s, p in zip(S0, P)]
     losses = []
     for users, items, negs in batches:
         r = omf.mf_step(P[0], P[1], P[2], P[3], users, items, negs, loss, n_neg, np.float64)
         losses.append(float(r['loss']))
+        if each is not None:
+            each(r)
         for k, g in enumerate((r['dWu'], r['dWi'], r['dbu'], r['dbi'])):
             S[k] += g * g
             P[k] -= lr * g / (np.sqrt(S[k]) + eps)
-    return P, losses
+        del r
+    return (P, losses) if S0 is None else (P, losses, S)
+
+
+def seeded_accumulators(seed, params, scales):
+    """Positive Adagrad accumulators for (Wu, Wi, bu, bi): ``scales[k]`` times U[0.5, 1.5], as
+    float32.  From a positive start every update is -lr g / sqrt(S0 + g^2), smooth in g, where
+    the zero start's first step is lr sign(g) whatever g's magnitude."""
+    rs = np.random.RandomState(seed)
+    return [(s * rs.uniform(0.5, 1.5, p.shape)).astype(np.float32) for p, s in zip(params, scales)]
+
+
+def scale_hot_row(S0, table, row, hits):
+    """Seeds the accumulators of a row that a minibatch hits ``hits`` times (of embedding table
+    ``table`` = 0 for users, 1 for items, and of its bias) at its own gradient scale: its elements
+    sum that many terms of random sign.  At the one-hit scale the elements of such a row that
+    happen to sum near zero sit in Adagrad's linear regime with a tiny sqrt(S0), which multiplies
+    the float32 rounding of their long sums far past that of every other row."""
+    S0[table][row] *= hits
+    S0[table + 2][row] *= hits
+
+
+def seed_accumulators(st, S0, pad=1.0):
+    """Writes this rank's slices of the full-table accumulators ``S0`` = (Wu, Wi, bu, bi) into a
+    ShardState; the padded item rows past the table's end get ``pad``."""
+    n = st.ihi - st.ilo
+    t = lambda x: torch.from_numpy(np.ascontiguousarray(x)).to(st.sWu.device)      # noqa: E731
+    st.sWu.copy_(t(S0[0][st.ulo:st.uhi]))
+    st.sbu.copy_(t(S0[2].reshape(-1)[st.ulo:st.uhi]))
+    st.sWi.fill_(pad)
+    st.sbi.fill_(pad)
+    st.sWi[:n] = t(S0[1][st.ilo:st.ihi])
+    st.sbi[:n] = t(S0[3].reshape(-1)[st.ilo:st.ihi])
+
+
+def gather_accumulators(st, plan, U, I):
+    """The full sWu, sWi, sbu and sbi (biases as columns) of a ShardState on every rank."""
+    return [gather_rows(shard, chunk, n) for shard, n, chunk in
+            ((st.sWu, U, plan.uchunk), (st.sWi, I, plan.ichunk),
+             (st.sbu.reshape(-1, 1), U, plan.uchunk), (st.sbi.reshape(-1, 1), I, plan.ichunk))]
+
+
+def padded_rows(st):
+    """The padded item rows of this rank's shard (past the table's end): W, S, b, sb as NumPy."""
+    n = st.ihi - st.ilo
+    return [x[n:].cpu().numpy() for x in (st.Wi, st.sWi, st.bi, st.sbi)]
+
+
+def worst_change(got, ref, start):
+    """(index, start, got's change, the oracle's change) of the element where they differ most."""
+    start = np.asarray(start, dtype=np.float64).reshape(np.shape(ref))
+    d_got = np.asarray(got, dtype=np.float64).reshape(np.shape(ref)) - start
+    d_ref = np.asarray(ref, dtype=np.float64) - start
+    k = np.unravel_index(np.argmax(np.abs(d_got - d_ref)), d_ref.shape)
+    return tuple(int(x) for x in k), float(start[k]), float(d_got[k]), float(d_ref[k])
+
+
+def change_error(got, ref, start, scale=None):
+    """max |(got - start) - (ref - start)| / scale: a table's change against the oracle's, by
+    default relative to the oracle's largest change."""
+    start = np.asarray(start, dtype=np.float64).reshape(np.shape(ref))
+    d_got = np.asarray(got, dtype=np.float64).reshape(np.shape(ref)) - start
+    d_ref = np.asarray(ref, dtype=np.float64) - start
+    if scale is None:
+        scale = np.abs(d_ref).max()
+        assert scale > 0, 'the oracle moved nothing'
+    return float(np.abs(d_got - d_ref).max() / scale)
+
+
+TABLE_NAMES = ('Wu', 'Wi', 'bu', 'bi', 'sWu', 'sWi', 'sbu', 'sbi')
+
+
+def change_errors(got, ref, start, loss, lr):
+    """change_error of (Wu, Wi, bu, bi) and their accumulators, by name.  Under bpr and hinge the
+    user-bias gradient gp + gn is zero in exact arithmetic, so the oracle moves bu and sbu by
+    summation residues only: those two are held relative to one Adagrad step (lr) and to their
+    largest starting accumulator instead -- a real gradient there moves them by that much."""
+    scales = {}
+    if loss in ('bpr', 'hinge'):
+        scales = {'bu': lr, 'sbu': float(np.abs(start[6]).max())}
+    return {nm: change_error(a, b, s, scales.get(nm)) for a, b, s, nm in zip(got, ref, start, TABLE_NAMES)}
 
 
 def sharded_run(rank, world, params, batches, loss, lr, device, backend, cache_capacity=None,
@@ -344,7 +454,10 @@ def gather_tables(st, plan, U, I):
 
 
 def sharded_fit_run(rank, world, params, users, items, loss, device, backend, seed, B, n_iter, exchange,
-                    n_neg=5):
+                    n_neg=5, S0=None):
+    """fit() on this rank; returns (all-gathered full tables, epoch losses, final RandomState).
+    With ``S0`` (seed_accumulators) also a fourth value: (all-gathered accumulators, this rank's
+    padded item rows)."""
     from spotlight_b200.interactions import Interactions
     from spotlight_b200.sharded import ShardedImplicitFactorizationModel
     U, D = params[0].shape
@@ -355,8 +468,13 @@ def sharded_fit_run(rank, world, params, users, items, loss, device, backend, se
                                               learning_rate=0.05, random_state=rs, exchange=exchange,
                                               init=[torch.from_numpy(p) for p in params],
                                               num_negative_samples=n_neg)
+    if S0 is not None:
+        seed_accumulators(model.state, S0)
     model.fit(Interactions(users, items, num_users=U, num_items=I))
-    return gather_tables(model.state, model.plan, U, I), model.epoch_losses, rs.get_state()
+    out = gather_tables(model.state, model.plan, U, I), model.epoch_losses, rs.get_state()
+    if S0 is None:
+        return out
+    return out + ((gather_accumulators(model.state, model.plan, U, I), padded_rows(model.state)),)
 
 
 # ---------------------------------------------------------------- hashed item table (config 4)

@@ -108,6 +108,55 @@ def test_sharded_fit_is_the_single_process_fit(world, loss, exchange):
     assert np.array_equal(state[1], want[1]) and state[2] == want[2]      # stream position too
 
 
+SEEDED = dict(seed=23, U=90, I=37, D=8, n=500, B=64, n_iter=2)
+
+
+def _seeded_problem(users_in):
+    p = SEEDED
+    params = sc.make_margin_params(6, p['U'], p['I'], p['D'])
+    rs = np.random.RandomState(12)
+    users = rs.randint(0, users_in, p['n']).astype(np.int32)
+    items = rs.randint(0, p['I'], p['n']).astype(np.int32)
+    S0 = sc.seeded_accumulators(7, params, sc.accumulator_scales(p['B']))
+    return params, users, items, S0
+
+
+def _seeded_fit_job(rank, world, dev, loss, users_in):
+    p = SEEDED
+    params, users, items, S0 = _seeded_problem(users_in)
+    return sc.sharded_fit_run(rank, world, params, users, items, loss, dev, sc.NumpyBackend(), p['seed'], p['B'],
+                              p['n_iter'], 'dense', S0=S0)
+
+
+@pytest.mark.parametrize('loss,users_in', [('bpr', SEEDED['U']), ('hinge', SEEDED['U']), ('pointwise', 40)])
+def test_seeded_accumulator_replay_is_the_sharded_fit(loss, users_in):
+    """The float64 replay the GPU tests hold the dense-exchange fit() to -- oracle_run from seeded
+    accumulators over reference_epochs' minibatches -- is the sharded fit() of the NumPy backend
+    at world 2 with I odd: the changes of all four tables and their accumulators, relative to the
+    largest change, the epoch losses and the final RandomState agree; the padded row of the last
+    item shard keeps its zeros and its accumulator bit for bit.  users_in = 40 puts every user in
+    rank 0's range, so rank 1 serves item rows with no members of its own."""
+    p = SEEDED
+    res = sc.run_world(_seeded_fit_job, 2, (loss, users_in))
+    got, losses, state, (acc, _) = res[0]
+    params, users, items, S0 = _seeded_problem(users_in)
+    epochs, rs = sc.reference_epochs(p['seed'], users, items, p['I'], p['B'], p['n_iter'])
+    margins = []
+    ref, ref_losses, ref_acc = sc.oracle_run(params, [b for e in epochs for b in e], loss, 0.05, S0=S0,
+                                             each=lambda r: margins.append(sc.hinge_margin(r)))
+    if loss == 'hinge':
+        assert min(margins) > 1e-4
+    per_epoch = np.array(ref_losses).reshape(p['n_iter'], -1).mean(axis=1)
+    assert_close(np.array(losses), per_epoch, 1e-5, what='epoch losses')
+    for nm, e in sc.change_errors(got + acc, ref + ref_acc, list(params) + S0, loss, 0.05).items():
+        assert e <= 1e-5, (nm, e)
+    want = rs.get_state()
+    assert np.array_equal(state[1], want[1]) and state[2] == want[2]
+    W, S, b, sb = res[1][3][1]                               # rank 1: 19 rows for 18 items
+    assert W.shape[0] == 1 and not W.any() and not b.any()
+    assert np.all(S == 1.0) and np.all(sb == 1.0)
+
+
 def test_shard_plan_ranges():
     from spotlight_b200.sharded import ShardPlan
     plan = ShardPlan(10, 7, 4)

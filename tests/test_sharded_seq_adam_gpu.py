@@ -33,12 +33,16 @@ T = 6                # the step the kernel tests take; rows start current for ea
 def _kernel_case(kind, D, seed=7, rows=300):
     """Request lists of four peers (one empty) concatenated in rank order, so rows repeat across
     requesters, with Adam state from earlier steps and rows current for different steps.
-    'hot': one row at 300 positions (past any lane group's in-register sort); 'zero': rows whose
-    every received gradient row and bias is zero."""
-    ids, g_rows, g_bias, W, _, b, _ = owner_case(seed, rows, D, peers=(90, 0, 140, 50), padding=3)
+    'hot': one row at 300 positions (past any lane group's in-register sort); 'tiles': the same over
+    a row space of several 4096-row scan tiles, the hot row just past a tile edge; 'zero': rows
+    whose every received gradient row and bias is zero."""
+    peers, hot_row = (90, 0, 140, 50), 7
+    if kind == 'tiles':
+        rows, peers, hot_row = 3 * 4096 + 17, (900, 0, 1400, 500), 4096
+    ids, g_rows, g_bias, W, _, b, _ = owner_case(seed, rows, D, peers=peers, padding=3)
     rs = np.random.RandomState(seed + 1)
-    if kind == 'hot':
-        ids = np.concatenate([ids, np.full(300, 7, dtype=np.int64)])
+    if kind in ('hot', 'tiles'):
+        ids = np.concatenate([ids, np.full(300, hot_row, dtype=np.int64)])
         g_rows = np.concatenate([g_rows, rs.randn(300, D).astype(np.float32)])
         g_bias = np.concatenate([g_bias, rs.randn(300).astype(np.float32)])
     if kind == 'zero':
@@ -104,7 +108,7 @@ NAMES = ('W', 'exp_avg', 'exp_avg_sq', 'bias', 'bias exp_avg', 'bias exp_avg_sq'
 
 
 @pytest.mark.parametrize('wd', [0.0, 1e-2])
-@pytest.mark.parametrize('kind', ['peers', 'hot', 'zero'])
+@pytest.mark.parametrize('kind', ['peers', 'hot', 'zero', 'tiles'])
 @pytest.mark.parametrize('D', [3, 16, 128, 256])
 def test_owner_adam_kernels_match_lazy_adam(D, kind, wd):
     """Catch-up then step T on every distinct requested row (rank-order sums of duplicates across

@@ -41,11 +41,14 @@ def _run_owner(case, dev):
     return [x.cpu().numpy() for x in (st.Wi, st.sWi, st.bi, st.sbi)]
 
 
-def _hot_case(seed, rows, D):
+TILES = 3 * 4096 + 17           # rows spanning several of segindex.cuh's 4096-row scan tiles
+
+
+def _hot_case(seed, rows, D, hot_row=7, peers=(9, 0, 14, 5)):
     """One row requested at 300 positions (more than any lane group's in-register sort holds)."""
-    ids, g_rows, g_bias, W, S, b, sb = owner_case(seed, rows, D)
+    ids, g_rows, g_bias, W, S, b, sb = owner_case(seed, rows, D, peers=peers)
     rs = np.random.RandomState(seed + 1)
-    hot = np.full(300, 7, dtype=np.int64)
+    hot = np.full(300, hot_row, dtype=np.int64)
     ids = np.concatenate([ids, hot])
     g_rows = np.concatenate([g_rows, rs.randn(300, D).astype(np.float32)])
     g_bias = np.concatenate([g_bias, rs.randn(300).astype(np.float32)])
@@ -53,15 +56,18 @@ def _hot_case(seed, rows, D):
 
 
 @pytest.mark.parametrize('D', [1, 3, 4, 64, 128, 512])
-@pytest.mark.parametrize('kind', ['peers', 'padding', 'hot'])
+@pytest.mark.parametrize('kind', ['peers', 'padding', 'hot', 'tiles'])
 def test_owner_update_kernel_matches_numpy(D, kind):
-    """Duplicate ids across peers, an empty peer, -1 padding slots or a hot row: each distinct row
-    takes one Adagrad step on the rank-order sum of its contributions; untouched rows and their
-    states are unchanged bit for bit; two runs are bit-identical."""
+    """Duplicate ids across peers, an empty peer, -1 padding slots or a hot row ('tiles': over a
+    row space of several scan tiles, the hot row just past a tile edge): each distinct row takes one
+    Adagrad step on the rank-order sum of its contributions; untouched rows and their states are
+    unchanged bit for bit; two runs are bit-identical."""
     dev = torch.device('cuda', 0)
-    rows = 300
+    rows = TILES if kind == 'tiles' else 300
     if kind == 'hot':
         case = _hot_case(5, rows, D)
+    elif kind == 'tiles':
+        case = _hot_case(5, rows, D, hot_row=4096, peers=(900, 0, 1400, 500))
     else:
         case = owner_case(5, rows, D, peers=(90, 0, 140, 50), padding=5 if kind == 'padding' else 0)
     ids, g_rows, g_bias, W, S, b, sb = case
