@@ -210,6 +210,15 @@ def _row_sums(shape, rows, vals):
     return out
 
 
+def touched(n, rows, g):
+    """Rows (of a table of ``n``) that carry a gradient term with g != 0: the rows the compact
+    segment list holds (mf_fill_kernel places a term only when its score gradient is non-zero).
+    ``rows`` / ``g``: the terms' row ids and score gradients."""
+    out = np.zeros(n, dtype=bool)
+    out[np.asarray(rows)[np.asarray(g) != 0]] = True
+    return out
+
+
 def fused_step(params, users, items, negs, loss, opt, lr, weight_decay=0.0, eps=1e-10, states=None,
                norm=None, mutate=(), cap=128):
     """One in-place float64 step of the planned route (pointwise / bpr / hinge) with the fused
@@ -261,8 +270,7 @@ def fused_step(params, users, items, negs, loss, opt, lr, weight_decay=0.0, eps=
     dWu = _row_sums(Wu.shape, users[ku], gp[ku, None] * Wi[items[ku]] + gn[ku, None] * Wi[negs[ku]])
     gbu = gp if 'user_bias_no_gn' in mutate else gp + gn
     dbu = _row_sums(bu.shape, users[ku], gbu[ku])
-    tu = np.zeros(Wu.shape[0], dtype=bool)
-    tu[users[((gp != 0) | (gn != 0)) & keep_u]] = True
+    tu = touched(Wu.shape[0], t_user, np.where(np.repeat(keep_u, 2), t_g, 0.0))
     if 'decay_all_rows' in mutate:
         tu[users] = True
     apply_rowwise((Wu, bu), (dWu, dbu), (tu, tu), opt, lr, (wds[0], wds[2]), eps,
@@ -273,8 +281,7 @@ def fused_step(params, users, items, negs, loss, opt, lr, weight_decay=0.0, eps=
     ki = np.nonzero(keep_i)[0]
     dWi = _row_sums(Wi.shape, t_row[ki], t_g[ki, None] * src[t_user[ki]])
     dbi = _row_sums(bi.shape, t_row[ki], t_g[ki])
-    ti = np.zeros(Wi.shape[0], dtype=bool)
-    ti[t_row[(t_g != 0) & keep_i]] = True
+    ti = touched(Wi.shape[0], t_row, np.where(keep_i, t_g, 0.0))
     if 'decay_all_rows' in mutate:
         ti[t_row] = True
     apply_rowwise((Wi, bi), (dWi, dbi), (ti, ti), opt, lr, (wds[1], wds[3]), eps,

@@ -40,9 +40,10 @@ def seg_sort_cap(D):
     return 128 if G >= 8 else (64 if G >= 4 else 16 * G)
 
 
-def long_groups(D):
-    """Lane groups per CTA of mf_user_long_kernel / mf_item_long_kernel (LPR = D / 4)."""
-    return 256 // (D // 4)
+def long_groups(D, first_gen=False):
+    """Lane groups per CTA of mf_user_long_kernel / mf_item_long_kernel (LPR = D / 4), or with
+    ``first_gen`` of the first-generation step's mf_bwd_long_kernel (LPR = lpr_for_dim(D))."""
+    return 256 // (lpr_for_dim(D) if first_gen else D // 4)
 
 
 def small_limit(sms):
@@ -64,28 +65,34 @@ def large_case(D, loss, sms=132):
     return make_case(D, small_limit(sms) + 1001, loss, seed=100 + D + LOSSES.index(loss), sms=sms)
 
 
-def very_hot_length(D):
+def very_hot_length(D, first_gen=False):
     """Longer than cap + 1, and not a multiple of the long kernels' lane groups."""
-    G = long_groups(D)
+    G = long_groups(D, first_gen)
     return (seg_sort_cap(D) // G + 2) * G + 5
 
 
-def _user_lengths(D, rs, hot, extra_hot):
+def _user_lengths(D, rs, hot, extra_hot, first_gen=False):
     cap = seg_sort_cap(D)
-    lens = [1] * 4 + [2] * 4 + list(range(3, 17)) + [17, int(rs.randint(18, cap)), cap - 1, cap]
+    if cap >= 19:
+        lens = [1] * 4 + [2] * 4 + list(range(3, 17)) + [17, int(rs.randint(18, cap)), cap - 1, cap]
+    else:                   # cap 16 (LPR 1): no 17..cap class
+        lens = [1] * 4 + [2] * 4 + list(range(3, cap + 1))
     if hot:
-        lens += [cap + 1, very_hot_length(D)]
-    G = long_groups(D)
+        lens += [cap + 1, very_hot_length(D, first_gen)]
+    G = long_groups(D, first_gen)
     lens += [cap + 1 + int(rs.randint(0, 2 * G)) for _ in range(extra_hot)]
     return lens
 
 
-def _item_lengths(D, rs, hot):
+def _item_lengths(D, rs, hot, first_gen=False):
     cap = seg_sort_cap(D)
-    lens = [1, 2, 3, 4] * 2 + [5, 6, 7, 8] + [9] + list(range(10, 17)) + [17, int(rs.randint(18, cap)),
-                                                                          cap - 1, cap]
+    if cap >= 19:
+        lens = [1, 2, 3, 4] * 2 + [5, 6, 7, 8] + [9] + list(range(10, 17)) + [17, int(rs.randint(18, cap)),
+                                                                              cap - 1, cap]
+    else:
+        lens = [1, 2, 3, 4] * 2 + [5, 6, 7, 8] + [9] + list(range(10, cap + 1))
     if hot:
-        lens += [cap + 1, very_hot_length(D)]
+        lens += [cap + 1, very_hot_length(D, first_gen)]
     return lens
 
 
@@ -101,18 +108,20 @@ def _ids(n, forced, rs):
     return out
 
 
-def make_case(D, B, loss, seed, sms=132, hot=True, extra_hot_users=0, min_users=0):
+def make_case(D, B, loss, seed, sms=132, hot=True, extra_hot_users=0, min_users=0, first_gen=False):
     """One minibatch of B interactions at dimension D: dict(D, B, loss, U, I, Wu, Wi, bu, bi,
     users, items, negs, cap, hot, fixed) with float32 tables and int64 ids.  ``fixed`` marks the
     interactions that carry a prescribed edge (same item, hinge tie, inactive user).
     ``extra_hot_users`` adds that many more users with cap + 1 .. cap + 2G interactions, and
-    ``min_users`` pads the user table so that ids spread over many scan tiles."""
+    ``min_users`` pads the user table so that ids spread over many scan tiles.  ``first_gen``:
+    the very hot lists are sized for the lane groups of the first-generation step's long kernel
+    (any D that is a multiple of 4) instead of the planned step's."""
     rs = np.random.RandomState(seed)
     cap = seg_sort_cap(D)
     hinge = loss == 'hinge'
-    ulens = _user_lengths(D, rs, hot, extra_hot_users)
+    ulens = _user_lengths(D, rs, hot, extra_hot_users, first_gen)
     nb = len(ulens) - extra_hot_users        # the last two prescribed lists get ids 0 and U - 1
-    ilens = _item_lengths(D, rs, hot)
+    ilens = _item_lengths(D, rs, hot, first_gen)
     n_ded = 4 if hinge else 0                 # dedicated hinge interactions: 1 tie + 3 inactive
     Bf = B - n_ded
     if Bf < sum(ulens) or 2 * Bf < sum(ilens) + 2:
@@ -154,7 +163,7 @@ def make_case(D, B, loss, seed, sms=132, hot=True, extra_hot_users=0, min_users=
     Wi = rs.randn(I, D) * se
     bu = rs.randn(U, 1) * 0.1
     bi = rs.randn(I, 1) * 0.1
-    case = dict(D=D, B=B, loss=loss, U=U, I=I, cap=cap, hot=hot, sms=sms, same=int(same))
+    case = dict(D=D, B=B, loss=loss, U=U, I=I, cap=cap, hot=hot, sms=sms, same=int(same), first_gen=first_gen)
     if hinge:
         # tie: zero user row, pos = 0.25 + 0.75, neg = 0.25 - 0.25, z = neg - pos + 1 = 0 exactly
         tu, iu = uid[nu_struct + pool_u], uid[nu_struct + pool_u + 1]
@@ -222,6 +231,9 @@ def length_classes(D, hot=True):
     user = [('1', 1, 1), ('2', 2, 2), ('3-16', 3, 16), ('17-cap', 17, cap - 1), ('cap', cap, cap)]
     item = [('1-4', 1, 4), ('5-8', 5, 8), ('9', 9, 9), ('10-16', 10, 16), ('17-cap', 17, cap - 1),
             ('cap', cap, cap)]
+    if cap < 19:                      # cap 16: 3..16 reaches the cap
+        user = [c for c in user if c[0] != '17-cap']
+        item = [c for c in item if c[0] != '17-cap']
     if hot:
         user.append(('cap+1', cap + 1, cap + 1))
         item.append(('cap+1', cap + 1, cap + 1))
@@ -232,7 +244,7 @@ def check_properties(case, ref):
     """Problems (an empty list when none) of the case's scales on the oracle result ``ref``
     (oracle.mf.fused_step's dict: pos, neg, gp, gn)."""
     out = []
-    D, cap, G = case['D'], case['cap'], long_groups(case['D'])
+    D, cap, G = case['D'], case['cap'], long_groups(case['D'], case.get('first_gen', False))
     lens = member_lengths(case)
     for side, classes in length_classes(D, case['hot']).items():
         for name, lo, hi in classes:

@@ -87,6 +87,11 @@ class FusedAdam(torch.optim.Optimizer):
     sequence model's item table and bias) are registered through ``fused_states`` and flushed;
     every other parameter (convolutions, LSTM, projection) takes ordinary dense Adam in
     ``step()``, which on the fused routes runs after the kernel with the same step count.
+
+    Hyperparameters may change between steps (``param_groups[0]``, by hand or through a
+    ``torch.optim.lr_scheduler``): dense Adam took the steps a row missed with the values of their
+    time, so before the first use of new values every pending step is flushed with the values it
+    was taken under, and the schedule is rebuilt.  One O(table) flush per change.
     """
 
     fused_kind = _lib.OPT_ADAM
@@ -96,17 +101,21 @@ class FusedAdam(torch.optim.Optimizer):
         super(FusedAdam, self).__init__(params, defaults)
         self._t = 0                      # optimizer steps taken (torch's state['step'])
         self._sched = None
+        self._hp = None                  # the hyperparameters the lazy state was advanced with
 
     # torch.optim.Optimizer pickles only defaults / state / param_groups: keep the step count so
-    # that a pickled model resumes fit() with the right bias corrections
+    # that a pickled model resumes fit() with the right bias corrections, and the hyperparameters
+    # of its pending steps
     def __getstate__(self):
         st = super(FusedAdam, self).__getstate__()
         st['_t'] = self._t
+        st['_hp'] = self._hp
         return st
 
     def __setstate__(self, state):
         state = dict(state)
         self._t = state.pop('_t', 0)
+        self._hp = state.pop('_hp', None)
         self._sched = None
         super(FusedAdam, self).__setstate__(state)
 
@@ -134,12 +143,26 @@ class FusedAdam(torch.optim.Optimizer):
         self.state[param]['lazy'] = 'own' if own_last else 'pair'
         return states
 
+    def _current_hparams(self):
+        """``fused_hparams()``, after the lazy state has caught up with any change of them: when
+        they differ from those the pending steps were taken under, every lazy table is flushed
+        with the recorded values first and the schedule is dropped.  ``schedule()``, ``flush()``
+        and ``step()`` all start here."""
+        hp = self.fused_hparams()
+        if self._hp is not None and hp != self._hp:
+            self._flush(self._hp)
+            self._sched = None
+        self._hp = hp
+        return hp
+
     def schedule(self, upto, device):
         """Device table of the per-step scalars lr / (1 - beta1^t), sqrt(1 - beta2^t), t <= upto
         (computed in double, as torch's Python does)."""
+        return self._schedule(self._current_hparams(), upto, device)
+
+    def _schedule(self, hp, upto, device):
         import numpy as np
         if self._sched is None or self._sched.shape[0] < 2 * (upto + 1) or self._sched.device != device:
-            hp = self.fused_hparams()
             cap = max(4096, 2 * upto)
             t = np.arange(cap + 1, dtype=np.float64)
             tab = np.empty((cap + 1, 2), dtype=np.float64)
@@ -166,11 +189,14 @@ class FusedAdam(torch.optim.Optimizer):
     def flush(self):
         """Replay the pending (gradient-free) steps of every row of the lazily updated tables (those
         registered through ``fused_states``); every other parameter is always current."""
+        self._flush(self._current_hparams())
+
+    def _flush(self, hp):
+        """``flush()`` with the hyperparameters ``hp``."""
         from spotlight_b200 import ops
         if self._t == 0:
             return
         lib = _lib.load()
-        hp = self.fused_hparams()
         scalars = (hp['beta1'], hp['beta2'], 1.0 - hp['beta1'], 1.0 - hp['beta2'], hp['eps'], hp['weight_decay'],
                    ops._stream())
         params = self._lazy('pair')
@@ -186,7 +212,7 @@ class FusedAdam(torch.optim.Optimizer):
             rows = W.shape[0]
             m, v, last = self.fused_states(W)
             bm, bv, _ = self.fused_states(b)
-            sched = self.schedule(self._t, W.device)
+            sched = self._schedule(hp, self._t, W.device)
             with torch.no_grad():
                 _lib.check(lib.slb_adam_flush(ops._ptr(W), ops._ptr(m), ops._ptr(v), ops._ptr(b), ops._ptr(bm),
                                               ops._ptr(bv), ops._ptr(last), rows, W.shape[1], ops._ptr(sched),
@@ -195,7 +221,7 @@ class FusedAdam(torch.optim.Optimizer):
             if not p.is_cuda:
                 continue
             m, v, last = self._moments(p)
-            sched = self.schedule(self._t, p.device)
+            sched = self._schedule(hp, self._t, p.device)
             with torch.no_grad():
                 _lib.check(lib.slb_adam_flush_table(ops._ptr(p), ops._ptr(m), ops._ptr(v), ops._ptr(last),
                                                     p.shape[0], p[0].numel(), ops._ptr(sched), self._t, *scalars),
@@ -211,9 +237,9 @@ class FusedAdam(torch.optim.Optimizer):
         current.  Sparse gradients are rejected, as torch.optim.Adam rejects them."""
         loss = closure() if closure is not None else None
         params = [p for g in self.param_groups for p in g['params'] if p.grad is not None]
+        hp = self._current_hparams()
         if any(self.state.get(p, {}).get('lazy') for p in params):
-            self.flush()
-        hp = self.fused_hparams()
+            self._flush(hp)
         self._t += 1
         t = self._t
         ss = hp['lr'] / (1.0 - hp['beta1'] ** t)
