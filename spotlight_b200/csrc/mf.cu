@@ -1212,8 +1212,15 @@ int validate(const slb_mf_step_args* x) {
                     "mf_train_step: compact mode needs urows/gWu/gbu/irows/gWi/gbi/compact_counts");
     }
     SLB_REQUIRE(x->opt >= SLB_OPT_NONE && x->opt <= SLB_OPT_ADAM, "mf_train_step: bad optimizer");
-    if (x->opt == SLB_OPT_ADAM) {
-        SLB_REQUIRE(x->grad_mode == SLB_GRAD_COMPACT && !x->opt_users_only, "mf_train_step: fused Adam needs compact grads");
+    if (x->opt == SLB_OPT_ADAM && x->opt_users_only) {
+        // sharded item rows: Adam on the user tables only, the item gradient handed out dense
+        SLB_REQUIRE(x->grad_mode == SLB_GRAD_DENSE, "mf_train_step: users-only Adam needs dense item grads");
+        SLB_REQUIRE(x->state_Wu && x->state_bu && x->state2_Wu && x->state2_bu && x->last_u && x->adam_sched &&
+                    x->adam_step >= 1 && x->adam_step < (1ll << 31),
+                    "mf_train_step: users-only Adam needs the user exp_avg / exp_avg_sq / last_u / schedule and "
+                    "adam_step >= 1");
+    } else if (x->opt == SLB_OPT_ADAM) {
+        SLB_REQUIRE(x->grad_mode == SLB_GRAD_COMPACT, "mf_train_step: fused Adam needs compact grads");
         SLB_REQUIRE(x->state_Wu && x->state_Wi && x->state_bu && x->state_bi && x->state2_Wu && x->state2_Wi &&
                     x->state2_bu && x->state2_bi && x->last_u && x->last_i && x->adam_sched && x->adam_step >= 1,
                     "mf_train_step: fused Adam needs exp_avg / exp_avg_sq / last / schedule and adam_step >= 1");
@@ -1263,7 +1270,17 @@ int launch_step(const slb_mf_step_args* x, const int64_t* users, const int64_t* 
     const int groups = MF_THREADS / lpr;
     const int sms = slb_sms();
     const int grid = min(slb_grid((B + groups - 1) / groups, 8), MF_MAX_GRID);
-    if ((phases & 1) && x->opt == SLB_OPT_ADAM) {
+    const bool adam_users_only = x->opt == SLB_OPT_ADAM && x->opt_users_only;
+    if ((phases & 1) && adam_users_only) {
+        // sharded item rows: their owners caught them up; the referenced user rows become current here
+        AdamDev o = {x->beta1, x->beta2, x->one_minus_beta1, x->one_minus_beta2, x->eps, x->weight_decay, x->adam_sched,
+                     static_cast<int32_t>(x->adam_step + step_idx)};
+        const int pgrid = slb_grid((B + groups - 1) / groups, 8);
+        with_lpr(lpr, [&](auto L) {
+            mf_adam_users_prepass_kernel<L><<<pgrid, MF_THREADS, 0, st>>>(a, o, x->state2_Wu, x->state2_bu, x->last_u);
+        });
+        SLB_LAUNCH_CHECK("mf_adam_users_prepass_kernel");
+    } else if ((phases & 1) && x->opt == SLB_OPT_ADAM) {
         // lazy-exact Adam: the rows this minibatch reads become current (through step t-1) first
         AdamDev o = {x->beta1, x->beta2, x->one_minus_beta1, x->one_minus_beta2, x->eps, x->weight_decay, x->adam_sched,
                      static_cast<int32_t>(x->adam_step + step_idx)};
@@ -1311,7 +1328,23 @@ int launch_step(const slb_mf_step_args* x, const int64_t* users, const int64_t* 
     const int bti = bsmall ? 8 : 32;
     const int64_t tw = ((2 * B + bti - 1) / bti + 3) / 4;     // upper bound on segment tiles
     const int tgrid = slb_grid(tw, 16);
-    if (x->opt == SLB_OPT_NONE || x->opt == SLB_OPT_ADAM) {
+    if (adam_users_only) {
+        // the dense item gradient first (it reads the user rows at t - 1), then Adam on the user rows
+        if (phases & 8) {
+            launch_bwd_tile<1>(a, lpr, bsmall, tgrid, st);
+            SLB_LAUNCH_CHECK("mf_bwd_tile_kernel<items>");
+            launch_long<1>(lpr, st, a);
+            SLB_LAUNCH_CHECK("mf_bwd_long_kernel<items>");
+        }
+        if (phases & 16) {
+            AdamDev o = {x->beta1, x->beta2, x->one_minus_beta1, x->one_minus_beta2, x->eps, x->weight_decay, x->adam_sched,
+                         static_cast<int32_t>(x->adam_step + step_idx)};
+            with_lpr(lpr, [&](auto L) {
+                mf_adam_users_kernel<L><<<bgrid, MF_THREADS, 0, st>>>(a, o, x->state2_Wu, x->state2_bu, x->last_u);
+            });
+            SLB_LAUNCH_CHECK("mf_adam_users_kernel");
+        }
+    } else if (x->opt == SLB_OPT_NONE || x->opt == SLB_OPT_ADAM) {
         if (phases & 8) {
             launch_bwd_tile<0>(a, lpr, bsmall, tgrid, st);
             SLB_LAUNCH_CHECK("mf_bwd_tile_kernel");
@@ -1727,6 +1760,29 @@ int slb_adam_flush_table(float* W, float* exp_avg, float* exp_avg_sq, int32_t* l
         adam_flush_table_kernel<L><<<grid, MF_THREADS, 0, st>>>(W, exp_avg, exp_avg_sq, last, rows, dim, o);
     });
     SLB_LAUNCH_CHECK("adam_flush_table_kernel");
+    return SLB_OK;
+}
+
+int slb_adam_dense(float* W, float* exp_avg, float* exp_avg_sq, float* bias, float* bias_avg, float* bias_avg_sq,
+                   int32_t* last, const float* grad, const float* bias_grad, int64_t rows, int32_t dim,
+                   const float* sched, int64_t step, float beta1, float beta2, float one_minus_beta1,
+                   float one_minus_beta2, float eps, float weight_decay, slb_stream_t stream) {
+    SLB_REQUIRE(rows >= 0 && dim >= 1 && step >= 1 && step < (1ll << 31), "adam_dense: bad sizes");
+    if (rows == 0) return SLB_OK;       // an empty shard: the tensors may have no storage
+    SLB_REQUIRE(W && exp_avg && exp_avg_sq && bias && bias_avg && bias_avg_sq && last && grad && bias_grad && sched,
+                "adam_dense: null pointer");
+    SLB_REQUIRE(rows < (1ll << 40) && dim < (1 << 28), "adam_dense: too large");
+    AdamDev o = {beta1, beta2, one_minus_beta1, one_minus_beta2, eps, weight_decay, sched, static_cast<int32_t>(step)};
+    int lpr = 1;                                  // one element per lane: D lanes, a power of two, at most a warp
+    while (lpr < dim && lpr < 32) lpr <<= 1;
+    const int groups = MF_THREADS / lpr;
+    const int grid = slb_grid((rows + groups - 1) / groups, 16);
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    with_lpr(lpr, [&](auto L) {
+        adam_dense_kernel<L><<<grid, MF_THREADS, 0, st>>>(W, exp_avg, exp_avg_sq, bias, bias_avg, bias_avg_sq, last,
+                                                         grad, bias_grad, rows, dim, o);
+    });
+    SLB_LAUNCH_CHECK("adam_dense_kernel");
     return SLB_OK;
 }
 

@@ -96,9 +96,10 @@ class GpuBackend(object):
         return rows, bias
 
     def local_step(self, st, cache_rows, cache_bias, n_cache, users_local, pos_idx, neg_idx,
-                   loss, global_batch, n_neg=1):
+                   loss, global_batch, n_neg=1, t=None):
         """Fused forward/backward on (user shard, row cache).  Updates the user
-        shard in place (row-wise Adagrad); returns (loss share, d cache rows, d cache bias)."""
+        shard in place (row-wise Adagrad; under ``st.opt``, lazy-exact Adam step ``t``); returns
+        (loss share, d cache rows, d cache bias)."""
         lib = _lib.load()
         cap, D = cache_rows.shape
         a = ops.mf_step_args(st.Wu, cache_rows, st.bu, cache_bias, users_local, pos_idx, neg_idx,
@@ -109,15 +110,28 @@ class GpuBackend(object):
         a.loss_out = loss_out.data_ptr()
         a.grad_mode = _lib.GRAD_DENSE
         a.dWi, a.dbi = dWi.data_ptr(), dbi.data_ptr()
-        a.opt, a.lr, a.weight_decay, a.eps = _lib.OPT_ADAGRAD, st.lr, 0.0, st.eps
-        a.state_Wu, a.state_bu = st.sWu.data_ptr(), st.sbu.data_ptr()
         a.norm_batch, a.opt_users_only = int(global_batch), 1
+        if st.opt is not None:
+            # users-only lazy-exact Adam (first-generation step): the referenced user rows catch up
+            # through t - 1, the touched ones take step t; the cache rows' owners keep their state
+            sched = st.opt.schedule(t, self.device)
+            hp = st.opt.fused_hparams()
+            a.opt, a.lr, a.weight_decay, a.eps = _lib.OPT_ADAM, hp['lr'], hp['weight_decay'], hp['eps']
+            a.beta1, a.beta2 = hp['beta1'], hp['beta2']
+            a.one_minus_beta1, a.one_minus_beta2 = 1.0 - hp['beta1'], 1.0 - hp['beta2']
+            a.state_Wu, a.state_bu = st.mWu.data_ptr(), st.mbu.data_ptr()
+            a.state2_Wu, a.state2_bu, a.last_u = st.vWu.data_ptr(), st.vbu.data_ptr(), st.last_u.data_ptr()
+            a.adam_sched, a.adam_step = sched.data_ptr(), int(t)
+        else:
+            a.opt, a.lr, a.weight_decay, a.eps = _lib.OPT_ADAGRAD, st.lr, 0.0, st.eps
+            a.state_Wu, a.state_bu = st.sWu.data_ptr(), st.sbu.data_ptr()
         need = lib.slb_mf_step_workspace_bytes(a.batch, n_neg, a.loss, a.num_users, a.num_items)
         ws = ops.workspace('mf%d_%d' % (a.num_users, a.num_items), need, self.device)
         a.workspace, a.workspace_bytes = ws.data_ptr(), ws.numel()
         # planned two-kernel step (csrc/mf_v2.cuh): user rows updated in place, the item kernel
-        # hands the dense cache-row gradient out for the owners
-        need2 = lib.slb_mf_fused_workspace_bytes(a.batch, a.num_users, a.num_items, a.dim) if n_neg == 1 else 0
+        # hands the dense cache-row gradient out for the owners (Adagrad only)
+        need2 = (lib.slb_mf_fused_workspace_bytes(a.batch, a.num_users, a.num_items, a.dim)
+                 if n_neg == 1 and st.opt is None else 0)
         if need2:
             fws = ops.workspace('mfv2_%d_%d_%d' % (a.num_users, a.num_items, a.dim), need2,
                                 self.device)
@@ -141,13 +155,14 @@ class GpuBackend(object):
                                               rows, D, st.lr, st.eps, ops._ptr(ws), ws.numel(), ops._stream()),
                    'shard_rows_adagrad')
 
-    def _adam_tables(self, st, t):
-        """The item shard, its bias and their lazy-exact Adam state, with step t's scalars (the
-        arguments the owner-side Adam entries share after their ids)."""
+    def _adam_tables(self, st, t, users=False):
+        """The item shard (the user shard: ``users``), its bias and their lazy-exact Adam state, with
+        step t's scalars (the arguments the row-wise Adam entries share after their ids)."""
         hp = st.opt.fused_hparams()
-        rows, D = st.Wi.shape
-        return (ops._ptr(st.Wi), ops._ptr(st.mWi), ops._ptr(st.vWi), ops._ptr(st.bi), ops._ptr(st.mbi),
-                ops._ptr(st.vbi), ops._ptr(st.last), rows, D, ops._ptr(st.opt.schedule(t, self.device)), t,
+        W, m, v, b, bm, bv, last = self._adam_pair(st, users)
+        rows, D = W.shape
+        return (ops._ptr(W), ops._ptr(m), ops._ptr(v), ops._ptr(b), ops._ptr(bm), ops._ptr(bv), ops._ptr(last),
+                rows, D, ops._ptr(st.opt.schedule(t, self.device)), t,
                 hp['beta1'], hp['beta2'], 1.0 - hp['beta1'], 1.0 - hp['beta2'], hp['eps'], hp['weight_decay'])
 
     def owner_adam_catch_up(self, st, local_ids, t):
@@ -158,6 +173,16 @@ class GpuBackend(object):
             return
         ids = local_ids.contiguous().long()
         _lib.check(_lib.load().slb_shard_rows_adam_catch_up(ops._ptr(ids), R, *self._adam_tables(st, t),
+                                                            ops._stream()), 'shard_rows_adam_catch_up')
+
+    def user_adam_catch_up(self, st, user_ids, t):
+        """Lazy-exact Adam before adaptive hinge scores step t: the user rows ``user_ids`` (local,
+        repeats allowed) and their biases replay the steps they missed, through t - 1."""
+        R = user_ids.numel()
+        if R == 0:
+            return
+        ids = user_ids.contiguous().long()
+        _lib.check(_lib.load().slb_shard_rows_adam_catch_up(ops._ptr(ids), R, *self._adam_tables(st, t, True),
                                                             ops._stream()), 'shard_rows_adam_catch_up')
 
     def owner_adam_update(self, st, local_ids, g_rows, g_bias, t):
@@ -174,6 +199,39 @@ class GpuBackend(object):
         _lib.check(lib.slb_shard_rows_adam(ops._ptr(ids), ops._ptr(g_rows), ops._ptr(g_bias), R,
                                            *self._adam_tables(st, t), ops._ptr(ws), ws.numel(), ops._stream()),
                    'shard_rows_adam')
+
+    def _adam_pair(self, st, users):
+        """The user shard (``users``) or the item shard, with its bias and their Adam state."""
+        if users:
+            return st.Wu, st.mWu, st.vWu, st.bu, st.mbu, st.vbu, st.last_u
+        return st.Wi, st.mWi, st.vWi, st.bi, st.mbi, st.vbi, st.last
+
+    def _adam_scalars(self, st):
+        hp = st.opt.fused_hparams()
+        return (hp['beta1'], hp['beta2'], 1.0 - hp['beta1'], 1.0 - hp['beta2'], hp['eps'], hp['weight_decay'],
+                ops._stream())
+
+    def owner_adam_catch_up_shard(self, st, upto):
+        """Every row of the item shard and its bias current through step ``upto``: before the dense
+        exchange gathers the whole shard."""
+        W, m, v, b, bm, bv, last = self._adam_pair(st, False)
+        if upto < 1:
+            return
+        sched = st.opt.schedule(upto, self.device)
+        _lib.check(_lib.load().slb_adam_flush(ops._ptr(W), ops._ptr(m), ops._ptr(v), ops._ptr(b), ops._ptr(bm),
+                                              ops._ptr(bv), ops._ptr(last), W.shape[0], W.shape[1], ops._ptr(sched),
+                                              upto, *self._adam_scalars(st)), 'adam_flush')
+
+    def adam_dense(self, st, users, g, g_bias, t):
+        """Dense Adam step t on the user shard (``users``) or the item shard and its bias: every
+        row replays its pending steps, then takes step t with its gradient row, zero rows included."""
+        W, m, v, b, bm, bv, last = self._adam_pair(st, users)
+        sched = st.opt.schedule(t, self.device)
+        g, g_bias = g.contiguous(), g_bias.reshape(-1).contiguous()
+        _lib.check(_lib.load().slb_adam_dense(ops._ptr(W), ops._ptr(m), ops._ptr(v), ops._ptr(b), ops._ptr(bm),
+                                              ops._ptr(bv), ops._ptr(last), ops._ptr(g), ops._ptr(g_bias),
+                                              W.shape[0], W.shape[1], ops._ptr(sched), t,
+                                              *self._adam_scalars(st)), 'adam_dense')
 
     def owner_adam_flush(self, st):
         """Every row of the item shard and its bias current for the steps taken (FusedAdam.flush);
@@ -315,9 +373,17 @@ def adagrad_dense_(W, state, grad, lr, eps):
 
 
 class ShardState(object):
-    """This rank's parameter shards and Adagrad state."""
+    """This rank's parameter shards and their optimizer state.
 
-    def __init__(self, plan, rank, dim, device, lr=0.05, eps=1e-10, init=None):
+    ``optimizer_func``: None (row-wise Adagrad at ``lr``, ``eps``), ``optim.fused_adagrad`` without
+    weight decay (Adagrad with its ``lr``, ``eps``) or ``optim.fused_adam``; it is called on
+    :meth:`params`.  Under ``fused_adam``, ``opt`` is that ``FusedAdam``: the user shard and its bias
+    (``bu2``, the (rows, 1) view of ``bu``) and the item shard and its bias (``bi2``) are its two
+    lazily updated table pairs, with moments ``mWu``, ``vWu``, ``mbu``, ``vbu`` / ``mWi``, ``vWi``,
+    ``mbi``, ``vbi`` and the step each row is current for, ``last_u`` / ``last``.  A rank that owns no
+    users registers the item pair only."""
+
+    def __init__(self, plan, rank, dim, device, lr=0.05, eps=1e-10, init=None, optimizer_func=None):
         ulo, uhi = plan.user_range(rank)
         ilo, ihi = plan.item_range(rank)
         self.ulo, self.uhi, self.ilo, self.ihi = ulo, uhi, ilo, ihi
@@ -338,8 +404,40 @@ class ShardState(object):
             self.Wu = torch.randn((uhi - ulo, dim), device=dev) / dim
             self.Wi[:ihi - ilo] = torch.randn((ihi - ilo, dim), device=dev) / dim
             self.bu = torch.zeros(uhi - ulo, device=dev)
-        self.sWu, self.sWi = torch.zeros_like(self.Wu), torch.zeros_like(self.Wi)
-        self.sbu, self.sbi = torch.zeros_like(self.bu), torch.zeros_like(self.bi)
+        self.bu2, self.bi2 = self.bu.reshape(-1, 1), self.bi.reshape(-1, 1)
+        self.opt = None
+        state = torch.zeros_like                    # Adagrad's accumulators
+        if optimizer_func is not None:
+            from spotlight_b200.optim import FusedAdagrad, FusedAdam
+            opt = optimizer_func(self.params())
+            if isinstance(opt, FusedAdam):
+                self.opt = opt
+                self.mWi, self.vWi, self.last = opt.fused_states(self.Wi)
+                self.mbi, self.vbi, _ = opt.fused_states(self.bi2)
+                if self.Wu.shape[0]:
+                    self.mWu, self.vWu, self.last_u = opt.fused_states(self.Wu)
+                    self.mbu, self.vbu, _ = opt.fused_states(self.bu2)
+                else:                               # no users here: nothing to step or flush
+                    self.mWu, self.vWu = torch.zeros_like(self.Wu), torch.zeros_like(self.Wu)
+                    self.mbu, self.vbu = torch.zeros_like(self.bu2), torch.zeros_like(self.bu2)
+                    self.last_u = torch.zeros(0, dtype=torch.int32, device=dev)
+                state = lambda p: None              # noqa: E731
+            elif isinstance(opt, FusedAdagrad) and opt.fused_hparams()['weight_decay'] == 0:
+                hp = opt.fused_hparams()
+                self.lr, self.eps = hp['lr'], hp['eps']
+            else:
+                # fused_adagrad's weight decay moves the rows a minibatch updates, which the owners
+                # do not see as the single-process step does
+                raise ValueError('the sharded factorization model trains with optimizer_func=None (row-wise '
+                                 'Adagrad at learning_rate), optim.fused_adagrad without weight decay or '
+                                 'optim.fused_adam; got %s' % type(opt).__name__)
+        self.sWu, self.sWi = state(self.Wu), state(self.Wi)
+        self.sbu, self.sbi = state(self.bu), state(self.bi)
+
+    def params(self):
+        """The table pairs (user shard, its bias as a (rows, 1) view, item shard, its bias) -- the user
+        pair only when this rank owns users."""
+        return ([self.Wu, self.bu2] if self.Wu.shape[0] else []) + [self.Wi, self.bi2]
 
 
 def _global_loss(loss_share, group):
@@ -457,6 +555,11 @@ class ShardedMF(_RowExchange):
         plan, st, P = self.plan, self.st, self.plan.world
         chunk, D = plan.ichunk, st.Wi.shape[1]
         dev = users.device
+        adam, kw = st.opt is not None, {}
+        if adam:                            # lazy-exact Adam: every rank gathers every row, current through t - 1
+            t = st.opt.steps_taken + 1
+            kw = {'t': t}
+            self.backend.owner_adam_catch_up_shard(st, t - 1)
         pad_W, pad_b = st.Wi, st.bi          # shards are stored padded to the common chunk
         full_W = st.Wi.new_empty((P * chunk, D))
         full_b = st.bi.new_empty(P * chunk)
@@ -466,15 +569,19 @@ class ShardedMF(_RowExchange):
         self.stats['rows_requested'] += P * chunk
         if users.numel():
             loss_share, g_rows, g_bias = self.backend.local_step(
-                st, full_W, full_b, P * chunk, users - st.ulo, items, negs, loss, global_batch, n_neg)
+                st, full_W, full_b, P * chunk, users - st.ulo, items, negs, loss, global_batch, n_neg, **kw)
         else:                               # none of this minibatch's users live here
             loss_share, g_rows, g_bias = full_b.new_zeros(()), torch.zeros_like(full_W), torch.zeros_like(full_b)
         g_shard = _reduce_scatter(g_rows.contiguous(), chunk, self.rank, self.group)
         gb_shard = _reduce_scatter(g_bias.contiguous(), chunk, self.rank, self.group)
         self.stats['bytes_a2a'] += (g_rows.numel() + g_bias.numel()) * 4
         n = st.Wi.shape[0]
-        adagrad_dense_(st.Wi, st.sWi, g_shard[:n], st.lr, st.eps)
-        adagrad_dense_(st.bi, st.sbi, gb_shard[:n], st.lr, st.eps)
+        if adam:                            # dense Adam step t on the whole shard, then count it
+            self.backend.adam_dense(st, False, g_shard[:n], gb_shard[:n], t)
+            st.opt.advance(1)
+        else:
+            adagrad_dense_(st.Wi, st.sWi, g_shard[:n], st.lr, st.eps)
+            adagrad_dense_(st.bi, st.sbi, gb_shard[:n], st.lr, st.eps)
         return _global_loss(loss_share, self.group)
 
     def step_a2a(self, users, items, negs, loss, global_batch, n_neg=1):
@@ -485,16 +592,35 @@ class ShardedMF(_RowExchange):
         """
         st = self.st
         B = users.numel()
-        cache_rows, cache_bias, inverse, n_cache, route = self._fetch_rows(torch.cat([items, negs]))
+        catch_up, kw = self._adam_hooks()
+        cache_rows, cache_bias, inverse, n_cache, route = self._fetch_rows(torch.cat([items, negs]), catch_up)
         # fused local step (user rows updated in place)
         if B:
             loss_share, g_rows, g_bias = self.backend.local_step(
                 st, cache_rows, cache_bias, n_cache, users - st.ulo, inverse[:B], inverse[B:], loss,
-                global_batch, n_neg)
+                global_batch, n_neg, **kw)
         else:
             loss_share, g_rows, g_bias = st.bi.new_zeros(()), cache_rows[:0], cache_bias[:0]
-        self.backend.owner_update(st, *self._return_grads(route, g_rows, g_bias))
+        self._owner_step(self._return_grads(route, g_rows, g_bias), kw)
         return _global_loss(loss_share, self.group)
+
+    def _adam_hooks(self):
+        """(before_gather, local-step keywords) of this step: under lazy-exact Adam the owner catches
+        the requested rows up through t - 1 before it gathers them, and the step is t."""
+        st = self.st
+        if st.opt is None:
+            return None, {}
+        t = st.opt.steps_taken + 1
+        return (lambda local_req: self.backend.owner_adam_catch_up(st, local_req, t)), {'t': t}    # noqa: E731
+
+    def _owner_step(self, returned, kw):
+        """The owner's update of the rows its peers returned gradients for: Adagrad, or Adam step t,
+        which every rank then counts (also a rank without members, so t stays equal everywhere)."""
+        if not kw:
+            self.backend.owner_update(self.st, *returned)
+            return
+        self.backend.owner_adam_update(self.st, *returned, kw['t'])
+        self.st.opt.advance(1)
 
     def step_adaptive(self, users, items, negs_block, bpos, batch_users, n_neg):
         """Adaptive hinge on a sharded minibatch, with the reference's pairing.
@@ -513,11 +639,15 @@ class ShardedMF(_RowExchange):
         be = self.backend
         m, Bg, n = users.numel(), batch_users.numel(), int(n_neg)
         dev = users.device
-        cache_rows, cache_bias, inverse, n_cache, route = self._fetch_rows(torch.cat([items, negs_block]))
+        catch_up, kw = self._adam_hooks()
+        cache_rows, cache_bias, inverse, n_cache, route = self._fetch_rows(torch.cat([items, negs_block]), catch_up)
         ul = users - st.ulo
         ul_rep = ul.repeat_interleave(n)
         # scores of this rank's members and of their n-blocks
         if m:
+            if kw:
+                # the user rows scored current through t - 1 (the others catch up in adam_dense below)
+                be.user_adam_catch_up(st, ul, kw['t'])
             pos = be.scores(st, cache_rows, cache_bias, ul, inverse[:m])
             neg = be.scores(st, cache_rows, cache_bias, ul_rep, inverse[m:])
         else:
@@ -557,12 +687,15 @@ class ShardedMF(_RowExchange):
             g_neg[order] = g_sorted
             dWu, dcache, dbu, dbcache = be.scores_backward(
                 st, cache_rows, torch.cat([gp, g_neg]), torch.cat([ul, ul_rep]), inverse)
-            adagrad_dense_(st.Wu, st.sWu, dWu, st.lr, st.eps)
-            adagrad_dense_(st.bu, st.sbu, dbu.reshape(-1), st.lr, st.eps)
+            if kw:                          # dense Adam step t on the user shard
+                be.adam_dense(st, True, dWu, dbu, kw['t'])
+            else:
+                adagrad_dense_(st.Wu, st.sWu, dWu, st.lr, st.eps)
+                adagrad_dense_(st.bu, st.sbu, dbu.reshape(-1), st.lr, st.eps)
             g_rows, g_bias = dcache[:n_cache], dbcache.reshape(-1)[:n_cache]
         else:
             g_rows, g_bias = cache_rows[:0], cache_bias[:0]
-        self.backend.owner_update(st, *self._return_grads(route, g_rows, g_bias))
+        self._owner_step(self._return_grads(route, g_rows, g_bias), kw)
         return _global_loss(loss_share, self.group)
 
 
@@ -879,14 +1012,23 @@ class ShardedImplicitFactorizationModel(object):
     * ``epoch_loss`` is the mean of the global minibatch losses.
 
     Every rank is handed the same ``Interactions`` (the global shuffle needs all of it);
-    parameters and optimizer state are sharded, never replicated.  Optimizer: row-wise
-    Adagrad (``spotlight_b200.optim.fused_adagrad``'s update).  All four losses; adaptive
+    parameters and optimizer state are sharded, never replicated.  All four losses; adaptive
     hinge keeps the reference's global negative pairing (:meth:`ShardedMF.step_adaptive`).
+    Optimizer (``optimizer_func``):
+
+    * ``None``: row-wise Adagrad at ``learning_rate`` (``spotlight_b200.optim.fused_adagrad``'s
+      update); ``fused_adagrad(lr, eps)`` without weight decay is the same with its hyper-parameters;
+    * ``fused_adam(lr, betas, eps, weight_decay)``: row-wise lazy-exact Adam on the user shard and on
+      the item shard at its owners -- the trajectory of
+      ``ImplicitFactorizationModel(optimizer_func=fused_adam(...))``, i.e. dense ``torch.optim.Adam``
+      on all four tables, weight decay included, up to fp32 rounding.  ``fit()`` brings every row
+      current before it returns, and repeated calls resume the step count and the moments;
+    * anything else raises ``ValueError``.
     """
 
     def __init__(self, num_users, num_items, rank, world, device, backend=None, loss='bpr',
                  embedding_dim=32, n_iter=10, batch_size=256, learning_rate=0.05, random_state=None,
-                 exchange='auto', init=None, group=None, num_negative_samples=5):
+                 exchange='auto', init=None, group=None, num_negative_samples=5, optimizer_func=None):
         assert loss in ('pointwise', 'bpr', 'hinge', 'adaptive_hinge')
         self._n_neg = int(num_negative_samples) if loss == 'adaptive_hinge' else 1
         self._loss, self._n_iter, self._batch_size = loss, int(n_iter), int(batch_size)
@@ -901,7 +1043,8 @@ class ShardedImplicitFactorizationModel(object):
         seed = int(self._random_state.randint(-10 ** 8, 10 ** 8))
         if init is None:
             torch.manual_seed(seed + 7919 * rank)
-        self.state = ShardState(self.plan, rank, embedding_dim, device, lr=learning_rate, init=init)
+        self.state = ShardState(self.plan, rank, embedding_dim, device, lr=learning_rate, init=init,
+                                optimizer_func=optimizer_func)
         self.mf = ShardedMF(self.plan, self.state, rank, self.backend, group=group)
         self.epoch_losses = []
 
@@ -933,6 +1076,8 @@ class ShardedImplicitFactorizationModel(object):
                 print('Epoch {}: loss {}'.format(epoch, epoch_loss))
             if np.isnan(epoch_loss) or epoch_loss == 0.0:
                 raise ValueError('Degenerate epoch loss: {}'.format(epoch_loss))
+        if self.state.opt is not None:
+            be.owner_adam_flush(self.state)                 # lazy-exact Adam: every row current
         return self
 
     def _run_epoch_device(self, u, i):
@@ -951,7 +1096,7 @@ class ShardedImplicitFactorizationModel(object):
         bounds = torch.searchsorted(mine, edges).tolist()                   # the epoch's one sync
         dense = self._exchange == 'dense' or (self._exchange == 'auto' and
                                               self.mf._dense_exchange_pays(B // plan.world))
-        if dense and nn == 1 and isinstance(be, GpuBackend):
+        if dense and nn == 1 and isinstance(be, GpuBackend) and self.state.opt is None:
             return self._epoch_dense_gpu(u, i, mine, bounds)
         mu, mi = u[mine], i[mine]
         bpos = mine % B
