@@ -34,7 +34,7 @@ EXPORTS = (
     'slb_embedding_backward_workspace_bytes', 'slb_embedding_backward',
     'slb_mf_scores', 'slb_mf_scores_backward', 'slb_rank_pairs', 'slb_rank_targets', 'slb_mixture_scores', 'slb_mf_step_workspace_bytes', 'slb_mf_fused_workspace_bytes', 'slb_mf_compact_rows',
     'slb_mf_train_step', 'slb_mf_train_step_phases', 'slb_mf_fit_epoch', 'slb_mf_fit_epoch_events', 'slb_adam_flush',
-    'slb_adam_flush_table', 'slb_adam_dense',
+    'slb_adam_flush_table', 'slb_adam_dense', 'slb_adam_dense_table', 'slb_bias_sparse_adam',
     'slb_mf_bloom_workspace_bytes', 'slb_mf_bloom_train_step',
     'slb_bias_sparse_workspace_bytes', 'slb_bias_sparse_apply',
     'slb_unique_workspace_bytes', 'slb_unique_bucket', 'slb_shard_gather_batch', 'slb_adagrad_dense',
@@ -175,6 +175,10 @@ def _declare(lib):
                                          c_f32, c_f32, c_f32, c_f32, c_f32, c_f32, c_vp]
     lib.slb_adam_dense.argtypes = [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_i32, c_vp, c_i64,
                                    c_f32, c_f32, c_f32, c_f32, c_f32, c_f32, c_vp]
+    lib.slb_adam_dense_table.argtypes = [c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_i32, c_vp, c_i64,
+                                         c_f32, c_f32, c_f32, c_f32, c_f32, c_f32, c_vp]
+    lib.slb_bias_sparse_adam.argtypes = [c_vp, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_i64,
+                                         c_f32, c_f32, c_f32, c_f32, c_f32, c_f32, c_vp, c_sz, c_vp]
     lib.slb_unique_workspace_bytes.argtypes = [c_i64, c_i64]
     lib.slb_unique_workspace_bytes.restype = c_sz
     lib.slb_unique_bucket.argtypes = [c_vp, c_i64, c_i64, c_i64, c_i32, c_vp, c_vp, c_vp, c_vp, c_sz, c_vp]

@@ -1976,9 +1976,15 @@ struct BloomLayout {
 // scored sides per interaction: positive + negative, or the one rated pair of a rating loss
 static int bloom_sides(const slb_mf_bloom_args* x) { return is_rating_loss(x->base.loss) ? 1 : 2; }
 
+// users-only mode (multi-GPU local step): the optimizer runs on the user rows and user biases only
+static bool bloom_users_only(const slb_mf_bloom_args* x) {
+    return x->base.opt != SLB_OPT_NONE && x->base.opt_users_only != 0;
+}
+
 static BloomLayout bloom_layout(void* base, const slb_mf_bloom_args* x) {
     const int nu = x->user_hashes ? x->user_hashes : 1, ni = x->item_hashes ? x->item_hashes : 1;
     const int64_t B = x->base.batch, P = bloom_sides(x) * B, T = P * nu * ni;
+    const bool uo = bloom_users_only(x);
     WsCarver ws(base);
     BloomLayout l;
     l.done = ws.take<int32_t>(8);
@@ -2004,13 +2010,15 @@ static BloomLayout bloom_layout(void* base, const slb_mf_bloom_args* x) {
         // this workspace is dedicated to one (shapes, batch), so every offset is fixed.
         l.bws_u = ws.take<char>(bias_sparse_bytes(P));
         l.bws_i = ws.take<char>(bias_sparse_bytes(P));
-        const int64_t irow_cap = T < x->item_rows ? T : x->item_rows;
-        l.irows = ws.take<int64_t>(irow_cap + 1);
-        l.gWi = ws.take<float>(static_cast<size_t>(irow_cap + 1) * x->base.dim);
+        if (!uo) {                  // users-only: the item gradient goes to the caller's dense dWi
+            const int64_t irow_cap = T < x->item_rows ? T : x->item_rows;
+            l.irows = ws.take<int64_t>(irow_cap + 1);
+            l.gWi = ws.take<float>(static_cast<size_t>(irow_cap + 1) * x->base.dim);
+        }
         l.compact_counts = ws.take<int32_t>(4);
     }
     l.urows = nullptr; l.gWu = nullptr;
-    if (x->base.opt == SLB_OPT_ADAM) {
+    if (x->base.opt == SLB_OPT_ADAM && !uo) {       // users-only Adam sums the user rows from the terms
         const int64_t urow_cap = T < x->user_rows ? T : x->user_rows;
         l.urows = ws.take<int64_t>(urow_cap + 1);
         l.gWu = ws.take<float>(static_cast<size_t>(urow_cap + 1) * x->base.dim);
@@ -2024,6 +2032,10 @@ static int bloom_adam_prepass(const MfDev& a, const BloomSpec& h, const AdamDev&
                               cudaStream_t st);
 static int bloom_adam_step(const MfDev& a, const AdamDev& o, const BloomAdamDev& s, const BloomLayout& l,
                            const slb_mf_bloom_args* x, int lpr, int tgrid, cudaStream_t st);
+static int bloom_users_adam_prepass(const MfDev& a, const AdamDev& o, const slb_mf_bloom_args* x, int lpr,
+                                    cudaStream_t st);
+static int bloom_users_adam_step(const MfDev& a, const AdamDev& o, const BloomLayout& l, const slb_mf_bloom_args* x,
+                                 int lpr, cudaStream_t st);
 
 extern "C" {
 
@@ -2047,11 +2059,30 @@ int slb_mf_bloom_train_step(const slb_mf_bloom_args* x, slb_stream_t stream) {
     }
     const bool fused = b.opt != SLB_OPT_NONE;
     const bool adam = b.opt == SLB_OPT_ADAM;
+    const bool uo = bloom_users_only(x);
+    if (uo) {
+        // the multi-GPU local step: plain user shard (in place), full hashed item table (dense dWi for
+        // the reduce-scatter), replicated item bias (pairs for the all-gather)
+        SLB_REQUIRE(!rating && b.n_neg == 1 && b.loss != SLB_LOSS_ADAPTIVE_HINGE,
+                    "mf_bloom_train_step: users-only mode takes the pointwise, bpr and hinge losses (n_neg = 1)");
+        SLB_REQUIRE(b.opt == SLB_OPT_ADAGRAD || adam, "mf_bloom_train_step: users-only mode takes Adagrad or Adam");
+        SLB_REQUIRE(b.grad_mode == SLB_GRAD_DENSE && b.dWi && pairs_i && !x->pair_ids_u && !x->pair_g_u &&
+                    x->user_hashes == 0,
+                    "mf_bloom_train_step: users-only mode needs a plain user table, dense dWi and item-bias pairs "
+                    "(the user biases are updated in place: no user pairs)");
+        SLB_REQUIRE(b.state_Wu && b.state_bu, "mf_bloom_train_step: users-only mode needs the user state");
+        if (adam) {
+            SLB_REQUIRE(b.state2_Wu && b.state2_bu && b.last_u && b.state_bi && b.state2_bi && x->last_bi &&
+                        b.adam_sched && b.adam_step >= 1 && b.adam_step < (1ll << 31),
+                        "mf_bloom_train_step: users-only Adam needs the user exp_avg / exp_avg_sq / last_u, the item "
+                        "bias exp_avg / exp_avg_sq / last_bi, the schedule and adam_step >= 1");
+        }
+    }
     SLB_REQUIRE(fused ? (b.opt == SLB_OPT_SGD || b.opt == SLB_OPT_ADAGRAD || adam) : b.grad_mode == SLB_GRAD_DENSE,
                 "mf_bloom_train_step: dense gradients, or a fused SGD / Adagrad / Adam optimizer");
-    SLB_REQUIRE(!fused || b.opt == SLB_OPT_SGD || (b.state_Wu && b.state_Wi && b.state_bu && b.state_bi),
+    SLB_REQUIRE(!fused || uo || b.opt == SLB_OPT_SGD || (b.state_Wu && b.state_Wi && b.state_bu && b.state_bi),
                 "mf_bloom_train_step: adagrad / adam need state");
-    if (adam) {
+    if (adam && !uo) {
         SLB_REQUIRE(!rating, "mf_bloom_train_step: fused Adam takes the pairwise losses only");
         SLB_REQUIRE(b.grad_mode == SLB_GRAD_COMPACT, "mf_bloom_train_step: fused Adam needs compact mode");
         SLB_REQUIRE(b.state2_Wu && b.state2_Wi && b.state2_bu && b.state2_bi && b.last_u && b.last_i && x->last_bu &&
@@ -2086,7 +2117,7 @@ int slb_mf_bloom_train_step(const slb_mf_bloom_args* x, slb_stream_t stream) {
     a.seg = l.seg;
     const int lpr = lpr_for_dim(b.dim);
     a.seg.long_cap = seg_sort_cap(lpr);
-    a.grad_mode = fused ? SLB_GRAD_COMPACT : SLB_GRAD_DENSE;
+    a.grad_mode = fused && !uo ? SLB_GRAD_COMPACT : SLB_GRAD_DENSE;     // users-only: dense dWi out
     a.dWu = b.dWu; a.dWi = b.dWi; a.dbu = b.dbu; a.dbi = b.dbi;
     a.irows = l.irows; a.gWi = l.gWi; a.compact_counts = l.compact_counts;
     a.opt = b.opt; a.lr = b.lr; a.wd = b.weight_decay; a.eps = b.eps;
@@ -2102,16 +2133,23 @@ int slb_mf_bloom_train_step(const slb_mf_bloom_args* x, slb_stream_t stream) {
     h.ids_u2 = l.ids_u2; h.ids_i2 = l.ids_i2; h.g_u2 = l.g_u2; h.g_i2 = l.g_i2;
     h.idle_ids = fused ? 1 : 0;
     if (!fused && pairs_u) { h.ids_u2 = x->pair_ids_u; h.g_u2 = x->pair_g_u; }
-    if (!fused && pairs_i) { h.ids_i2 = x->pair_ids_i; h.g_i2 = x->pair_g_i; }
+    if ((!fused || uo) && pairs_i) { h.ids_i2 = x->pair_ids_i; h.g_i2 = x->pair_g_i; }
 
     const int groups = MF_THREADS / lpr;
     const int grid = min(slb_grid((B + groups - 1) / groups, 8), MF_MAX_GRID);
     AdamDev o = {};
     BloomAdamDev s = {};
     if (adam) {
-        // lazy-exact Adam: everything this minibatch reads becomes current (through step t-1) first
         o = {b.beta1, b.beta2, b.one_minus_beta1, b.one_minus_beta2, b.eps, b.weight_decay, b.adam_sched,
              static_cast<int32_t>(b.adam_step)};
+    }
+    if (adam && uo) {
+        // the referenced user rows (with their biases) and item-bias ids current through t-1; the hashed
+        // item table arrives current from its owners
+        const int rc = bloom_users_adam_prepass(a, o, x, lpr, st);
+        if (rc != SLB_OK) return rc;
+    } else if (adam) {
+        // lazy-exact Adam: everything this minibatch reads becomes current (through step t-1) first
         s = {b.state2_Wu, b.state2_Wi, b.state2_bu, b.state2_bi, b.last_u, b.last_i, x->last_bu, x->last_bi};
         a.urows = l.urows; a.gWu = l.gWu;
         const int rc = bloom_adam_prepass(a, h, o, s, lpr, st);
@@ -2131,6 +2169,19 @@ int slb_mf_bloom_train_step(const slb_mf_bloom_args* x, slb_stream_t stream) {
     seg_sort_long_kernel<<<SEG_LONG_CTAS, 256, 0, st>>>(a.seg);
     SLB_LAUNCH_CHECK("seg_sort_long_kernel");
     const int tgrid = slb_grid(((2 * T + 31) / 32 + 3) / 4, 16);
+    if (uo) {
+        // the dense hashed-row gradient first (it reads the user rows as the forward did), then the
+        // user rows and user biases take their step in place: O(batch), no dense user gradient
+        launch_bwd_tile<1>(a, lpr, false, tgrid, st);
+        SLB_LAUNCH_CHECK("mf_bwd_tile_kernel<items>");
+        launch_long<1>(lpr, st, a);
+        if (adam) return bloom_users_adam_step(a, o, l, x, lpr, st);
+        launch_bwd_tile<2>(a, lpr, false, tgrid, st);
+        SLB_LAUNCH_CHECK("mf_bwd_tile_kernel<users+opt>");
+        launch_long<2>(lpr, st, a);
+        return bias_sparse_apply(l.bws_u, l.ids_u2, l.g_u2, P, b.bu, b.state_bu, b.opt, b.lr, b.weight_decay, b.eps,
+                                 true, st);
+    }
     if (adam) {
         // compact gradients of both sides from the tables as the forward read them, then step t on
         // the touched rows and on the touched bias ids
@@ -2290,3 +2341,206 @@ static int bloom_adam_step(const MfDev& a, const AdamDev& o, const BloomAdamDev&
     if (rc != SLB_OK) return rc;
     return bias_sparse_adam<int>(l.bws_i, l.ids_i2, l.g_i2, P, b.bi, b.state_bi, b.state2_bi, x->last_bi, o, st);
 }
+
+// ---------------------------------------------------------------------------
+// Users-only mode of the hashed-table step (base.opt_users_only, the multi-GPU local step) and the
+// C entries the owners' side of that step uses.  Same two rules as above: the kernels are templates,
+// launched only from here.
+// ---------------------------------------------------------------------------
+namespace {
+
+// Before the forward of step t (users-only Adam): each user row of the minibatch with its bias (a plain
+// (row, bias) pair sharing last_u) and each item-bias id it reads (positives and negatives, on this
+// rank's replica, last_bi) becomes current through t-1.  The hashed item table is not touched: its
+// owners step every row of it every step.  One lane group per user, one thread per item id;
+// atomicMax on `last` elects one writer per distinct entry.
+template <int LPR>
+__global__ void __launch_bounds__(MF_THREADS)
+mf_bloom_users_prepass_kernel(MfDev a, AdamDev o, float* vWu, float* vbu, int32_t* last_u, float* vbi,
+                              int32_t* last_bi, int64_t num_items) {
+    constexpr int GROUPS = MF_THREADS / LPR;
+    const int gl = threadIdx.x & (LPR - 1);
+    const unsigned gmask = group_mask(LPR);
+    const int D = a.D;
+    const int upto = o.t - 1;
+    if (upto <= 0) return;
+    for (int64_t r = static_cast<int64_t>(blockIdx.x) * GROUPS + threadIdx.x / LPR; r < a.B;
+         r += static_cast<int64_t>(gridDim.x) * GROUPS) {
+        const int64_t row = a.users[r];
+        if (row < 0 || row >= a.U) continue;                               // the forward flags bad ids
+        int old = 0;
+        if (gl == 0) old = atomicMax(last_u + row, upto);
+        old = __shfl_sync(gmask, old, (threadIdx.x & 31) & ~(LPR - 1));
+        if (old >= upto) continue;
+        float* W = a.Wu + row * D;
+        float* M = a.sWu + row * D;
+        float* V = vWu + row * D;
+        for (int c = gl * 4; c < D; c += LPR * 4) {
+            float4 w = ld4(W + c), m = ld4(M + c), v = ld4(V + c);
+            adam_catch_up(o, old, upto, w, m, v);
+            st4(W + c, w); st4(M + c, m); st4(V + c, v);
+        }
+        if (gl == 0) {
+            float w = a.bu[row], m = a.sbu[row], v = vbu[row];
+            adam_catch_up1(o, old, upto, w, m, v);
+            a.bu[row] = w; a.sbu[row] = m; vbu[row] = v;
+        }
+    }
+    const int64_t nth = static_cast<int64_t>(gridDim.x) * MF_THREADS;
+    for (int64_t r = static_cast<int64_t>(blockIdx.x) * MF_THREADS + threadIdx.x; r < 2 * a.B; r += nth) {
+        const int64_t id = r < a.B ? a.items[r] : a.negs[r - a.B];
+        if (id < 0 || id >= num_items) continue;
+        const int old = atomicMax(last_bi + id, upto);
+        if (old >= upto) continue;
+        float w = a.bi[id], m = a.sbi[id], v = vbi[id];
+        adam_catch_up1(o, old, upto, w, m, v);
+        a.bi[id] = w; a.sbi[id] = m; vbi[id] = v;
+    }
+}
+
+// Users-only Adam: step t on the user rows with a gradient term, in place, after the item kernels
+// have read them.  One lane group per user segment sums the row's gradient over its terms in
+// ascending term order (the partners are the hashed item rows) and applies Adam straight away, as
+// mf_adam_users_kernel does for plain tables.  The user biases are id-indexed and take their step in
+// bias_sparse_adam afterwards: a plain user's row has a term with g != 0 exactly when its bias pair
+// is live, so the two halves of the pair sharing last_u take step t together.
+template <int LPR>
+__global__ void __launch_bounds__(MF_THREADS) mf_bloom_adam_users_kernel(MfDev a, AdamDev o, float* vWu,
+                                                                          int32_t* last_u) {
+    constexpr int GROUPS = MF_THREADS / LPR;
+    constexpr int CAP = seg_sort_cap(LPR);
+    __shared__ int32_t sh_all[GROUPS * 2 * CAP];
+    const int gl = threadIdx.x & (LPR - 1);
+    const int gib = threadIdx.x / LPR;
+    const unsigned gmask = group_mask(LPR);
+    int32_t* sh = sh_all + gib * 2 * CAP;
+    const int D = a.D;
+    const int nsegA = a.seg.totals[2];
+    const float ss = o.sched[2 * o.t], bc = o.sched[2 * o.t + 1];
+    for (int s = blockIdx.x * GROUPS + gib; s < nsegA; s += gridDim.x * GROUPS) {
+        const int start = a.seg.seg_start[s];
+        const int len = a.seg.seg_start[s + 1] - start;
+        const int64_t row = a.seg.seg_row[s];
+        float* W = a.Wu + row * D;
+        float* M = a.sWu + row * D;
+        float* V = vWu + row * D;
+        const int last = last_u[row];
+        for (int c0 = 0; c0 < D; c0 += LPR * 4) {
+            const int c = c0 + gl * 4;
+            float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
+            // hot rows (len > CAP) were sorted in place by seg_sort_long_kernel
+            seg_visit_sorted<LPR>(a.seg.members, start, len, gl, gmask, sh, [&](int32_t t) {
+                if (c < D) fma4(acc, a.t_g[t], ldg4(a.Wi + static_cast<int64_t>(a.t_b[t]) * D + c));
+            }, true);
+            if (c < D) {
+                float4 w = ld4(W + c), m = ld4(M + c), v = ld4(V + c);
+                adam_catch_up(o, last, o.t - 1, w, m, v);
+                adam_elem(o, ss, bc, acc.x, w.x, m.x, v.x);
+                adam_elem(o, ss, bc, acc.y, w.y, m.y, v.y);
+                adam_elem(o, ss, bc, acc.z, w.z, m.z, v.z);
+                adam_elem(o, ss, bc, acc.w, w.w, m.w, v.w);
+                st4(W + c, w); st4(M + c, m); st4(V + c, v);
+            }
+        }
+        __syncwarp(gmask);                    // every lane has read `last` before it moves
+        if (gl == 0) last_u[row] = o.t;
+    }
+}
+
+// Dense Adam step o.t on one table with its own `last` and no bias (a hashed table's shard after the
+// reduce-scatter): every row first replays its pending steps through o.t - 1, then takes step o.t
+// with its gradient row, zero rows included.  Any D >= 1: one element per lane at a time.
+template <int LPR>
+__global__ void __launch_bounds__(MF_THREADS)
+adam_dense_table_kernel(float* W, float* M, float* V, int32_t* last, const float* G, int64_t rows, int D, AdamDev o) {
+    constexpr int GROUPS = MF_THREADS / LPR;
+    const int gl = threadIdx.x & (LPR - 1);
+    const int gib = threadIdx.x / LPR;
+    const float ss = o.sched[2 * o.t], bc = o.sched[2 * o.t + 1];
+    for (int64_t row = static_cast<int64_t>(blockIdx.x) * GROUPS + gib; row < rows;
+         row += static_cast<int64_t>(gridDim.x) * GROUPS) {
+        const int lastv = last[row];
+        for (int c = gl; c < D; c += LPR) {
+            const int64_t e = row * D + c;
+            float w = W[e], m = M[e], v = V[e];
+            adam_catch_up1(o, lastv, o.t - 1, w, m, v);
+            adam_elem(o, ss, bc, G[e], w, m, v);
+            W[e] = w; M[e] = m; V[e] = v;
+        }
+        __syncwarp(group_mask(LPR));          // every lane has read `last` before it moves
+        if (gl == 0) last[row] = o.t;
+    }
+}
+
+}  // namespace
+
+static int bloom_users_adam_prepass(const MfDev& a, const AdamDev& o, const slb_mf_bloom_args* x, int lpr,
+                                    cudaStream_t st) {
+    const slb_mf_step_args& b = x->base;
+    const int groups = MF_THREADS / lpr;
+    const int pgrid = slb_grid((a.B + groups - 1) / groups, 8);
+    with_lpr(lpr, [&](auto L) {
+        mf_bloom_users_prepass_kernel<L><<<pgrid, MF_THREADS, 0, st>>>(a, o, b.state2_Wu, b.state2_bu, b.last_u,
+                                                                       b.state2_bi, x->last_bi, b.num_items);
+    });
+    SLB_LAUNCH_CHECK("mf_bloom_users_prepass_kernel");
+    return SLB_OK;
+}
+
+// Users-only Adam after the item kernels: step t on the touched user rows, then on the touched user
+// biases (bias_sparse_adam on the step's user pairs, sharing last_u with the rows).
+static int bloom_users_adam_step(const MfDev& a, const AdamDev& o, const BloomLayout& l, const slb_mf_bloom_args* x,
+                                 int lpr, cudaStream_t st) {
+    const slb_mf_step_args& b = x->base;
+    const int groups = MF_THREADS / lpr;
+    const int agrid = slb_grid((2 * a.B + groups - 1) / groups, 8);
+    with_lpr(lpr, [&](auto L) {
+        mf_bloom_adam_users_kernel<L><<<agrid, MF_THREADS, 0, st>>>(a, o, b.state2_Wu, b.last_u);
+    });
+    SLB_LAUNCH_CHECK("mf_bloom_adam_users_kernel");
+    return bias_sparse_adam<int>(l.bws_u, l.ids_u2, l.g_u2, 2 * b.batch, b.bu, b.state_bu, b.state2_bu, b.last_u, o,
+                                 st);
+}
+
+extern "C" {
+
+int slb_bias_sparse_adam(const int64_t* ids, const float* g, int64_t n, float* bias, float* exp_avg,
+                         float* exp_avg_sq, int32_t* last, const float* sched, int64_t step, float beta1,
+                         float beta2, float one_minus_beta1, float one_minus_beta2, float eps, float weight_decay,
+                         void* workspace, size_t workspace_bytes, slb_stream_t stream) {
+    if (n <= 0) return SLB_OK;
+    SLB_REQUIRE(ids && g && bias && exp_avg && exp_avg_sq && last && sched && workspace,
+                "bias_sparse_adam: null pointer");
+    SLB_REQUIRE(n < (1ll << 30), "bias_sparse_adam: too many pairs");
+    SLB_REQUIRE(step >= 1 && step < (1ll << 31), "bias_sparse_adam: step must be >= 1");
+    if (workspace_bytes < bias_sparse_bytes(n)) {
+        slb_set_error("bias_sparse_adam: workspace too small");
+        return SLB_ENOSPC;
+    }
+    AdamDev o = {beta1, beta2, one_minus_beta1, one_minus_beta2, eps, weight_decay, sched, static_cast<int32_t>(step)};
+    return bias_sparse_adam<int>(workspace, ids, g, n, bias, exp_avg, exp_avg_sq, last, o,
+                                 static_cast<cudaStream_t>(stream));
+}
+
+int slb_adam_dense_table(float* W, float* exp_avg, float* exp_avg_sq, int32_t* last, const float* grad, int64_t rows,
+                         int32_t dim, const float* sched, int64_t step, float beta1, float beta2,
+                         float one_minus_beta1, float one_minus_beta2, float eps, float weight_decay,
+                         slb_stream_t stream) {
+    SLB_REQUIRE(rows >= 0 && dim >= 1 && step >= 1 && step < (1ll << 31), "adam_dense_table: bad sizes");
+    if (rows == 0) return SLB_OK;       // an empty shard: the tensors may have no storage
+    SLB_REQUIRE(W && exp_avg && exp_avg_sq && last && grad && sched, "adam_dense_table: null pointer");
+    SLB_REQUIRE(rows < (1ll << 40) && dim < (1 << 28), "adam_dense_table: too large");
+    AdamDev o = {beta1, beta2, one_minus_beta1, one_minus_beta2, eps, weight_decay, sched, static_cast<int32_t>(step)};
+    int lpr = 1;                                  // one element per lane: D lanes, a power of two, at most a warp
+    while (lpr < dim && lpr < 32) lpr <<= 1;
+    const int groups = MF_THREADS / lpr;
+    const int grid = slb_grid((rows + groups - 1) / groups, 16);
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    with_lpr(lpr, [&](auto L) {
+        adam_dense_table_kernel<L><<<grid, MF_THREADS, 0, st>>>(W, exp_avg, exp_avg_sq, last, grad, rows, dim, o);
+    });
+    SLB_LAUNCH_CHECK("adam_dense_table_kernel");
+    return SLB_OK;
+}
+
+}  // extern "C"

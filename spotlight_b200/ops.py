@@ -537,10 +537,18 @@ def _bloom_adam_args(x, params, states, adam):
     a.adam_sched, a.adam_step = adam['sched'].data_ptr(), step
 
 
-def mf_bloom_step_pairs(Wu, Wi, bu, bi, users, items, negs, loss, item_seeds, item_pad, norm_batch=0):
+def mf_bloom_step_pairs(Wu, Wi, bu, bi, users, items, negs, loss, item_seeds, item_pad, norm_batch=0,
+                        users_only=None, dWi=None):
     """Dense-mode hashed-table step for the multi-GPU path: plain (local) user table, hashed item
     table given in full; returns (loss share, dWu, dWi, (ids_u, g_u), (ids_i, g_i)) -- the
-    id-space bias gradients as (id, g) pairs instead of dense tables."""
+    id-space bias gradients as (id, g) pairs instead of dense tables.
+
+    ``users_only``: the user rows and user biases take their optimizer step in place instead
+    (slb_mf_bloom_args' users-only mode; pointwise / bpr / hinge), and ``dWu`` and the user pairs
+    come back as None.  dict(opt=OPT_ADAGRAD, lr, eps, states=(sWu, sbu)), or dict(opt=OPT_ADAM,
+    lr, eps, weight_decay, beta1, beta2, sched, step, states=((mWu, vWu, last_u), (mbu, vbu),
+    (mbi, vbi, last_bi))): the user rows and biases share ``last_u``; ``last_bi`` is this replica's
+    item-bias ``last``.  ``dWi``: a zeroed (item_rows, D) buffer to write the item gradient to."""
     require_cuda(Wu, Wi, bu, bi, users, items, negs)
     lib = _lib.load()
     users, items, negs = _i64c(users).reshape(-1), _i64c(items).reshape(-1), _i64c(negs).reshape(-1)
@@ -555,27 +563,81 @@ def mf_bloom_step_pairs(Wu, Wi, bu, bi, users, items, negs, loss, item_seeds, it
         a.num_users, a.num_items, a.dim = bu.shape[0], bi.shape[0], Wu.shape[1]
         a.Wu, a.Wi, a.bu, a.bi = Wu.data_ptr(), Wi.data_ptr(), bu.data_ptr(), bi.data_ptr()
         loss_out = torch.empty(1, dtype=torch.float32, device=dev)
-        dWu, dWi = torch.zeros_like(Wu), torch.zeros_like(Wi)
-        pu_i = torch.empty(2 * B, dtype=torch.int64, device=dev)
-        pu_g = torch.empty(2 * B, dtype=torch.float32, device=dev)
+        if dWi is None:
+            dWi = torch.zeros_like(Wi)
+        elif dWi.shape != Wi.shape or dWi.dtype != torch.float32 or not dWi.is_contiguous():
+            raise ValueError('mf_bloom_step_pairs: dWi must be contiguous float32 of the item table\'s shape')
         pi_i = torch.empty(2 * B, dtype=torch.int64, device=dev)
         pi_g = torch.empty(2 * B, dtype=torch.float32, device=dev)
         a.loss_out = loss_out.data_ptr()
         a.grad_mode = _lib.GRAD_DENSE
-        a.dWu, a.dWi = dWu.data_ptr(), dWi.data_ptr()
+        a.dWi = dWi.data_ptr()
         a.norm_batch = int(norm_batch)
-        x.pair_ids_u, x.pair_g_u, x.pair_ids_i, x.pair_g_i = pu_i.data_ptr(), pu_g.data_ptr(), pi_i.data_ptr(), pi_g.data_ptr()
+        x.pair_ids_i, x.pair_g_i = pi_i.data_ptr(), pi_g.data_ptr()
+        if users_only is None:
+            dWu = torch.zeros_like(Wu)
+            pu_i = torch.empty(2 * B, dtype=torch.int64, device=dev)
+            pu_g = torch.empty(2 * B, dtype=torch.float32, device=dev)
+            a.dWu = dWu.data_ptr()
+            x.pair_ids_u, x.pair_g_u = pu_i.data_ptr(), pu_g.data_ptr()
+            upairs = (pu_i, pu_g)
+        else:
+            dWu, upairs = None, None
+            _bloom_users_only_args(x, users_only)
         x.user_rows, x.item_rows = Wu.shape[0], Wi.shape[0]
         x.user_hashes, x.item_hashes = 0, len(item_seeds)
         for k, sd in enumerate(item_seeds):
             x.item_seeds[k] = int(sd) & 0xFFFFFFFF
         x.user_padding_idx, x.item_padding_idx = -1, item_pad
         need = lib.slb_mf_bloom_workspace_bytes(ctypes.byref(x))
-        ws = workspace('mfbp%d_%d_%d_%d_%d_%d' % (Wu.shape[0], Wi.shape[0], bu.shape[0], bi.shape[0],
-                                                  len(item_seeds), B), need, dev)
+        kind = 'mfbp' if users_only is None else 'mfbu%d_' % a.opt
+        ws = workspace(kind + '%d_%d_%d_%d_%d_%d' % (Wu.shape[0], Wi.shape[0], bu.shape[0], bi.shape[0],
+                                                     len(item_seeds), B), need, dev)
         a.workspace, a.workspace_bytes = ws.data_ptr(), ws.numel()
         _lib.check(lib.slb_mf_bloom_train_step(ctypes.byref(x), _stream()), 'mf_bloom_train_step')
-    return loss_out.reshape(()), dWu, dWi, (pu_i, pu_g), (pi_i, pi_g)
+    return loss_out.reshape(()), dWu, dWi, upairs, (pi_i, pi_g)
+
+
+def _bloom_users_only_args(x, uo):
+    """The users-only fields of slb_mf_bloom_args (see mf_bloom_step_pairs)."""
+    a = x.base
+    a.opt, a.opt_users_only = int(uo['opt']), 1
+    a.lr, a.eps, a.weight_decay = float(uo['lr']), float(uo['eps']), float(uo.get('weight_decay', 0.0))
+    if uo['opt'] == _lib.OPT_ADAGRAD:
+        sWu, sbu = uo['states']
+        require_cuda(sWu, sbu)
+        a.state_Wu, a.state_bu = sWu.data_ptr(), sbu.data_ptr()
+        return
+    (mWu, vWu, last_u), (mbu, vbu), (mbi, vbi, last_bi) = uo['states']
+    require_cuda(mWu, vWu, last_u, mbu, vbu, mbi, vbi, last_bi, uo['sched'])
+    step = int(uo['step'])
+    if uo['sched'].numel() < 2 * (step + 1):
+        raise ValueError('mf_bloom_step_pairs: the Adam schedule does not reach step %d' % step)
+    a.state_Wu, a.state2_Wu, a.last_u = mWu.data_ptr(), vWu.data_ptr(), last_u.data_ptr()
+    a.state_bu, a.state2_bu = mbu.data_ptr(), vbu.data_ptr()
+    a.state_bi, a.state2_bi, x.last_bi = mbi.data_ptr(), vbi.data_ptr(), last_bi.data_ptr()
+    b1, b2 = float(uo['beta1']), float(uo['beta2'])
+    a.beta1, a.beta2, a.one_minus_beta1, a.one_minus_beta2 = b1, b2, 1.0 - b1, 1.0 - b2
+    a.adam_sched, a.adam_step = uo['sched'].data_ptr(), step
+
+
+def bias_sparse_adam(ids, g, bias, exp_avg, exp_avg_sq, last, sched, step, beta1, beta2, eps, weight_decay):
+    """Lazy-exact Adam step ``step`` of an id-indexed bias table from (id, g) pairs
+    (slb_bias_sparse_adam): each id with a pair (id >= 0) catches up from its ``last``, sums its
+    pairs in pair order and takes the step."""
+    require_cuda(ids, g, bias, exp_avg, exp_avg_sq, last, sched)
+    lib = _lib.load()
+    n = ids.numel()
+    if n == 0:
+        return
+    ws = workspace('bsp%d' % n, lib.slb_bias_sparse_workspace_bytes(n), bias.device)
+    ids, g = _i64c(ids), _f32c(g)           # held until the launch: a temporary's block could be reused
+    with torch.no_grad():
+        _lib.check(lib.slb_bias_sparse_adam(_ptr(ids), _ptr(g), n, _ptr(bias), _ptr(exp_avg),
+                                            _ptr(exp_avg_sq), _ptr(last), _ptr(sched), int(step), float(beta1),
+                                            float(beta2), 1.0 - float(beta1), 1.0 - float(beta2), float(eps),
+                                            float(weight_decay), _ptr(ws), ws.numel(), _stream()),
+                   'bias_sparse_adam')
 
 
 def bias_sparse_apply(ids, g, bias, state, opt_kind, lr, weight_decay=0.0, eps=1e-10):

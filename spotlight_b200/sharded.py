@@ -240,11 +240,37 @@ class GpuBackend(object):
             st.opt.flush()
 
     # ---- hashed item table (BloomEmbedding, config 4) ----
-    def bloom_local_step(self, st, W_full, users_local, items, negs, loss, global_batch):
-        """Dense-mode hashed step on (local user shard, full hashed item table, replicated item
-        bias): returns (loss share, dWu, dWi, user bias pairs, item bias pairs)."""
-        return ops.mf_bloom_step_pairs(st.Wu, W_full, st.bu.reshape(-1, 1), st.bi.reshape(-1, 1), users_local, items,
-                                       negs, loss, st.item_seeds, 0, norm_batch=global_batch)
+    def bloom_local_step(self, st, W_full, users_local, items, negs, loss, global_batch, t=None):
+        """Users-only hashed step on (local user shard, full hashed item table, replicated item
+        bias): the user rows and user biases take their step in place (row-wise Adagrad; under
+        ``st.opt``, lazy-exact Adam step ``t``), O(batch).  Returns (loss share, None, dWi, None, item
+        bias pairs), dWi padded to the whole-table exchange's ``world * mchunk`` rows."""
+        D = W_full.shape[1]
+        dW = torch.zeros((st.world * st.mchunk, D), dtype=torch.float32, device=self.device)
+        if st.opt is None:
+            uo = dict(opt=_lib.OPT_ADAGRAD, lr=st.lr, eps=st.eps, states=(st.sWu, st.sbu))
+        else:
+            hp = st.opt.fused_hparams()
+            uo = dict(opt=_lib.OPT_ADAM, lr=hp['lr'], eps=hp['eps'], weight_decay=hp['weight_decay'],
+                      beta1=hp['beta1'], beta2=hp['beta2'], sched=st.opt.schedule(t, self.device), step=t,
+                      states=((st.mWu, st.vWu, st.last_u), (st.mbu, st.vbu), (st.mbi, st.vbi, st.last_bi)))
+        out = ops.mf_bloom_step_pairs(st.Wu, W_full, st.bu2, st.bi2, users_local, items, negs, loss,
+                                      st.item_seeds, 0, norm_batch=global_batch, users_only=uo, dWi=dW[:st.M])
+        return out[0], None, dW, None, out[4]
+
+    def bloom_adam_dense(self, st, g_shard, t):
+        """Dense Adam step t on this rank's hashed shard: every row current through t afterwards."""
+        g_shard = g_shard.contiguous()
+        _lib.check(_lib.load().slb_adam_dense_table(
+            ops._ptr(st.Wi), ops._ptr(st.mWi), ops._ptr(st.vWi), ops._ptr(st.last_i), ops._ptr(g_shard),
+            st.Wi.shape[0], st.Wi.shape[1], ops._ptr(st.opt.schedule(t, self.device)), t,
+            *self._adam_scalars(st)), 'adam_dense_table')
+
+    def bloom_bias_adam(self, st, ids, g, t):
+        """Adam step t of the replicated item bias from the all-gathered (id, g) pairs."""
+        hp = st.opt.fused_hparams()
+        ops.bias_sparse_adam(ids, g, st.bi, st.mbi, st.vbi, st.last_bi, st.opt.schedule(t, self.device), t,
+                             hp['beta1'], hp['beta2'], hp['eps'], hp['weight_decay'])
 
     def adagrad_dense(self, W, S, G, lr, eps):
         _lib.check(_lib.load().slb_adagrad_dense(ops._ptr(W), ops._ptr(S), ops._ptr(G.contiguous()), W.numel(),
@@ -1024,29 +1050,108 @@ class ShardedImplicitFactorizationModel(object):
       on all four tables, weight decay included, up to fp32 rounding.  ``fit()`` brings every row
       current before it returns, and repeated calls resume the step count and the moments;
     * anything else raises ``ValueError``.
+
+    ``representation``: a ``BilinearNet`` with a plain user layer and a ``BloomEmbedding(padding_idx=0)``
+    item layer (BASELINE config 4) trains from that net's weights on :class:`ShardedBloomMF`: user
+    shards, the hashed table sharded by row range and exchanged whole, the item bias replicated.
+    Pointwise, bpr and hinge, under either optimizer above; ``exchange`` 'auto' or 'dense' (the
+    hashed table always travels whole).  Anything else raises ``ValueError``.  :meth:`gathered_net`
+    returns the trained net of either kind.
     """
 
     def __init__(self, num_users, num_items, rank, world, device, backend=None, loss='bpr',
                  embedding_dim=32, n_iter=10, batch_size=256, learning_rate=0.05, random_state=None,
-                 exchange='auto', init=None, group=None, num_negative_samples=5, optimizer_func=None):
+                 exchange='auto', init=None, group=None, num_negative_samples=5, optimizer_func=None,
+                 representation=None):
         assert loss in ('pointwise', 'bpr', 'hinge', 'adaptive_hinge')
         self._n_neg = int(num_negative_samples) if loss == 'adaptive_hinge' else 1
         self._loss, self._n_iter, self._batch_size = loss, int(n_iter), int(batch_size)
         self._num_users, self._num_items = int(num_users), int(num_items)
         self._random_state = random_state or np.random.RandomState()
         self._exchange = exchange
-        self.rank, self.world = rank, world
+        self.rank, self.world, self.device = rank, world, torch.device(device)
         self.plan = ShardPlan(num_users, num_items, world)
         self.backend = backend or GpuBackend(device)
+        self._net = None
+        if representation is not None:
+            self._check_bloom_net(representation)
         # the reference seeds torch from the model stream at construction (implicit.py:114);
         # the draw is kept so that the stream position matches the single-process model
         seed = int(self._random_state.randint(-10 ** 8, 10 ** 8))
-        if init is None:
-            torch.manual_seed(seed + 7919 * rank)
-        self.state = ShardState(self.plan, rank, embedding_dim, device, lr=learning_rate, init=init,
-                                optimizer_func=optimizer_func)
-        self.mf = ShardedMF(self.plan, self.state, rank, self.backend, group=group)
+        if representation is not None:
+            net = self._net = representation
+            layer = net.item_embeddings
+            init = [t.detach() for t in (net.user_embeddings.weight, layer.embeddings.weight,
+                                         net.user_biases.weight, net.item_biases.weight)]
+            self.state = BloomShardState(self.plan, rank, net.embedding_dim, device, self._num_items,
+                                         layer.compressed_num_embeddings, layer.num_hash_functions,
+                                         lr=learning_rate, init=init, optimizer_func=optimizer_func)
+            self.mf = ShardedBloomMF(self.plan, self.state, rank, self.backend, group=group)
+        else:
+            if init is None:
+                torch.manual_seed(seed + 7919 * rank)
+            self.state = ShardState(self.plan, rank, embedding_dim, device, lr=learning_rate, init=init,
+                                    optimizer_func=optimizer_func)
+            self.mf = ShardedMF(self.plan, self.state, rank, self.backend, group=group)
         self.epoch_losses = []
+
+    def _check_bloom_net(self, net):
+        """ValueError unless ``net`` is a BilinearNet that :class:`ShardedBloomMF` trains as given."""
+        from spotlight_b200.factorization.representations import BilinearNet
+        from spotlight_b200.layers import BloomEmbedding, ScaledEmbedding
+        if self._loss == 'adaptive_hinge':
+            raise ValueError('the sharded Bloom model trains pointwise, bpr and hinge; adaptive hinge needs the '
+                             'per-row exchange')
+        if self._exchange == 'a2a':
+            raise ValueError("the sharded Bloom model exchanges the hashed table whole: exchange='auto' or 'dense'")
+        if not isinstance(net, BilinearNet):
+            raise ValueError('representation must be a BilinearNet; got %s' % type(net).__name__)
+        ul, il = net.user_embeddings, net.item_embeddings
+        if type(ul) is not ScaledEmbedding or ul.padding_idx is not None:
+            raise ValueError('the sharded Bloom model takes a plain user layer (ScaledEmbedding without padding); '
+                             'got %s' % type(ul).__name__)
+        if type(il) is not BloomEmbedding or getattr(il, '_bag', False) or il.padding_idx != 0:
+            raise ValueError('the sharded Bloom model takes a BloomEmbedding(bag=False, padding_idx=0) item layer; '
+                             'got %r' % (il,))
+        if ul.sparse or il.embeddings.sparse or net.user_biases.sparse or net.item_biases.sparse:
+            raise ValueError('the sharded Bloom model takes dense gradients: build the net with sparse=False')
+        if net.embedding_dim % 4:
+            raise ValueError('the sharded Bloom model needs embedding_dim % 4 == 0')
+        if ul.num_embeddings != self._num_users or net.user_biases.num_embeddings != self._num_users:
+            raise ValueError('representation has %d user rows, the model %d' % (ul.num_embeddings, self._num_users))
+        if il.num_embeddings != self._num_items or net.item_biases.num_embeddings != self._num_items:
+            raise ValueError('representation has %d item ids, the model %d' % (il.num_embeddings, self._num_items))
+
+    def gathered_net(self):
+        """Collective: the trained ``BilinearNet`` on this rank's device, its tables all-gathered from
+        the shards (a Bloom model: the representation it was built from, its replicated item bias as
+        it is).  Score it with ``mrr_score`` / ``precision_recall_score``."""
+        from spotlight_b200.factorization.representations import BilinearNet
+        st, plan = self.state, self.plan
+
+        def gather(shard, chunk, n):
+            pad = shard.new_zeros((chunk,) + tuple(shard.shape[1:]))
+            pad[:shard.shape[0]] = shard
+            parts = [torch.empty_like(pad) for _ in range(self.world)]
+            dist.all_gather(parts, pad, group=self.mf.group)
+            return torch.cat(parts)[:n]
+
+        Wu = gather(st.Wu, plan.uchunk, self._num_users)
+        bu = gather(st.bu.reshape(-1, 1), plan.uchunk, self._num_users)
+        if self._net is not None:
+            net = self._net.to(self.device)
+            Wi, Wi_dst = gather(st.Wi, st.mchunk, st.M), net.item_embeddings.embeddings.weight
+            bi = st.bi.reshape(-1, 1)
+        else:
+            net = BilinearNet(self._num_users, self._num_items, st.Wu.shape[1]).to(self.device)
+            Wi, Wi_dst = gather(st.Wi, plan.ichunk, self._num_items), net.item_embeddings.weight
+            bi = gather(st.bi.reshape(-1, 1), plan.ichunk, self._num_items)
+        with torch.no_grad():
+            net.user_embeddings.weight.copy_(Wu)
+            net.user_biases.weight.copy_(bu)
+            Wi_dst.copy_(Wi)
+            net.item_biases.weight.copy_(bi)
+        return net
 
     def fit(self, interactions, verbose=False):
         be = self.backend
@@ -1094,8 +1199,9 @@ class ShardedImplicitFactorizationModel(object):
         mine = torch.nonzero((u >= ulo) & (u < uhi)).reshape(-1)
         edges = torch.arange(0, n + B, B, device=mine.device).clamp_(max=n)
         bounds = torch.searchsorted(mine, edges).tolist()                   # the epoch's one sync
-        dense = self._exchange == 'dense' or (self._exchange == 'auto' and
-                                              self.mf._dense_exchange_pays(B // plan.world))
+        bloom = self._net is not None
+        dense = not bloom and (self._exchange == 'dense' or (self._exchange == 'auto' and
+                                                             self.mf._dense_exchange_pays(B // plan.world)))
         if dense and nn == 1 and isinstance(be, GpuBackend) and self.state.opt is None:
             return self._epoch_dense_gpu(u, i, mine, bounds)
         mu, mi = u[mine], i[mine]
@@ -1118,7 +1224,9 @@ class ShardedImplicitFactorizationModel(object):
             for kk in range(k, hi_k):
                 sl = slice(bounds[kk], bounds[kk + 1])
                 mn = negs[mine[sl] - lo_e].reshape(-1)
-                if self._loss == 'adaptive_hinge':
+                if bloom:
+                    losses.append(self.mf.step(mu[sl], mi[sl], mn, self._loss, min(B, n - kk * B)))
+                elif self._loss == 'adaptive_hinge':
                     losses.append(self.mf.step_adaptive(mu[sl], mi[sl], mn, bpos[sl], u[kk * B:(kk + 1) * B], nn))
                 else:
                     losses.append(self.mf.step(mu[sl], mi[sl], mn, self._loss, min(B, n - kk * B),
@@ -1262,12 +1370,22 @@ class BloomShardState(object):
     the common chunk, the item bias (one float per raw item id) REPLICATED -- its forward lookup
     needs 2 values per interaction from arbitrary owners, which would cost a host-synchronised
     all-to-all per step for 4-byte payloads; its replicas are kept identical by applying the same
-    all-gathered sparse updates on every rank."""
+    all-gathered sparse updates on every rank.
 
-    def __init__(self, plan, rank, dim, device, num_ids, hashed_rows, num_hash, lr=0.05, eps=1e-10, init=None):
+    ``optimizer_func`` as :class:`ShardState`'s: None (row-wise Adagrad at ``lr``, ``eps``),
+    ``optim.fused_adagrad`` without weight decay or ``optim.fused_adam``, called on :meth:`params`.
+    Under ``fused_adam``, ``opt`` is that ``FusedAdam`` with three kinds of lazily updated table: the
+    user shard and its bias (``bu2``, (rows, 1)) as a pair sharing ``last_u`` (registered only when
+    this rank owns users), the hashed shard with its own ``last_i`` and the replicated item bias
+    (``bi2``) with its own ``last_bi``; moments ``mWu``, ``vWu``, ``mbu``, ``vbu``, ``mWi``, ``vWi``,
+    ``mbi``, ``vbi``."""
+
+    def __init__(self, plan, rank, dim, device, num_ids, hashed_rows, num_hash, lr=0.05, eps=1e-10, init=None,
+                 optimizer_func=None):
         from spotlight_b200.layers import SEEDS
         dev = torch.device(device)
         self.lr, self.eps = float(lr), float(eps)
+        self.world = plan.world
         self.ulo, self.uhi = plan.user_range(rank)
         self.M, self.num_ids = int(hashed_rows), int(num_ids)
         self.mchunk = -(-self.M // plan.world)
@@ -1288,8 +1406,40 @@ class BloomShardState(object):
             if self.mlo == 0:
                 self.Wi[0] = 0                      # padding row of the hashed table
             self.bi = torch.zeros(self.num_ids, device=dev)
-        self.sWu, self.sWi = torch.zeros_like(self.Wu), torch.zeros_like(self.Wi)
-        self.sbu, self.sbi = torch.zeros_like(self.bu), torch.zeros_like(self.bi)
+        self.bu2, self.bi2 = self.bu.reshape(-1, 1), self.bi.reshape(-1, 1)
+        self.opt = None
+        state = torch.zeros_like                    # Adagrad's accumulators
+        if optimizer_func is not None:
+            from spotlight_b200.optim import FusedAdagrad, FusedAdam
+            opt = optimizer_func(self.params())
+            if isinstance(opt, FusedAdam):
+                self.opt = opt
+                self.mWi, self.vWi, self.last_i = opt.fused_states(self.Wi, own_last=True)
+                self.mbi, self.vbi, self.last_bi = opt.fused_states(self.bi2, own_last=True)
+                if self.Wu.shape[0]:
+                    self.mWu, self.vWu, self.last_u = opt.fused_states(self.Wu)
+                    self.mbu, self.vbu, _ = opt.fused_states(self.bu2)
+                else:                               # no users here: nothing to step or flush
+                    self.mWu, self.vWu = torch.zeros_like(self.Wu), torch.zeros_like(self.Wu)
+                    self.mbu, self.vbu = torch.zeros_like(self.bu2), torch.zeros_like(self.bu2)
+                    self.last_u = torch.zeros(0, dtype=torch.int32, device=dev)
+                state = lambda p: None              # noqa: E731
+            elif isinstance(opt, FusedAdagrad) and opt.fused_hparams()['weight_decay'] == 0:
+                hp = opt.fused_hparams()
+                self.lr, self.eps = hp['lr'], hp['eps']
+            else:
+                # fused_adagrad's weight decay moves the rows a minibatch updates, which the owners
+                # do not see as the single-process step does
+                raise ValueError('the sharded factorization model trains with optimizer_func=None (row-wise '
+                                 'Adagrad at learning_rate), optim.fused_adagrad without weight decay or '
+                                 'optim.fused_adam; got %s' % type(opt).__name__)
+        self.sWu, self.sWi = state(self.Wu), state(self.Wi)
+        self.sbu, self.sbi = state(self.bu), state(self.bi)
+
+    def params(self):
+        """The user shard and its bias as a (rows, 1) view (when this rank owns users), the hashed
+        shard and the replicated item bias as a (num_ids, 1) view."""
+        return ([self.Wu, self.bu2] if self.Wu.shape[0] else []) + [self.Wi, self.bi2]
 
 
 class ShardedBloomMF(object):
@@ -1299,10 +1449,16 @@ class ShardedBloomMF(object):
     Interactions are routed to the rank that owns their user (user gathers and updates local).
     The hashed table is range-sharded; a rank's minibatch references 2 * B * H hashed rows -- at
     config 4 sizes a large fraction of all M rows -- so the table travels whole: all-gather of the
-    shards, the fused hashed step on the full table (in-register murmur3, layers.py:178-204),
-    reduce-scatter of the dense table gradient to the owners, who apply Adagrad.  The id-space
-    bias gradients travel as (id, g) pairs: all-gather, then the same sparse update on every
-    replica.  Loss: one scalar all-reduce."""
+    shards, the fused hashed step on the full table (in-register murmur3, layers.py:178-204) with
+    the user rows and user biases updated in place (users-only mode, O(batch)), reduce-scatter of the
+    dense table gradient to the owners, who step their whole shard.  The id-space item-bias
+    gradients travel as (id, g) pairs: all-gather, then the same sparse update on every replica, in
+    rank order.  Loss: one scalar all-reduce.
+
+    Under lazy-exact Adam (``state.opt``) the step is t = ``steps_taken + 1`` on every rank, also on
+    a rank without members in the minibatch: it contributes a zero gradient and no pairs, and steps
+    its shard and the replica all the same.  The owners' dense step leaves every hashed row current
+    through t, so the next all-gather needs no catch-up."""
 
     def __init__(self, plan, state, rank, backend, group=None, pair_capacity=None):
         self.plan, self.st, self.rank, self.backend, self.group = plan, state, rank, backend, group
@@ -1313,6 +1469,8 @@ class ShardedBloomMF(object):
         st, P, be = self.st, self.plan.world, self.backend
         dev = st.Wi.device
         D = st.Wi.shape[1]
+        adam = st.opt is not None
+        kw = {'t': st.opt.steps_taken + 1} if adam else {}
         W_full = st.Wi.new_empty((P * st.mchunk, D))
         dist.all_gather_into_tensor(W_full, st.Wi, group=self.group)
         m = users.numel()
@@ -1320,24 +1478,36 @@ class ShardedBloomMF(object):
         ids_pad = torch.zeros(cap, dtype=torch.int64, device=dev)
         g_pad = torch.zeros(cap, dtype=torch.float32, device=dev)
         if m:
-            loss_share, dWu, dWi, (iu, gu), (ii, gi) = be.bloom_local_step(st, W_full[:st.M], users - st.ulo, items,
-                                                                           negs, loss, global_batch)
-            be.adagrad_dense(st.Wu, st.sWu, dWu, st.lr, st.eps)
-            be.bias_sparse_adagrad(iu, gu, st.bu, st.sbu, st.lr, st.eps)
+            loss_share, dWu, dWi, upairs, (ii, gi) = be.bloom_local_step(st, W_full[:st.M], users - st.ulo, items,
+                                                                         negs, loss, global_batch, **kw)
+            if dWu is not None:             # a backend that hands the user gradient out: Adagrad here
+                be.adagrad_dense(st.Wu, st.sWu, dWu, st.lr, st.eps)
+                be.bias_sparse_adagrad(upairs[0], upairs[1], st.bu, st.sbu, st.lr, st.eps)
             ids_pad[:ii.numel()] = ii
             g_pad[:gi.numel()] = gi
-            dW_pad = dWi.new_zeros((P * st.mchunk, D))
-            dW_pad[:st.M] = dWi
+            if dWi.shape[0] == P * st.mchunk:
+                dW_pad = dWi
+            else:
+                dW_pad = dWi.new_zeros((P * st.mchunk, D))
+                dW_pad[:st.M] = dWi
         else:
             loss_share = st.bu.new_zeros(())
             dW_pad = st.Wi.new_zeros((P * st.mchunk, D))
         g_shard = _reduce_scatter(dW_pad, st.mchunk, self.rank, self.group)
-        be.adagrad_dense(st.Wi, st.sWi, g_shard, st.lr, st.eps)
+        if adam:
+            be.bloom_adam_dense(st, g_shard, kw['t'])
+        else:
+            be.adagrad_dense(st.Wi, st.sWi, g_shard, st.lr, st.eps)
         ids_all = torch.empty(P * cap, dtype=torch.int64, device=dev)
         g_all = torch.empty(P * cap, dtype=torch.float32, device=dev)
         dist.all_gather_into_tensor(ids_all, ids_pad, group=self.group)
         dist.all_gather_into_tensor(g_all, g_pad, group=self.group)
-        be.bias_sparse_adagrad(ids_all, g_all, st.bi, st.sbi, st.lr, st.eps)
+        if adam:
+            # the zero padding pairs (id 0, g 0) take a real step for id 0: dense Adam steps every id
+            # with a zero gradient too, so that step is exact
+            be.bloom_bias_adam(st, ids_all, g_all, kw['t'])
+            st.opt.advance(1)
+        else:
+            be.bias_sparse_adagrad(ids_all, g_all, st.bi, st.sbi, st.lr, st.eps)
         self.stats['bytes_exchanged'] += (W_full.numel() + dW_pad.numel()) * 4 + P * cap * 12
         return _global_loss(loss_share, self.group)
-
