@@ -277,6 +277,12 @@ int slb_rank_pairs(const float* scores, int64_t n_rows, int64_t n_items, const i
 // result does not depend on the order the elements are visited in.  A row with more than
 // RT_CAP targets is handled in chunks of RT_CAP and re-read once per chunk.  NaN compares as
 // neither greater nor equal, as in rank_pairs_kernel.
+//
+// The kernel is written once over an output policy.  RankFinal (slb_rank_targets) reads each
+// target's score from its row and writes the average rank and stable position; RankCounts
+// (slb_rank_counts) ranks against a block of the columns [col_offset, col_offset + n_cols) of the
+// full row, takes the targets' scores from the caller (a target may lie outside the block) and
+// writes the three counts, which add up across disjoint column ranges.
 namespace {
 
 constexpr int RT_THREADS = 256;
@@ -336,10 +342,34 @@ __device__ __forceinline__ void rt_write(int64_t p, int gt, int eq, int eq_befor
     if (position) position[p] = static_cast<int64_t>(gt) + eq_before;
 }
 
+// the whole row: the target's score is its own element, the counts become rank and position
+struct RankFinal {
+    float* avg_rank;
+    int64_t* position;
+    static constexpr int64_t col0 = 0;
+    __device__ __forceinline__ float key(const float* row, int64_t, int64_t t) const { return row[t]; }
+    __device__ __forceinline__ void write(int64_t p, int gt, int eq, int eq_before) const {
+        rt_write(p, gt, eq, eq_before, avg_rank, position);
+    }
+};
+
+// one column range of the row: scores supplied per target, the counts written as they are
+struct RankCounts {
+    const float* target_scores;
+    int64_t col0;                                 // global id of the block's first column
+    int32_t* gt;
+    int32_t* eq;
+    int32_t* eq_before;
+    __device__ __forceinline__ float key(const float*, int64_t p, int64_t) const { return target_scores[p]; }
+    __device__ __forceinline__ void write(int64_t p, int g, int e, int b) const {
+        gt[p] = g; eq[p] = e; eq_before[p] = b;
+    }
+};
+
+template <class Out>
 __global__ void __launch_bounds__(RT_THREADS)
 rank_targets_kernel(const float* __restrict__ scores, int64_t n_rows, int64_t n_items,
-                    const int64_t* __restrict__ row_ptr, const int64_t* __restrict__ targets,
-                    float* __restrict__ avg_rank, int64_t* __restrict__ position) {
+                    const int64_t* __restrict__ row_ptr, const int64_t* __restrict__ targets, Out out) {
     __shared__ float key[RT_CAP];
     __shared__ int32_t id[RT_CAP];
     __shared__ int16_t slot[RT_CAP];              // index of the sorted entry within its chunk
@@ -352,17 +382,17 @@ rank_targets_kernel(const float* __restrict__ scores, int64_t n_rows, int64_t n_
         if (t1 - t0 == 1) {
             // one target (sequence_mrr_score): plain compares and a block reduction
             const int64_t t = targets[t0];
-            const float s = row[t];
+            const float s = out.key(row, t0, t);
             int c[3] = {0, 0, 0};
             rt_stream_row(row, n_items, [&](float v, int64_t i) {
                 c[0] += v > s;
                 c[1] += v == s;
-                c[2] += (v == s) & (i < t);
+                c[2] += (v == s) & (out.col0 + i < t);
             });
             int tot[3] = {c[0], c[1], c[2]};
             rt_exclusive_scan3(c, warp_tot);
             if (threadIdx.x == RT_THREADS - 1)
-                rt_write(t0, c[0] + tot[0], c[1] + tot[1], c[2] + tot[2], avg_rank, position);
+                out.write(t0, c[0] + tot[0], c[1] + tot[1], c[2] + tot[2]);
             continue;
         }
         for (int64_t c0 = t0; c0 < t1; c0 += RT_CAP) {
@@ -373,7 +403,7 @@ rank_targets_kernel(const float* __restrict__ scores, int64_t n_rows, int64_t n_
                 if (j < m) {
                     const int64_t t = targets[c0 + j];
                     id[j] = static_cast<int32_t>(t);
-                    key[j] = row[t];
+                    key[j] = out.key(row, c0 + j, t);
                 } else {
                     id[j] = INT32_MAX;
                     key[j] = __int_as_float(0x7fffffff);
@@ -418,9 +448,10 @@ rank_targets_kernel(const float* __restrict__ scores, int64_t n_rows, int64_t n_
                     const int b = lo;
                     atomicAdd(&hist[1][b], 1);
                     atomicSub(&hist[1][a], 1);
-                    // within [b, a) the ids ascend: v precedes the targets with id > i
+                    // within [b, a) the ids ascend: v precedes the targets with id > its global id gi
                     hi = a;
-                    while (lo < hi) { const int mid = (lo + hi) >> 1; if (id[mid] <= i) lo = mid + 1; else hi = mid; }
+                    const int64_t gi = out.col0 + i;
+                    while (lo < hi) { const int mid = (lo + hi) >> 1; if (id[mid] <= gi) lo = mid + 1; else hi = mid; }
                     if (lo < a) {
                         atomicAdd(&hist[2][lo], 1);
                         atomicSub(&hist[2][a], 1);
@@ -436,9 +467,9 @@ rank_targets_kernel(const float* __restrict__ scores, int64_t n_rows, int64_t n_
             rt_exclusive_scan3(run, warp_tot);
             for (int x = beg; x < end; ++x) {
                 for (int k = 0; k < 3; ++k) run[k] += hist[k][x];
-                rt_write(c0 + slot[x], run[0], run[1], run[2], avg_rank, position);
+                out.write(c0 + slot[x], run[0], run[1], run[2]);
             }
-            for (int x = nv + threadIdx.x; x < m; x += RT_THREADS) rt_write(c0 + slot[x], 0, 0, 0, avg_rank, position);
+            for (int x = nv + threadIdx.x; x < m; x += RT_THREADS) out.write(c0 + slot[x], 0, 0, 0);
             __syncthreads();
         }
     }
@@ -458,7 +489,36 @@ int slb_rank_targets(const float* scores, int64_t n_rows, int64_t n_items, const
     const int64_t cap = static_cast<int64_t>(slb_sms()) * 8;
     const int grid = static_cast<int>(n_rows < cap ? n_rows : cap);
     rank_targets_kernel<<<grid, RT_THREADS, 0, static_cast<cudaStream_t>(stream)>>>(
-        scores, n_rows, n_items, row_ptr, targets, avg_rank, position);
+        scores, n_rows, n_items, row_ptr, targets, RankFinal{avg_rank, position});
+    SLB_LAUNCH_CHECK("rank_targets_kernel");
+    return SLB_OK;
+}
+
+int slb_rank_counts(const float* scores, int64_t n_rows, int64_t n_cols, int64_t col_offset,
+                    const int64_t* row_ptr, const int64_t* targets, const float* target_scores,
+                    int64_t n_targets, int32_t* gt, int32_t* eq, int32_t* eq_before, slb_stream_t stream) {
+    if (n_targets <= 0 || n_rows <= 0) return SLB_OK;
+    SLB_REQUIRE(row_ptr && targets && target_scores && gt && eq && eq_before, "rank_counts: null pointer");
+    SLB_REQUIRE(n_cols >= 0 && n_cols <= INT32_MAX && col_offset >= 0 && col_offset <= INT32_MAX - n_cols,
+                "rank_counts: columns [%lld, %lld + %lld) outside [0, INT32_MAX]", static_cast<long long>(col_offset),
+                static_cast<long long>(col_offset), static_cast<long long>(n_cols));
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    if (n_cols == 0) {                  // an empty item range: nothing ranks above or beside any target
+        int32_t* outs[3] = {gt, eq, eq_before};
+        for (int32_t* c : outs) {
+            const cudaError_t e = cudaMemsetAsync(c, 0, sizeof(int32_t) * n_targets, st);
+            if (e != cudaSuccess) {
+                slb_set_error("rank_counts: %s", cudaGetErrorString(e));
+                return SLB_ECUDA;
+            }
+        }
+        return SLB_OK;
+    }
+    SLB_REQUIRE(scores, "rank_counts: null pointer");
+    const int64_t cap = static_cast<int64_t>(slb_sms()) * 8;
+    const int grid = static_cast<int>(n_rows < cap ? n_rows : cap);
+    rank_targets_kernel<<<grid, RT_THREADS, 0, st>>>(scores, n_rows, n_cols, row_ptr, targets,
+                                                     RankCounts{target_scores, col_offset, gt, eq, eq_before});
     SLB_LAUNCH_CHECK("rank_targets_kernel");
     return SLB_OK;
 }

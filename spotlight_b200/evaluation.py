@@ -20,12 +20,16 @@ ties in an unspecified order.
 
 Test and train sets may also hold CUDA tensors (``Interactions`` / ``SequenceInteractions`` made on
 the device); each scorer downloads them once at entry.
+
+``mrr_score`` and ``precision_recall_score`` also take a ``ShardedImplicitFactorizationModel``; they
+are then collective (every rank calls them with the same arguments and gets the whole result) and
+rank every target on the item shards where the items live (``spotlight_b200.sharded``).
 """
 
 import numpy as np
 import torch
 
-from spotlight_b200 import _lib, ops
+from spotlight_b200 import _lib, ops, sharded
 from spotlight_b200.factorization.representations import BilinearNet
 from spotlight_b200.interactions import _to_host
 from spotlight_b200.layers import ScaledEmbedding
@@ -176,8 +180,11 @@ def mrr_score(model, test, train=None, user_block=2048):
 
     One score per user with test items: the mean of 1 / average rank (``rankdata`` of the
     negated predictions) over the user's test items; train items, when given, are pushed to
-    the bottom.  ``user_block`` users are scored per GEMM.
+    the bottom.  ``user_block`` users are scored per GEMM.  A sharded factorization model is scored
+    collectively on its item shards (``sharded.sharded_mrr_score``).
     """
+    if isinstance(model, sharded.ShardedImplicitFactorizationModel):
+        return sharded.sharded_mrr_score(model, test, train, user_block)
     test, train = _to_host(test), None if train is None else _to_host(train)
     n_users = int((np.diff(test.tocsr().indptr) > 0).sum())
     out = np.empty(n_users, dtype=np.float64)
@@ -209,8 +216,12 @@ def precision_recall_score(model, test, train=None, k=10, user_block=2048):
     hits / min(k, num_items), recall = hits / the user's number of test items.  Shapes follow
     the reference's ``.squeeze()``: ``(n_users,)`` for a scalar k, ``(n_users, len(k))`` for an
     array.  Exact score ties across the k boundary are ordered by ascending item id (numpy's
-    ``argsort(kind='stable')``); the reference's default argsort orders them arbitrarily.
+    ``argsort(kind='stable')``); the reference's default argsort orders them arbitrarily.  A sharded
+    factorization model is scored collectively on its item shards
+    (``sharded.sharded_precision_recall_score``).
     """
+    if isinstance(model, sharded.ShardedImplicitFactorizationModel):
+        return sharded.sharded_precision_recall_score(model, test, train, k, user_block)
     test, train = _to_host(test), None if train is None else _to_host(train)
     ks = np.array([k]) if np.isscalar(k) else np.asarray(k)
     n_users = int((np.diff(test.tocsr().indptr) > 0).sum())

@@ -337,6 +337,41 @@ class GpuBackend(object):
         hand-back): draw(count) -> (tensor, event the consumer stream must wait for)."""
         return _GpuEpochSampler(self.device, num_items, random_state, total)
 
+    # ---- evaluation on the item shards (mrr_score, precision_recall_score, predict) ----
+    def bloom_item_rows(self, W_full, ids, seeds):
+        """Item vectors of the global ids ``ids`` from the whole hashed table: the lookup
+        ``BloomEmbedding.forward`` does (the sum of each id's hashed rows, padding id 0)."""
+        return ops.embedding(W_full, ids, seeds, 0)
+
+    def shard_scores(self, users, user_bias, items, item_bias):
+        """(len(users), len(items)) scores with the arithmetic of evaluation._score_block: the GEMM,
+        then += user bias, then += item bias."""
+        out = users @ items.t()                             # plain library GEMM (cuBLAS)
+        out += user_bias.reshape(-1, 1)
+        out += item_bias.reshape(1, -1)
+        return out
+
+    def pair_scores(self, users, user_bias, items, item_bias, u_idx, i_idx):
+        """scores[n] = <users[u_idx[n]], items[i_idx[n]]> + user_bias[u_idx[n]] + item_bias[i_idx[n]]:
+        the kernel BilinearNet.forward runs on plain tables."""
+        return ops.mf_scores(users, items, user_bias.reshape(-1, 1), item_bias.reshape(-1, 1), u_idx, i_idx)
+
+    def rank_counts(self, scores, col_offset, row_ptr, targets, target_scores):
+        """(3, n_targets) int32: slb_rank_counts' gt, eq and eq_before of every target over the block's
+        columns, the global items [col_offset, col_offset + scores.shape[1]).  ``row_ptr`` and
+        ``targets`` are host arrays in global item ids, ``target_scores`` the targets' full-row scores."""
+        dev = target_scores.device
+        scores = scores.contiguous()
+        rp = torch.from_numpy(np.ascontiguousarray(row_ptr, dtype=np.int64)).to(dev)
+        tg = torch.from_numpy(np.ascontiguousarray(targets, dtype=np.int64)).to(dev)
+        n = tg.numel()
+        out = torch.empty((3, n), dtype=torch.int32, device=dev)
+        _lib.check(_lib.load().slb_rank_counts(ops._ptr(scores), scores.shape[0], scores.shape[1], col_offset,
+                                               ops._ptr(rp), ops._ptr(tg), ops._ptr(target_scores.contiguous()), n,
+                                               ops._ptr(out[0]), ops._ptr(out[1]), ops._ptr(out[2]), ops._stream()),
+                   'rank_counts')
+        return out
+
     def seq_local_step(self, E_cache, bias_cache, n_cache, seqs_idx, negs_idx, loss, cnn, norm_count,
                        lstm=None, mixture=None, n_neg=1):
         """Fused sequence step on the row cache (ids already remapped onto it; cache
@@ -1057,6 +1092,11 @@ class ShardedImplicitFactorizationModel(object):
     Pointwise, bpr and hinge, under either optimizer above; ``exchange`` 'auto' or 'dense' (the
     hashed table always travels whole).  Anything else raises ``ValueError``.  :meth:`gathered_net`
     returns the trained net of either kind.
+
+    Evaluation, on the shards: ``evaluation.mrr_score`` and ``evaluation.precision_recall_score`` take
+    this model, and :meth:`predict` scores pairs; all three are collective (every rank calls them with
+    the same arguments and gets the whole result) and gather no table whole.  They score the model as
+    it stands: ``fit()`` leaves every lazily updated row current, so nothing is needed between the two.
     """
 
     def __init__(self, num_users, num_items, rank, world, device, backend=None, loss='bpr',
@@ -1125,7 +1165,8 @@ class ShardedImplicitFactorizationModel(object):
     def gathered_net(self):
         """Collective: the trained ``BilinearNet`` on this rank's device, its tables all-gathered from
         the shards (a Bloom model: the representation it was built from, its replicated item bias as
-        it is).  Score it with ``mrr_score`` / ``precision_recall_score``."""
+        it is).  ``mrr_score``, ``precision_recall_score`` and :meth:`predict` score the sharded model
+        itself, on its shards, without gathering it."""
         from spotlight_b200.factorization.representations import BilinearNet
         st, plan = self.state, self.plan
 
@@ -1152,6 +1193,109 @@ class ShardedImplicitFactorizationModel(object):
             Wi_dst.copy_(Wi)
             net.item_biases.weight.copy_(bi)
         return net
+
+    # ------------------------------------------------------------------ evaluation
+    def _hashed_table(self):
+        """Collective: the whole hashed item table (M rows) of a Bloom model, all-gathered."""
+        st = self.state
+        W_full = st.Wi.new_empty((self.world * st.mchunk, st.Wi.shape[1]))
+        dist.all_gather_into_tensor(W_full, st.Wi, group=self.mf.group)
+        return W_full[:st.M]
+
+    def _user_rows(self, users):
+        """Collective: (rows (n, D), biases (n,)) of the global user ids ``users`` (host int64) on every
+        rank.  Each owner writes its users into a zero buffer and one all-reduce sums it: every
+        element has a single non-zero contributor, so the sum is exact."""
+        st, be = self.state, self.backend
+        D = st.Wu.shape[1]
+        buf = torch.zeros((len(users), D + 1), dtype=torch.float32, device=st.Wu.device)
+        mine = np.nonzero((users >= st.ulo) & (users < st.uhi))[0]
+        if len(mine):
+            rows, local = be.to_device(mine.astype(np.int64)), be.to_device((users[mine] - st.ulo).astype(np.int64))
+            buf[rows, :D] = st.Wu[local]
+            buf[rows, D] = st.bu[local]
+        dist.all_reduce(buf, group=self.mf.group)
+        return buf[:, :D].contiguous(), buf[:, D].contiguous()
+
+    def _check_ids(self, users, items):
+        """ValueError, raised on every rank before any collective (all ranks hold the same ids)."""
+        if len(users) and (users.min() < 0 or users.max() >= self._num_users):
+            raise ValueError('User ids must lie in [0, %d), the model\'s number of users.' % self._num_users)
+        if len(items) and (items.min() < 0 or items.max() >= self._num_items):
+            raise ValueError('Item ids must lie in [0, %d), the model\'s number of items.' % self._num_items)
+
+    def _eval_blocks(self, test, train, user_block):
+        """Collective: yields (first output row, CSR test rows of the block, (3, n_targets) int64 counts
+        gt, eq, eq_before over all items) for every block of ``user_block`` users with test items.
+
+        Per block: the user rows are all-reduced, each rank scores them against its item range, pushes
+        the train items inside the range to the bottom, and the targets' scores (written by their
+        owners) and then the rank counts of every range are all-reduced."""
+        be, group = self.backend, self.mf.group
+        test = test.tocsr()
+        train = train.tocsr() if train is not None else None
+        for m in (test, train):
+            if m is not None:
+                self._check_ids(np.nonzero(np.diff(m.indptr))[0], m.indices)
+        ilo, ihi = self.plan.item_range(self.rank)
+        st = self.state
+        if self._net is None:
+            items, item_bias = st.Wi[:ihi - ilo], st.bi[:ihi - ilo]
+        else:
+            ids = torch.arange(ilo, ihi, dtype=torch.int64, device=st.Wi.device)
+            items, item_bias = be.bloom_item_rows(self._hashed_table(), ids, st.item_seeds), st.bi[ilo:ihi]
+        users = np.nonzero(np.diff(test.indptr))[0]
+        for lo in range(0, len(users), user_block):
+            blk = users[lo:lo + user_block]
+            u, ub = self._user_rows(blk)
+            scores = be.shard_scores(u, ub, items, item_bias)
+            if train is not None:
+                tr = train[blk]
+                rows, cols = np.repeat(np.arange(len(blk)), np.diff(tr.indptr)), tr.indices
+                keep = (cols >= ilo) & (cols < ihi)
+                if keep.any():
+                    scores[be.to_device(rows[keep].astype(np.int64)),
+                           be.to_device((cols[keep] - ilo).astype(np.int64))] = -float(np.finfo(np.float32).max)
+            te = test[blk]
+            rows, targets = np.repeat(np.arange(len(blk)), np.diff(te.indptr)), te.indices.astype(np.int64)
+            target_scores = torch.zeros(len(targets), dtype=torch.float32, device=scores.device)
+            own = np.nonzero((targets >= ilo) & (targets < ihi))[0]
+            if len(own):
+                target_scores[be.to_device(own.astype(np.int64))] = scores[be.to_device(rows[own].astype(np.int64)),
+                                                                           be.to_device(targets[own] - ilo)]
+            dist.all_reduce(target_scores, group=group)
+            counts = be.rank_counts(scores, ilo, te.indptr, targets, target_scores)
+            dist.all_reduce(counts, group=group)
+            yield lo, te, counts.cpu().numpy().astype(np.int64)
+
+    def predict(self, user_ids, item_ids=None):
+        """Collective: scores of (user, item) pairs, or of one user against ``item_ids`` (all items when
+        None), as a NumPy array on every rank -- ``ImplicitFactorizationModel.predict``'s arguments and
+        result.  Every rank calls it with the same ids.  Each pair is scored by the rank that owns its
+        item, from the all-reduced user rows; the zero-filled outputs are all-reduced.  The model must
+        be current: ``fit()`` brings every lazily updated row up to date before it returns."""
+        from spotlight_b200.factorization._components import _predict_process_ids
+        st, be = self.state, self.backend
+        users, items = _predict_process_ids(user_ids, item_ids, self._num_items, False)
+        users, items = users.numpy(), items.numpy()
+        self._check_ids(users, items)
+        uniq, inverse = np.unique(users, return_inverse=True)
+        U, ub = self._user_rows(uniq)
+        W_full = None if self._net is None else self._hashed_table()
+        ilo, ihi = self.plan.item_range(self.rank)
+        own = np.nonzero((items >= ilo) & (items < ihi))[0]
+        out = torch.zeros(len(items), dtype=torch.float32, device=st.Wu.device)
+        if len(own):
+            u_idx = be.to_device(inverse.reshape(-1)[own].astype(np.int64))
+            if W_full is None:
+                s = be.pair_scores(U, ub, st.Wi, st.bi, u_idx, be.to_device(items[own] - ilo))
+            else:
+                ids = be.to_device(items[own])
+                s = be.pair_scores(U, ub, be.bloom_item_rows(W_full, ids, st.item_seeds), st.bi[ids], u_idx,
+                                   torch.arange(len(own), dtype=torch.int64, device=out.device))
+            out[be.to_device(own.astype(np.int64))] = s
+        dist.all_reduce(out, group=self.mf.group)
+        return out.cpu().numpy()
 
     def fit(self, interactions, verbose=False):
         be = self.backend
@@ -1511,3 +1655,54 @@ class ShardedBloomMF(object):
             be.bias_sparse_adagrad(ids_all, g_all, st.bi, st.sbi, st.lr, st.eps)
         self.stats['bytes_exchanged'] += (W_full.numel() + dW_pad.numel()) * 4 + P * cap * 12
         return _global_loss(loss_share, self.group)
+
+
+# ---------------------------------------------------------------- evaluation on the item shards
+
+def _finalize_ranks(counts):
+    """(average rank as float64 of its float32 value, stable position int64) from the all-reduced
+    (3, n) counts gt, eq, eq_before: the float32 expression of rank_targets_kernel's rt_write
+    (csrc/embed.cu), so that equal counts give slb_rank_targets' ranks bit for bit."""
+    gt, eq, eq_before = counts
+    avg = np.float32(1.0) + gt.astype(np.float32) + np.float32(0.5) * (eq - 1).astype(np.float32)
+    return avg.astype(np.float64), gt + eq_before
+
+
+def sharded_mrr_score(model, test, train=None, user_block=2048):
+    """Collective ``evaluation.mrr_score`` of a :class:`ShardedImplicitFactorizationModel`: every rank
+    calls it with the same arguments and gets the whole result.  Each rank ranks the test targets
+    among its own item range (:meth:`ShardedImplicitFactorizationModel._eval_blocks`); the summed
+    counts are those of the whole score row, so the result equals the single-GPU scorer's on the
+    same tables, ties included, wherever the per-range GEMM reproduces the full GEMM's scores."""
+    from spotlight_b200.interactions import _to_host
+    test, train = _to_host(test), None if train is None else _to_host(train)
+    n_users = int((np.diff(test.tocsr().indptr) > 0).sum())
+    out = np.empty(n_users, dtype=np.float64)
+    for lo, te, counts in model._eval_blocks(test, train, user_block):
+        ranks, _ = _finalize_ranks(counts)
+        n_per = np.diff(te.indptr)
+        sums = np.add.reduceat(1.0 / ranks, te.indptr[:-1])
+        out[lo:lo + len(n_per)] = sums / n_per
+    return out
+
+
+def sharded_precision_recall_score(model, test, train=None, k=10, user_block=2048):
+    """Collective ``evaluation.precision_recall_score`` of a :class:`ShardedImplicitFactorizationModel`
+    (see :func:`sharded_mrr_score`): precision = hits / min(k, num_items) with the global number of
+    items, recall = hits / the user's number of test items; ties across the k boundary ordered by
+    ascending item id."""
+    from spotlight_b200.evaluation import _hits_at
+    from spotlight_b200.interactions import _to_host
+    test, train = _to_host(test), None if train is None else _to_host(train)
+    ks = np.array([k]) if np.isscalar(k) else np.asarray(k)
+    n_users = int((np.diff(test.tocsr().indptr) > 0).sum())
+    hits = np.empty((n_users, len(ks)), dtype=np.int64)
+    n_test = np.empty(n_users, dtype=np.int64)
+    for lo, te, counts in model._eval_blocks(test, train, user_block):
+        _, pos = _finalize_ranks(counts)
+        n = len(te.indptr) - 1
+        hits[lo:lo + n] = _hits_at(pos, te.indptr, ks)
+        n_test[lo:lo + n] = np.diff(te.indptr)
+    precision = hits / np.minimum(ks, model._num_items).reshape(1, -1).astype(np.float64)
+    recall = hits / n_test.reshape(-1, 1).astype(np.float64)
+    return precision.squeeze(), recall.squeeze()
