@@ -42,20 +42,16 @@ import torch
 import torch.optim as optim
 
 from spotlight_b200 import _lib, ops
+from spotlight_b200.factorization import implicit
 from spotlight_b200.factorization._components import _predict_process_ids
-from spotlight_b200.factorization.implicit import (_NO_CPU, DEVICE_SHUFFLE_MIN, _plan_stream, _side_stream,
-                                                   _to_device_narrow)
+from spotlight_b200.factorization.implicit import (_NO_CPU, DEVICE_SHUFFLE_MIN, _fused_optimizer, _plan_stream,
+                                                   _side_stream, _to_device_narrow)
 from spotlight_b200.factorization.representations import BilinearNet
 from spotlight_b200.helpers import _repr_model
 from spotlight_b200.losses import logistic_loss, poisson_loss, regression_loss
 from spotlight_b200.rng import (SHUFFLE_DEVICE_MAX, permute_ids, shuffle_begin, shuffle_end,
                                 shuffled_order_device)
 from spotlight_b200.torch_utils import cpu, gpu, minibatch, set_seed, shuffled_order
-
-
-# route fused SGD / Adagrad epochs through the planned two-kernel step (csrc/mf_v2.cuh) in its one-term
-# mode; False selects the first-generation step (the reference the planned step is tested against)
-PLANNED_STEP = True
 
 
 class ExplicitFactorizationModel(object):
@@ -254,56 +250,21 @@ class ExplicitFactorizationModel(object):
     def _fit_epoch_pipeline(self, users, items, ratings):
         """One ``slb_mf_fit_epoch`` call enqueues every minibatch step (fused optimizer,
         compact gradients); returns the mean of the per-batch losses (explicit.py:231,236)."""
-        net, opt = self._net, self._optimizer
+        net = self._net
         lib = _lib.load()
         n, B = users.numel(), int(self._batch_size)
-        Wu, Wi = net.user_embeddings.weight, net.item_embeddings.weight
-        bu, bi = net.user_biases.weight, net.item_biases.weight
-        dev = Wu.device
+        params = (net.user_embeddings.weight, net.item_embeddings.weight, net.user_biases.weight,
+                  net.item_biases.weight)
+        dev = params[0].device
+        n_steps = (n + B - 1) // B
         with torch.no_grad():
-            a = ops.mf_step_args(Wu, Wi, bu, bi, users, items, None, self._loss, 1,
-                                 batch=min(B, n), ratings=ratings)
-            a.grad_mode = _lib.GRAD_COMPACT
-            # planned two-kernel step in one-term mode (csrc/mf_v2.cuh) for fused SGD / Adagrad at the
-            # dims it supports; otherwise (lazy Adam, other D) the first-generation compact step
-            fused_need = 0
-            if PLANNED_STEP and opt.fused_kind != _lib.OPT_ADAM:
-                fused_need = lib.slb_mf_fused_workspace_bytes(a.batch, a.num_users, a.num_items, a.dim)
-            if fused_need:
-                fws = ops.workspace('mfv2_%d_%d_%d' % (a.num_users, a.num_items, a.dim), fused_need, dev)
-                a.fused_workspace, a.fused_workspace_bytes = fws.data_ptr(), fws.numel()
+            kind, hp, states, adam = _fused_optimizer(self._optimizer, params, n_steps, dev)
+            # the planned step runs in its one-term mode (csrc/mf_v2.cuh)
+            a, ws, keep = ops.mf_fused_step_args(*params, users, items, None, self._loss, 1, kind, hp, states,
+                                                 batch=min(B, n), ratings=ratings, adam=adam,
+                                                 planned=implicit.PLANNED_STEP)
+            if a.fused_workspace:
                 a.plan_stream = _plan_stream(dev).cuda_stream
-                keep = [fws]
-            else:
-                rows = lib.slb_mf_compact_rows(a.batch, 1, a.loss, 0)
-                D = a.dim
-                keep = [torch.empty(rows, dtype=torch.int64, device=dev), torch.empty(rows, dtype=torch.int64, device=dev),
-                        torch.empty((rows, D), dtype=torch.float32, device=dev),
-                        torch.empty((rows, D), dtype=torch.float32, device=dev),
-                        torch.empty(rows, dtype=torch.float32, device=dev),
-                        torch.empty(rows, dtype=torch.float32, device=dev),
-                        torch.zeros(2, dtype=torch.int32, device=dev)]
-                a.urows, a.irows, a.gWu, a.gWi, a.gbu, a.gbi, a.compact_counts = [t.data_ptr() for t in keep]
-            hp = opt.fused_hparams()
-            a.opt, a.lr, a.weight_decay, a.eps = opt.fused_kind, hp['lr'], hp['weight_decay'], hp['eps']
-            n_steps = (n + B - 1) // B
-            if opt.fused_kind == _lib.OPT_ADAGRAD:
-                states = [opt.fused_state(p) for p in (Wu, Wi, bu, bi)]
-                a.state_Wu, a.state_Wi, a.state_bu, a.state_bi = [s.data_ptr() for s in states]
-            elif opt.fused_kind == _lib.OPT_ADAM:
-                states = [opt.fused_states(p) for p in (Wu, Wi, bu, bi)]
-                a.state_Wu, a.state_Wi, a.state_bu, a.state_bi = [s[0].data_ptr() for s in states]
-                a.state2_Wu, a.state2_Wi, a.state2_bu, a.state2_bi = [s[1].data_ptr() for s in states]
-                a.last_u, a.last_i = states[0][2].data_ptr(), states[1][2].data_ptr()
-                a.beta1, a.beta2 = hp['beta1'], hp['beta2']
-                a.one_minus_beta1, a.one_minus_beta2 = 1.0 - hp['beta1'], 1.0 - hp['beta2']
-                sched = opt.schedule(opt.steps_taken + n_steps, dev)
-                keep.append(sched)
-                a.adam_sched, a.adam_step = sched.data_ptr(), opt.steps_taken + 1
-                opt.advance(n_steps)
-            need = lib.slb_mf_step_workspace_bytes(a.batch, 1, a.loss, a.num_users, a.num_items)
-            ws = ops.workspace('mf%d_%d' % (a.num_users, a.num_items), need, dev)
-            a.workspace, a.workspace_bytes = ws.data_ptr(), ws.numel()
             losses = torch.empty(n_steps, dtype=torch.float32, device=dev)
             rc = lib.slb_mf_fit_epoch(ctypes.byref(a), ops._ptr(users), ops._ptr(items), None, n,
                                       ops._ptr(losses), ops._stream())

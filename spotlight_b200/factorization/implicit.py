@@ -61,6 +61,24 @@ def _plan_stream(device):
     return _PLAN_STREAMS[key]
 
 
+def _fused_optimizer(opt, params, n_steps, device, own_last=False):
+    """(opt_kind, hparams, states, adam) of a fused optimizer for ``n_steps`` fused steps on the
+    four tables ``params``, in the form ops.mf_fused_step_args takes.  Adagrad's states are its sums;
+    lazy-exact Adam's are (exp_avg, exp_avg_sq, last) (``own_last``: every table with its own
+    ``last``, else the bias shares its embedding's), with ``adam`` = dict(beta1, beta2, sched,
+    step (the first of the ``n_steps``)); the steps are counted here."""
+    hp = opt.fused_hparams()
+    states, adam = None, None
+    if opt.fused_kind == _lib.OPT_ADAGRAD:
+        states = [opt.fused_state(p) for p in params]
+    elif opt.fused_kind == _lib.OPT_ADAM:
+        states = [opt.fused_states(p, own_last=own_last) for p in params]
+        adam = dict(beta1=hp['beta1'], beta2=hp['beta2'], sched=opt.schedule(opt.steps_taken + n_steps, device),
+                    step=opt.steps_taken + 1)
+        opt.advance(n_steps)
+    return opt.fused_kind, hp, states, adam
+
+
 def _to_device_ids(ids, device):
     """Host id array -> int64 CUDA tensor (narrow on the wire, widened on the device)."""
     return _to_device_narrow(ids, device).long()
@@ -81,9 +99,9 @@ def _to_device_narrow(ids, device):
     return host.to(device, non_blocking=host.is_pinned())     # page-locked callers get an async DMA
 
 
-# route pointwise / bpr / hinge epochs through the planned two-kernel step (csrc/mf_v2.cuh);
-# False selects the first-generation step (kept for A/B measurements and as the reference
-# implementation of the compact-gradient mode)
+# route the implicit and explicit models' epochs through the planned two-kernel step
+# (csrc/mf_v2.cuh) wherever ops.v2_eligible allows; False selects the first-generation step
+# (kept for A/B measurements and as the reference implementation of the compact-gradient mode)
 PLANNED_STEP = True
 
 # epochs at least this long take their permutation from the device shuffle (csrc/shuffle.cu);
@@ -363,62 +381,20 @@ class ImplicitFactorizationModel(object):
     def _fit_epoch_pipeline(self, users, items, negatives, sync=True, waits=()):
         """One C call enqueues every minibatch step of ``users``/``items``; returns the
         device tensor of per-batch losses (``sync=False``) or their mean."""
-        net, opt = self._net, self._optimizer
+        net = self._net
         lib = _lib.load()
         n, B, n_neg = users.numel(), int(self._batch_size), self._n_neg()
-        Wu, Wi = net.user_embeddings.weight, net.item_embeddings.weight
-        bu, bi = net.user_biases.weight, net.item_biases.weight
-        dev = Wu.device
+        params = (net.user_embeddings.weight, net.item_embeddings.weight, net.user_biases.weight,
+                  net.item_biases.weight)
+        dev = params[0].device
+        n_steps = (n + B - 1) // B
         with torch.no_grad():
-            a = ops.mf_step_args(Wu, Wi, bu, bi, users, items, negatives, self._loss, n_neg,
-                                 batch=min(B, n))
-            a.grad_mode = _lib.GRAD_COMPACT
-            # planned two-kernel step (plan + user kernel + item kernel, csrc/mf_v2.cuh) whenever the
-            # library supports the shape; otherwise the first-generation step with compact gradients
-            fused_need = 0
-            if self._loss != 'adaptive_hinge' and PLANNED_STEP and opt.fused_kind != _lib.OPT_ADAM:
-                fused_need = lib.slb_mf_fused_workspace_bytes(a.batch, a.num_users, a.num_items, a.dim)
-            if fused_need:
-                fws = ops.workspace('mfv2_%d_%d_%d' % (a.num_users, a.num_items, a.dim),
-                                    fused_need, dev)
-                a.fused_workspace, a.fused_workspace_bytes = fws.data_ptr(), fws.numel()
-                if not os.environ.get('SLB_PLAN_SAME_STREAM'):      # A/B switch for measurements
-                    a.plan_stream = _plan_stream(dev).cuda_stream
-                keep = (fws,)
-            else:
-                rows = lib.slb_mf_compact_rows(a.batch, n_neg, a.loss, 0)
-                D = a.dim
-                urows = torch.empty(rows, dtype=torch.int64, device=dev)
-                irows = torch.empty(rows, dtype=torch.int64, device=dev)
-                gWu = torch.empty((rows, D), dtype=torch.float32, device=dev)
-                gWi = torch.empty((rows, D), dtype=torch.float32, device=dev)
-                gbu = torch.empty(rows, dtype=torch.float32, device=dev)
-                gbi = torch.empty(rows, dtype=torch.float32, device=dev)
-                counts = torch.zeros(2, dtype=torch.int32, device=dev)
-                a.urows, a.gWu, a.gbu = urows.data_ptr(), gWu.data_ptr(), gbu.data_ptr()
-                a.irows, a.gWi, a.gbi = irows.data_ptr(), gWi.data_ptr(), gbi.data_ptr()
-                a.compact_counts = counts.data_ptr()
-                keep = (urows, irows, gWu, gWi, gbu, gbi, counts)
-            hp = opt.fused_hparams()
-            a.opt, a.lr, a.weight_decay, a.eps = opt.fused_kind, hp['lr'], hp['weight_decay'], hp['eps']
-            n_steps = (n + B - 1) // B
-            if opt.fused_kind == _lib.OPT_ADAGRAD:
-                states = [opt.fused_state(p) for p in (Wu, Wi, bu, bi)]
-                a.state_Wu, a.state_Wi, a.state_bu, a.state_bi = [s.data_ptr() for s in states]
-            elif opt.fused_kind == _lib.OPT_ADAM:
-                states = [opt.fused_states(p) for p in (Wu, Wi, bu, bi)]
-                a.state_Wu, a.state_Wi, a.state_bu, a.state_bi = [s[0].data_ptr() for s in states]
-                a.state2_Wu, a.state2_Wi, a.state2_bu, a.state2_bi = [s[1].data_ptr() for s in states]
-                a.last_u, a.last_i = states[0][2].data_ptr(), states[1][2].data_ptr()
-                a.beta1, a.beta2 = hp['beta1'], hp['beta2']
-                a.one_minus_beta1, a.one_minus_beta2 = 1.0 - hp['beta1'], 1.0 - hp['beta2']
-                sched = opt.schedule(opt.steps_taken + n_steps, dev)
-                a.adam_sched, a.adam_step = sched.data_ptr(), opt.steps_taken + 1
-                opt.advance(n_steps)
-            need = lib.slb_mf_step_workspace_bytes(a.batch, n_neg, a.loss, a.num_users, a.num_items)
-            ws = ops.workspace('mf%d_%d' % (a.num_users, a.num_items), need, dev)
-            a.workspace, a.workspace_bytes = ws.data_ptr(), ws.numel()
-            n_steps = (n + B - 1) // B
+            kind, hp, states, adam = _fused_optimizer(self._optimizer, params, n_steps, dev)
+            a, ws, keep = ops.mf_fused_step_args(*params, users, items, negatives, self._loss, n_neg, kind, hp,
+                                                 states, batch=min(B, n), adam=adam, planned=PLANNED_STEP)
+            # the planned step's integer plan runs one step ahead on its own stream
+            if a.fused_workspace and not os.environ.get('SLB_PLAN_SAME_STREAM'):    # A/B switch for measurements
+                a.plan_stream = _plan_stream(dev).cuda_stream
             losses = torch.empty(n_steps, dtype=torch.float32, device=dev)
             # steps wait (on the device) for the event of the chunk of negatives they read
             w_steps = (ctypes.c_int64 * max(1, len(waits)))(*[int(k) for k, _ in waits])
@@ -440,20 +416,13 @@ class ImplicitFactorizationModel(object):
         (csrc/mf.cu slb_mf_bloom_train_step, fused mode), no dense gradient of any table.  Under
         ``FusedAdam`` the step is lazy-exact Adam: each of the four tables keeps its own ``last``,
         and the ``flush()`` at the end of ``fit()`` brings every row current."""
-        net, opt = self._net, self._optimizer
+        net = self._net
         spec = net.fused_spec()
         n_neg = self._n_neg()
-        hp = opt.fused_hparams()
         params = (spec['Wu'], spec['Wi'], net.user_biases.weight, net.item_biases.weight)
-        states, adam = None, None
-        if opt.fused_kind == _lib.OPT_ADAGRAD:
-            states = [opt.fused_state(p) for p in params]
-        elif opt.fused_kind == _lib.OPT_ADAM:
-            states = [opt.fused_states(p, own_last=True) for p in params]
-            n_steps = (users.numel() + self._batch_size - 1) // self._batch_size
-            t0 = opt.steps_taken + 1
-            adam = dict(beta1=hp['beta1'], beta2=hp['beta2'], sched=opt.schedule(t0 + n_steps - 1, users.device))
-            opt.advance(n_steps)
+        n_steps = (users.numel() + self._batch_size - 1) // self._batch_size
+        kind, hp, states, adam = _fused_optimizer(self._optimizer, params, n_steps, users.device, own_last=True)
+        t0 = adam['step'] if adam is not None else None
         losses = []
         lo = 0
         for k, (batch_user, batch_item) in enumerate(minibatch(users, items, batch_size=self._batch_size)):
@@ -464,7 +433,7 @@ class ImplicitFactorizationModel(object):
                 adam['step'] = t0 + k
             losses.append(ops.mf_bloom_train_step_inplace(
                 *params, batch_user, batch_item, batch_neg, self._loss, n_neg, spec['user_seeds'],
-                spec['item_seeds'], spec['user_pad'], spec['item_pad'], opt.fused_kind, hp['lr'], states,
+                spec['item_seeds'], spec['user_pad'], spec['item_pad'], kind, hp['lr'], states,
                 hp['weight_decay'], hp['eps'], adam=adam))
         host = torch.stack(losses).cpu().numpy().astype(np.float64)        # one sync per epoch
         return float(host.sum() / len(host))

@@ -315,6 +315,77 @@ def _(Wu, Wi, bu, bi, users, items, negs, loss, n_neg, want_scores):
             torch.empty_like(Wu), torch.empty_like(Wi), torch.empty_like(bu), torch.empty_like(bi))
 
 
+def _adam_scalars(a, beta1, beta2, sched, step):
+    """The lazy-exact Adam scalars of an MF, hashed-table or sequence step's arguments (the structs
+    share the field names): ``1 - beta`` is taken in double, as torch's Python does, and ``sched``
+    is ``FusedAdam.schedule``'s table reaching step ``step``."""
+    b1, b2 = float(beta1), float(beta2)
+    a.beta1, a.beta2, a.one_minus_beta1, a.one_minus_beta2 = b1, b2, 1.0 - b1, 1.0 - b2
+    a.adam_sched, a.adam_step = sched.data_ptr(), int(step)
+
+
+def v2_eligible(a):
+    """Whether the step ``a`` (optimizer filled in) runs the planned two-kernel step (csrc/mf_v2.cuh)
+    once it is given the fused workspace: the host's side of ``v2_eligible`` in csrc/mf.cu.  Adaptive
+    hinge and lazy-exact Adam run the first-generation kernels, and so does a width for which
+    slb_mf_fused_workspace_bytes is 0."""
+    return a.loss != LOSS_KIND['adaptive_hinge'] and a.opt in (_lib.OPT_SGD, _lib.OPT_ADAGRAD)
+
+
+def _mf_workspaces(a, dev, planned=True):
+    """(step workspace, fused workspace) of the step ``a``: the fused one only for the planned step
+    (``planned``, :func:`v2_eligible` and a width the library has one for), else None."""
+    lib = _lib.load()
+    need2 = (lib.slb_mf_fused_workspace_bytes(a.batch, a.num_users, a.num_items, a.dim)
+             if planned and v2_eligible(a) else 0)
+    fws = workspace('mfv2_%d_%d_%d' % (a.num_users, a.num_items, a.dim), need2, dev) if need2 else None
+    ws = workspace('mf%d_%d' % (a.num_users, a.num_items),
+                   lib.slb_mf_step_workspace_bytes(a.batch, a.n_neg, a.loss, a.num_users, a.num_items), dev)
+    return ws, fws
+
+
+def mf_fused_step_args(Wu, Wi, bu, bi, users, items, negs, loss, n_neg, opt_kind, hp, states, batch=None,
+                       ratings=None, adam=None, planned=True):
+    """A filled ``slb_mf_step_args`` for steps with the row-wise optimizer fused in: both tables
+    take their update in place through compact gradients.  ``hp`` = dict(lr, weight_decay, eps)
+    (``fused_hparams()``); ``states`` = Adagrad's (sWu, sWi, sbu, sbi), or under lazy-exact Adam
+    four (exp_avg, exp_avg_sq, last) of (Wu, Wi, bu, bi) with ``adam`` = dict(beta1, beta2, sched,
+    step (the first step, 1-based)).
+
+    The planned step gets its fused workspace when ``planned`` and :func:`v2_eligible` allow and
+    the library has a workspace for the width; otherwise the first-generation step gets its seven
+    compact buffers.  Returns (args, ws, keep): the caller sets ``loss_out`` (and ``plan_stream``)
+    and launches, reads the id-range flag of the workspace ``ws`` (workspace_error_flag), and holds
+    ``keep`` until the launch is enqueued."""
+    lib = _lib.load()
+    dev = Wu.device
+    a = mf_step_args(Wu, Wi, bu, bi, users, items, negs, loss, n_neg, batch=batch, ratings=ratings)
+    a.grad_mode = _lib.GRAD_COMPACT
+    a.opt, a.lr, a.weight_decay, a.eps = int(opt_kind), float(hp['lr']), float(hp['weight_decay']), float(hp['eps'])
+    keep = []
+    if opt_kind == _lib.OPT_ADAGRAD:
+        a.state_Wu, a.state_Wi, a.state_bu, a.state_bi = [t.data_ptr() for t in states]
+    elif opt_kind == _lib.OPT_ADAM:
+        a.state_Wu, a.state_Wi, a.state_bu, a.state_bi = [s[0].data_ptr() for s in states]
+        a.state2_Wu, a.state2_Wi, a.state2_bu, a.state2_bi = [s[1].data_ptr() for s in states]
+        a.last_u, a.last_i = states[0][2].data_ptr(), states[1][2].data_ptr()
+        _adam_scalars(a, adam['beta1'], adam['beta2'], adam['sched'], adam['step'])
+        keep.append(adam['sched'])
+    ws, fws = _mf_workspaces(a, dev, planned)
+    a.workspace, a.workspace_bytes = ws.data_ptr(), ws.numel()
+    if fws is not None:
+        a.fused_workspace, a.fused_workspace_bytes = fws.data_ptr(), fws.numel()
+    else:
+        rows = lib.slb_mf_compact_rows(a.batch, a.n_neg, a.loss, 0)
+        bufs = [torch.empty(rows, dtype=torch.int64, device=dev), torch.empty(rows, dtype=torch.int64, device=dev),
+                torch.empty((rows, a.dim), device=dev), torch.empty((rows, a.dim), device=dev),
+                torch.empty(rows, device=dev), torch.empty(rows, device=dev),
+                torch.zeros(2, dtype=torch.int32, device=dev)]
+        a.urows, a.irows, a.gWu, a.gWi, a.gbu, a.gbi, a.compact_counts = [t.data_ptr() for t in bufs]
+        keep += bufs
+    return a, ws, keep
+
+
 def mf_train_step_inplace(Wu, Wi, bu, bi, users, items, negs, loss, opt_kind, lr, states=None,
                           weight_decay=0.0, eps=1e-10, planned=True, ratings=None):
     """One minibatch with the row-wise optimizer fused in: parameters (and Adagrad ``states`` =
@@ -326,36 +397,16 @@ def mf_train_step_inplace(Wu, Wi, bu, bi, users, items, negs, loss, opt_kind, lr
     Rating losses pass ``negs=None`` and ``ratings`` (spotlight/factorization/explicit.py:223-234).
     """
     require_cuda(Wu, Wi, bu, bi, users, items, negs, ratings)
-    lib = _lib.load()
     users, items = _i64c(users).reshape(-1), _i64c(items).reshape(-1)
     negs = _i64c(negs).reshape(-1) if negs is not None else None
     ratings = _f32c(ratings).reshape(-1) if ratings is not None else None
-    B = users.numel()
-    dev = Wu.device
     with torch.no_grad():
-        a = mf_step_args(Wu, Wi, bu, bi, users, items, negs, loss, 1, ratings=ratings)
-        loss_out = torch.empty(1, dtype=torch.float32, device=dev)
+        a, _, keep = mf_fused_step_args(Wu, Wi, bu, bi, users, items, negs, loss, 1, opt_kind,
+                                        dict(lr=lr, weight_decay=weight_decay, eps=eps), states,
+                                        ratings=ratings, planned=planned)
+        loss_out = torch.empty(1, dtype=torch.float32, device=Wu.device)
         a.loss_out = loss_out.data_ptr()
-        a.grad_mode = _lib.GRAD_COMPACT
-        a.opt, a.lr, a.weight_decay, a.eps = int(opt_kind), float(lr), float(weight_decay), float(eps)
-        if opt_kind == _lib.OPT_ADAGRAD:
-            a.state_Wu, a.state_Wi, a.state_bu, a.state_bi = [t.data_ptr() for t in states]
-        keep = []
-        need2 = lib.slb_mf_fused_workspace_bytes(B, a.num_users, a.num_items, a.dim) if planned else 0
-        if need2 and a.loss != 3:
-            fws = workspace('mfv2_%d_%d_%d' % (a.num_users, a.num_items, a.dim), need2, dev)
-            a.fused_workspace, a.fused_workspace_bytes = fws.data_ptr(), fws.numel()
-        else:
-            rows = lib.slb_mf_compact_rows(B, 1, a.loss, 0)
-            keep = [torch.empty(rows, dtype=torch.int64, device=dev), torch.empty(rows, dtype=torch.int64, device=dev),
-                    torch.empty((rows, a.dim), device=dev), torch.empty((rows, a.dim), device=dev),
-                    torch.empty(rows, device=dev), torch.empty(rows, device=dev),
-                    torch.zeros(2, dtype=torch.int32, device=dev)]
-            a.urows, a.irows, a.gWu, a.gWi, a.gbu, a.gbi, a.compact_counts = [t.data_ptr() for t in keep]
-        need = lib.slb_mf_step_workspace_bytes(B, 1, a.loss, a.num_users, a.num_items)
-        ws = workspace('mf%d_%d' % (a.num_users, a.num_items), need, dev)
-        a.workspace, a.workspace_bytes = ws.data_ptr(), ws.numel()
-        _lib.check(lib.slb_mf_train_step(ctypes.byref(a), _stream()), 'mf_train_step')
+        _lib.check(_lib.load().slb_mf_train_step(ctypes.byref(a), _stream()), 'mf_train_step')
     return loss_out.reshape(())
 
 
@@ -532,9 +583,7 @@ def _bloom_adam_args(x, params, states, adam):
     a.state2_Wu, a.state2_Wi, a.state2_bu, a.state2_bi = [st[1].data_ptr() for st in states]
     a.last_u, a.last_i = states[0][2].data_ptr(), states[1][2].data_ptr()
     x.last_bu, x.last_bi = states[2][2].data_ptr(), states[3][2].data_ptr()
-    b1, b2 = float(adam['beta1']), float(adam['beta2'])
-    a.beta1, a.beta2, a.one_minus_beta1, a.one_minus_beta2 = b1, b2, 1.0 - b1, 1.0 - b2
-    a.adam_sched, a.adam_step = adam['sched'].data_ptr(), step
+    _adam_scalars(a, adam['beta1'], adam['beta2'], adam['sched'], step)
 
 
 def mf_bloom_step_pairs(Wu, Wi, bu, bi, users, items, negs, loss, item_seeds, item_pad, norm_batch=0,
@@ -616,9 +665,7 @@ def _bloom_users_only_args(x, uo):
     a.state_Wu, a.state2_Wu, a.last_u = mWu.data_ptr(), vWu.data_ptr(), last_u.data_ptr()
     a.state_bu, a.state2_bu = mbu.data_ptr(), vbu.data_ptr()
     a.state_bi, a.state2_bi, x.last_bi = mbi.data_ptr(), vbi.data_ptr(), last_bi.data_ptr()
-    b1, b2 = float(uo['beta1']), float(uo['beta2'])
-    a.beta1, a.beta2, a.one_minus_beta1, a.one_minus_beta2 = b1, b2, 1.0 - b1, 1.0 - b2
-    a.adam_sched, a.adam_step = uo['sched'].data_ptr(), step
+    _adam_scalars(a, uo['beta1'], uo['beta2'], uo['sched'], step)
 
 
 def bias_sparse_adam(ids, g, bias, exp_avg, exp_avg_sq, last, sched, step, beta1, beta2, eps, weight_decay):
@@ -967,12 +1014,10 @@ def _seq_adam_args(a, fused, E, bias):
             raise ValueError('seq_train_step: Adam `last` must be contiguous int32 with one entry per row')
     if fused['sched'].numel() < 2 * (int(fused['step']) + 1):
         raise ValueError('seq_train_step: the Adam schedule does not reach step %d' % int(fused['step']))
-    b1, b2 = float(fused['beta1']), float(fused['beta2'])
-    a.beta1, a.beta2, a.one_minus_beta1, a.one_minus_beta2 = b1, b2, 1.0 - b1, 1.0 - b2
+    _adam_scalars(a, fused['beta1'], fused['beta2'], fused['sched'], fused['step'])
     a.state2_E, a.state2_bias = fused['state2_E'].data_ptr(), fused['state2_bias'].data_ptr()
     a.last_E = fused['last_E'].data_ptr()
     a.last_bias = last_bias.data_ptr() if last_bias is not None else None
-    a.adam_sched, a.adam_step = fused['sched'].data_ptr(), int(fused['step'])
 
 
 def seq_train_step(E, bias, seqs, negs, loss, n_neg, cnn=None, want_scores=False, norm_count=None, fused=None,

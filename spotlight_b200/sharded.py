@@ -61,6 +61,39 @@ class ShardPlan(object):
         return user_ids // self.uchunk
 
 
+def _users_only_args(st, W, b, users, items, negs, loss, n_neg, dWi, dbi, norm_batch, batch=None, t=None,
+                     workspaces=None):
+    """A filled ``slb_mf_step_args`` in the step's users-only mode: the user shard's rows and biases
+    take their row-wise Adagrad step in place (under ``st.opt`` lazy-exact Adam step ``t``: the
+    referenced user rows catch up through t - 1, the touched ones take step t), while the item rows
+    ``W`` / ``b`` stay as they are and their gradient goes to the zeroed dense ``dWi`` / ``dbi``
+    for the owners; loss and gradients are normalised by ``norm_batch``.  The planned step
+    (csrc/mf_v2.cuh) gets the fused workspace where ops.v2_eligible allows.
+
+    ``workspaces``: the (step, fused) workspaces of the stream the step runs on, for a caller that
+    fills the arguments on another stream (``ops.workspace`` is per stream); by default the current
+    stream's, the fused one only for the planned step.  The caller sets ``loss_out`` and launches."""
+    dev = st.Wu.device
+    a = ops.mf_step_args(st.Wu, W, st.bu, b, users, items, negs, loss, n_neg, batch=batch)
+    a.grad_mode = _lib.GRAD_DENSE
+    a.dWi, a.dbi = dWi.data_ptr(), dbi.data_ptr()
+    a.norm_batch, a.opt_users_only = int(norm_batch), 1
+    if st.opt is not None:
+        hp = st.opt.fused_hparams()
+        a.opt, a.lr, a.weight_decay, a.eps = _lib.OPT_ADAM, hp['lr'], hp['weight_decay'], hp['eps']
+        a.state_Wu, a.state_bu = st.mWu.data_ptr(), st.mbu.data_ptr()
+        a.state2_Wu, a.state2_bu, a.last_u = st.vWu.data_ptr(), st.vbu.data_ptr(), st.last_u.data_ptr()
+        ops._adam_scalars(a, hp['beta1'], hp['beta2'], st.opt.schedule(t, dev), t)
+    else:
+        a.opt, a.lr, a.weight_decay, a.eps = _lib.OPT_ADAGRAD, st.lr, 0.0, st.eps
+        a.state_Wu, a.state_bu = st.sWu.data_ptr(), st.sbu.data_ptr()
+    ws, fws = workspaces if workspaces is not None else ops._mf_workspaces(a, dev)
+    a.workspace, a.workspace_bytes = ws.data_ptr(), ws.numel()
+    if fws is not None and ops.v2_eligible(a):
+        a.fused_workspace, a.fused_workspace_bytes = fws.data_ptr(), fws.numel()
+    return a
+
+
 class GpuBackend(object):
     """The compute pieces of the sharded step on the product's CUDA kernels."""
 
@@ -100,43 +133,14 @@ class GpuBackend(object):
         """Fused forward/backward on (user shard, row cache).  Updates the user
         shard in place (row-wise Adagrad; under ``st.opt``, lazy-exact Adam step ``t``); returns
         (loss share, d cache rows, d cache bias)."""
-        lib = _lib.load()
         cap, D = cache_rows.shape
-        a = ops.mf_step_args(st.Wu, cache_rows, st.bu, cache_bias, users_local, pos_idx, neg_idx,
-                             loss, n_neg)
         loss_out = torch.empty(1, dtype=torch.float32, device=self.device)
         dWi = torch.zeros((cap, D), dtype=torch.float32, device=self.device)
         dbi = torch.zeros(cap, dtype=torch.float32, device=self.device)
+        a = _users_only_args(st, cache_rows, cache_bias, users_local, pos_idx, neg_idx, loss, n_neg, dWi, dbi,
+                             global_batch, t=t)
         a.loss_out = loss_out.data_ptr()
-        a.grad_mode = _lib.GRAD_DENSE
-        a.dWi, a.dbi = dWi.data_ptr(), dbi.data_ptr()
-        a.norm_batch, a.opt_users_only = int(global_batch), 1
-        if st.opt is not None:
-            # users-only lazy-exact Adam (first-generation step): the referenced user rows catch up
-            # through t - 1, the touched ones take step t; the cache rows' owners keep their state
-            sched = st.opt.schedule(t, self.device)
-            hp = st.opt.fused_hparams()
-            a.opt, a.lr, a.weight_decay, a.eps = _lib.OPT_ADAM, hp['lr'], hp['weight_decay'], hp['eps']
-            a.beta1, a.beta2 = hp['beta1'], hp['beta2']
-            a.one_minus_beta1, a.one_minus_beta2 = 1.0 - hp['beta1'], 1.0 - hp['beta2']
-            a.state_Wu, a.state_bu = st.mWu.data_ptr(), st.mbu.data_ptr()
-            a.state2_Wu, a.state2_bu, a.last_u = st.vWu.data_ptr(), st.vbu.data_ptr(), st.last_u.data_ptr()
-            a.adam_sched, a.adam_step = sched.data_ptr(), int(t)
-        else:
-            a.opt, a.lr, a.weight_decay, a.eps = _lib.OPT_ADAGRAD, st.lr, 0.0, st.eps
-            a.state_Wu, a.state_bu = st.sWu.data_ptr(), st.sbu.data_ptr()
-        need = lib.slb_mf_step_workspace_bytes(a.batch, n_neg, a.loss, a.num_users, a.num_items)
-        ws = ops.workspace('mf%d_%d' % (a.num_users, a.num_items), need, self.device)
-        a.workspace, a.workspace_bytes = ws.data_ptr(), ws.numel()
-        # planned two-kernel step (csrc/mf_v2.cuh): user rows updated in place, the item kernel
-        # hands the dense cache-row gradient out for the owners (Adagrad only)
-        need2 = (lib.slb_mf_fused_workspace_bytes(a.batch, a.num_users, a.num_items, a.dim)
-                 if n_neg == 1 and st.opt is None else 0)
-        if need2:
-            fws = ops.workspace('mfv2_%d_%d_%d' % (a.num_users, a.num_items, a.dim), need2,
-                                self.device)
-            a.fused_workspace, a.fused_workspace_bytes = fws.data_ptr(), fws.numel()
-        _lib.check(lib.slb_mf_train_step(ctypes.byref(a), ops._stream()), 'mf_train_step')
+        _lib.check(_lib.load().slb_mf_train_step(ctypes.byref(a), ops._stream()), 'mf_train_step')
         return loss_out.reshape(()), dWi[:n_cache], dbi[:n_cache]
 
     def owner_update(self, st, local_ids, g_rows, g_bias):
@@ -1442,18 +1446,11 @@ class ShardedImplicitFactorizationModel(object):
         next_wait = [0]
 
         def make_args(k):
-            slot = k & 1
-            m = bounds[k + 1] - bounds[k]
-            ul, it, ng = buf['ids'][slot]
-            a = ops.mf_step_args(st.Wu, buf['full_W'], st.bu, buf['full_b'], ul, it, ng, loss_kind, 1, batch=m)
+            # runs on the plan stream: the workspaces are the main stream's, which the step reads
+            ul, it, ng = buf['ids'][k & 1]
+            a = _users_only_args(st, buf['full_W'], buf['full_b'], ul, it, ng, loss_kind, 1, buf['dW'], buf['db'],
+                                 min(B, n - k * B), batch=bounds[k + 1] - bounds[k], workspaces=(ws, fws))
             a.loss_out = losses[k:k + 1].data_ptr()
-            a.grad_mode = _lib.GRAD_DENSE
-            a.dWi, a.dbi = buf['dW'].data_ptr(), buf['db'].data_ptr()
-            a.opt, a.lr, a.weight_decay, a.eps = _lib.OPT_ADAGRAD, st.lr, 0.0, st.eps
-            a.state_Wu, a.state_bu = st.sWu.data_ptr(), st.sbu.data_ptr()
-            a.norm_batch, a.opt_users_only = int(min(B, n - k * B)), 1
-            a.workspace, a.workspace_bytes = ws.data_ptr(), ws.numel()
-            a.fused_workspace, a.fused_workspace_bytes = fws.data_ptr(), fws.numel()
             return a
 
         def prep(k):
