@@ -32,7 +32,7 @@ EXPORTS = (
     'slb_shuffle_workspace_bytes', 'slb_shuffle_order', 'slb_permute_ids',
     'slb_embedding_forward', 'slb_bloom_rows',
     'slb_embedding_backward_workspace_bytes', 'slb_embedding_backward',
-    'slb_mf_scores', 'slb_mf_scores_backward', 'slb_rank_pairs', 'slb_rank_targets', 'slb_rank_counts', 'slb_mixture_scores', 'slb_mf_step_workspace_bytes', 'slb_mf_fused_workspace_bytes', 'slb_mf_compact_rows',
+    'slb_mf_scores', 'slb_mf_scores_backward', 'slb_rank_pairs', 'slb_rank_targets', 'slb_rank_counts', 'slb_shard_mask_targets', 'slb_mixture_scores', 'slb_mf_step_workspace_bytes', 'slb_mf_fused_workspace_bytes', 'slb_mf_compact_rows',
     'slb_mf_train_step', 'slb_mf_train_step_phases', 'slb_mf_fit_epoch', 'slb_mf_fit_epoch_events', 'slb_adam_flush',
     'slb_adam_flush_table', 'slb_adam_dense', 'slb_adam_dense_table', 'slb_bias_sparse_adam',
     'slb_mf_bloom_workspace_bytes', 'slb_mf_bloom_train_step',
@@ -153,6 +153,7 @@ def _declare(lib):
     lib.slb_rank_pairs.argtypes = [c_vp, c_i64, c_i64, c_vp, c_vp, c_i64, c_vp, c_vp]
     lib.slb_rank_targets.argtypes = [c_vp, c_i64, c_i64, c_vp, c_vp, c_i64, c_vp, c_vp, c_vp]
     lib.slb_rank_counts.argtypes = [c_vp, c_i64, c_i64, c_i64, c_vp, c_vp, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp]
+    lib.slb_shard_mask_targets.argtypes = [c_vp, c_i64, c_i64, c_i64, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp]
     lib.slb_mixture_scores.argtypes = [c_vp, c_i64, c_i32, c_i32, c_vp, c_vp, c_i64, c_vp, c_vp]
     lib.slb_mf_step_workspace_bytes.argtypes = [c_i64, c_i32, c_i32, c_i64, c_i64]
     lib.slb_mf_step_workspace_bytes.restype = c_sz

@@ -6,6 +6,8 @@
 // aten::embedding_dense_backward.  Bloom hashes are computed in registers
 // (murmur3 of the id, layers.py:178-204) instead of reading the reference's
 // 8*H bytes/id hash table.
+#include <cfloat>
+
 #include "segindex.cuh"
 
 namespace {
@@ -475,6 +477,33 @@ rank_targets_kernel(const float* __restrict__ scores, int64_t n_rows, int64_t n_
     }
 }
 
+// The shard-local step between scoring and counting in the sharded sequence scorers: one CTA per
+// row of the block [n_rows, n_cols] (the global items [col0, col0 + n_cols)) first writes -FLT_MAX
+// over the row's excluded items that fall in the block (repeated ids write the same value), then,
+// once those writes are visible to the CTA, reads every target's score when the target is in the
+// block and 0 otherwise, so that summing the ranks' target_scores gives each target's score.
+constexpr int MT_THREADS = 128;
+
+__global__ void __launch_bounds__(MT_THREADS)
+shard_mask_targets_kernel(float* scores, int64_t n_rows, int64_t n_cols, int64_t col0,
+                          const int64_t* __restrict__ excluded, int64_t n_excl,
+                          const int64_t* __restrict__ row_ptr, const int64_t* __restrict__ targets,
+                          float* __restrict__ target_scores) {
+    for (int64_t r = blockIdx.x; r < n_rows; r += gridDim.x) {
+        float* row = scores + r * n_cols;
+        for (int64_t j = threadIdx.x; j < n_excl; j += MT_THREADS) {
+            const int64_t c = __ldg(excluded + r * n_excl + j) - col0;
+            if (c >= 0 && c < n_cols) row[c] = -FLT_MAX;
+        }
+        __syncthreads();
+        const int64_t t1 = __ldg(row_ptr + r + 1);
+        for (int64_t p = __ldg(row_ptr + r) + threadIdx.x; p < t1; p += MT_THREADS) {
+            const int64_t c = __ldg(targets + p) - col0;
+            target_scores[p] = (c >= 0 && c < n_cols) ? row[c] : 0.f;
+        }
+    }
+}
+
 }  // namespace
 
 extern "C" {
@@ -520,6 +549,25 @@ int slb_rank_counts(const float* scores, int64_t n_rows, int64_t n_cols, int64_t
     rank_targets_kernel<<<grid, RT_THREADS, 0, st>>>(scores, n_rows, n_cols, row_ptr, targets,
                                                      RankCounts{target_scores, col_offset, gt, eq, eq_before});
     SLB_LAUNCH_CHECK("rank_targets_kernel");
+    return SLB_OK;
+}
+
+int slb_shard_mask_targets(float* scores, int64_t n_rows, int64_t n_cols, int64_t col_offset,
+                           const int64_t* excluded, int64_t n_excluded_per_row, const int64_t* row_ptr,
+                           const int64_t* targets, float* target_scores, slb_stream_t stream) {
+    SLB_REQUIRE(n_rows >= 0 && n_excluded_per_row >= 0, "shard_mask_targets: n_rows = %lld, excluded per row = %lld",
+                static_cast<long long>(n_rows), static_cast<long long>(n_excluded_per_row));
+    SLB_REQUIRE(n_cols >= 0 && n_cols <= INT32_MAX && col_offset >= 0 && col_offset <= INT32_MAX - n_cols,
+                "shard_mask_targets: columns [%lld, %lld + %lld) outside [0, INT32_MAX]",
+                static_cast<long long>(col_offset), static_cast<long long>(col_offset), static_cast<long long>(n_cols));
+    if (n_rows == 0) return SLB_OK;
+    SLB_REQUIRE(row_ptr && targets && target_scores && (scores || n_cols == 0) && (excluded || n_excluded_per_row == 0),
+                "shard_mask_targets: null pointer");
+    const int64_t cap = static_cast<int64_t>(slb_sms()) * 8;
+    const int grid = static_cast<int>(n_rows < cap ? n_rows : cap);
+    shard_mask_targets_kernel<<<grid, MT_THREADS, 0, static_cast<cudaStream_t>(stream)>>>(
+        scores, n_rows, n_cols, col_offset, excluded, n_excluded_per_row, row_ptr, targets, target_scores);
+    SLB_LAUNCH_CHECK("shard_mask_targets_kernel");
     return SLB_OK;
 }
 

@@ -21,9 +21,12 @@ ties in an unspecified order.
 Test and train sets may also hold CUDA tensors (``Interactions`` / ``SequenceInteractions`` made on
 the device); each scorer downloads them once at entry.
 
-``mrr_score`` and ``precision_recall_score`` also take a ``ShardedImplicitFactorizationModel``; they
+``mrr_score`` and ``precision_recall_score`` also take a ``ShardedImplicitFactorizationModel``, and
+``sequence_mrr_score`` and ``sequence_precision_recall_score`` a ``ShardedImplicitSequenceModel``; they
 are then collective (every rank calls them with the same arguments and gets the whole result) and
-rank every target on the item shards where the items live (``spotlight_b200.sharded``).
+rank every target on the item shards where the items live (``spotlight_b200.sharded``).  A sharded
+sequence model builds each block's representations on slices of the block, from item rows fetched
+from their owners, and all-gathers them; no rank holds the whole item table.
 """
 
 import numpy as np
@@ -253,8 +256,11 @@ def sequence_mrr_score(model, test, exclude_preceding=False, sequence_block=256)
     (evaluation.py:59-102).
 
     With ``exclude_preceding`` every item of the input prefix -- padding id 0 included, as in the
-    reference -- is pushed to the bottom.  ``sequence_block`` sequences are scored at once.
+    reference -- is pushed to the bottom.  ``sequence_block`` sequences are scored at once.  A sharded
+    sequence model is scored collectively on its item shards (``sharded.sharded_sequence_mrr_score``).
     """
+    if isinstance(model, sharded.ShardedImplicitSequenceModel):
+        return sharded.sharded_sequence_mrr_score(model, test, exclude_preceding, sequence_block)
     test = _to_host(test)
     _check_items(test.sequences.reshape(-1), model._num_items)
     sequences = test.sequences[:, :-1]
@@ -273,8 +279,12 @@ def sequence_precision_recall_score(model, test, k=10, exclude_preceding=False, 
 
     Hits count the distinct target items (padding id 0 counts as an item) ranked in the top k;
     precision = hits / min(k, num_items), recall = hits / k.  ``k`` must be shorter than the
-    sequences.  Exact score ties across the k boundary are ordered by ascending item id.
+    sequences.  Exact score ties across the k boundary are ordered by ascending item id.  A sharded
+    sequence model is scored collectively on its item shards
+    (``sharded.sharded_sequence_precision_recall_score``).
     """
+    if isinstance(model, sharded.ShardedImplicitSequenceModel):
+        return sharded.sharded_sequence_precision_recall_score(model, test, k, exclude_preceding, sequence_block)
     test = _to_host(test)
     S = test.sequences.shape[1]
     if not 0 < k < S:

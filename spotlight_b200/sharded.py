@@ -376,6 +376,47 @@ class GpuBackend(object):
                    'rank_counts')
         return out
 
+    # ---- sequence evaluation on the item shards (sequence scorers, predict) ----
+    def seq_representation(self, E_cache, seqs_idx, cnn, lstm, mixture):
+        """(n, S+1, width) causal representations of the sequences ``seqs_idx`` (ids remapped onto
+        the row cache ``E_cache``, cache row 0 the padding row): ops.seq_representation, the kernels
+        ``user_representation`` runs on a plain table.  width is D, or 2MD with ``mixture``."""
+        return ops.seq_representation(E_cache, seqs_idx, cnn, lstm=lstm, mixture=mixture)
+
+    def seq_dot_scores(self, final, items, item_bias):
+        """(len(final), len(items)) scores of the dot head with the arithmetic of
+        evaluation._score_sequences: the GEMM, then += item bias (no user bias)."""
+        out = final @ items.t()                             # plain library GEMM (cuBLAS)
+        out += item_bias.reshape(1, -1)
+        return out
+
+    def mixture_scores(self, final, items, item_bias):
+        """(n, len(items)) scores of MixtureLSTMNet's mixture-of-tastes head for the final
+        representations ``final`` (n, 2M, D): one slb_mixture_scores launch over the given rows."""
+        n, two_m, dim = final.shape
+        final, items, item_bias = final.contiguous(), items.contiguous(), item_bias.reshape(-1).contiguous()
+        out = torch.empty((n, items.shape[0]), dtype=torch.float32, device=final.device)
+        _lib.check(_lib.load().slb_mixture_scores(ops._ptr(final), n, two_m // 2, dim, ops._ptr(items),
+                                                  ops._ptr(item_bias), items.shape[0], ops._ptr(out), ops._stream()),
+                   'mixture_scores')
+        return out
+
+    def shard_mask_targets(self, scores, col_offset, excluded, row_ptr, targets):
+        """slb_shard_mask_targets: writes -FLOAT_MAX, in place, over the excluded ids (device (n, L)
+        int64, or None) inside the contiguous block's columns [col_offset, col_offset +
+        scores.shape[1]) and returns the targets' scores (0 for a target outside the block).
+        ``row_ptr`` and ``targets`` are host arrays in global item ids."""
+        dev = scores.device
+        rp = torch.from_numpy(np.ascontiguousarray(row_ptr, dtype=np.int64)).to(dev)
+        tg = torch.from_numpy(np.ascontiguousarray(targets, dtype=np.int64)).to(dev)
+        out = torch.empty(tg.numel(), dtype=torch.float32, device=dev)
+        ex = None if excluded is None else excluded.contiguous()
+        _lib.check(_lib.load().slb_shard_mask_targets(ops._ptr(scores), scores.shape[0], scores.shape[1], col_offset,
+                                                      ops._ptr(ex), 0 if ex is None else ex.shape[1], ops._ptr(rp),
+                                                      ops._ptr(tg), ops._ptr(out), ops._stream()),
+                   'shard_mask_targets')
+        return out
+
     def seq_local_step(self, E_cache, bias_cache, n_cache, seqs_idx, negs_idx, loss, cnn, norm_count,
                        lstm=None, mixture=None, n_neg=1):
         """Fused sequence step on the row cache (ids already remapped onto it; cache
@@ -958,6 +999,11 @@ class ShardedImplicitSequenceModel(object):
     Nets: PoolNet, CNNNet, LSTMNet, MixtureLSTMNet on a plain
     ``ScaledEmbedding(padding_idx=0)`` within the fused step's limits (``net.fusable()``); any
     other net raises ``ValueError``.
+
+    Evaluation, on the shards: ``evaluation.sequence_mrr_score`` and
+    ``evaluation.sequence_precision_recall_score`` take this model, and :meth:`predict` scores items
+    for one sequence; all three are collective (every rank calls them with the same arguments and
+    gets the whole result) and gather no table whole.
     """
 
     def __init__(self, num_items, rank, world, device, loss='pointwise', representation='pooling',
@@ -1039,7 +1085,8 @@ class ShardedImplicitSequenceModel(object):
 
     def gathered_net(self):
         """Collective: the representation module on this rank's device with the full trained item
-        table and bias (all-gathered from the shards) and the replicated parameters."""
+        table and bias (all-gathered from the shards) and the replicated parameters.  The sequence
+        scorers and :meth:`predict` score the sharded model itself, without gathering it."""
         st, plan = self.state, self.plan
         full = []
         for shard in (st.Wi, st.bi.reshape(-1, 1)):
@@ -1062,6 +1109,106 @@ class ShardedImplicitSequenceModel(object):
             for prm, (val, _) in zip(mine, st.replicated()):
                 prm.copy_(val.reshape(prm.shape))
         return net
+
+    # ------------------------------------------------------------------ evaluation
+    def _final_representations(self, seqs):
+        """Collective: the final representations of the block ``seqs`` (host int64 (n, S), the same on
+        every rank), in block order on every rank: (n, D), or (n, 2M, D) for MixtureLSTMNet (block j
+        of the projection's channels j*D + d, the layout evaluation._mixture_block scores).
+
+        Rank r builds those of its contiguous slice ``_rank_slice(n, r, world)`` on a row cache of the
+        slice's distinct items, fetched from their owners as a training step fetches them, with id 0
+        forced in so that padding lands on cache row 0 (PoolNet's mask reads the row's values).  A rank
+        with an empty slice still serves its peers' rows.  The slices, padded to ceil(n / world) rows,
+        are all-gathered."""
+        st, be, seq, world = self.state, self.backend, self.seq, self.world
+        n, S = seqs.shape
+        a, c = _rank_slice(n, self.rank, world)
+        mine = be.to_device(np.ascontiguousarray(seqs[a:c], dtype=np.int64))
+        cache_rows, _, inverse, _, _ = seq._fetch_rows(torch.cat([mine.reshape(-1), mine.new_zeros(1)]))
+        D = st.Wi.shape[1]
+        width = D if st.mixture is None else 2 * st.mixture['num_mixtures'] * D
+        per = -(-n // world)
+        part = cache_rows.new_zeros((per, width))
+        if c > a:
+            cnn = None
+            if seq.cnn is not None:
+                cnn = dict(seq.cnn, weights=[w for w, _ in st.convs], biases=[b for _, b in st.convs])
+            rep = be.seq_representation(cache_rows, inverse[:(c - a) * S].reshape(c - a, S), cnn, st.lstm,
+                                        st.mixture)
+            part[:c - a] = rep[:, -1]
+        full = part.new_empty((world * per, width))
+        dist.all_gather_into_tensor(full, part, group=seq.group)
+        sizes = [hi - lo for lo, hi in (_rank_slice(n, r, world) for r in range(world))]
+        final = full[be.to_device(np.concatenate([r * per + np.arange(m) for r, m in enumerate(sizes)]))]
+        return final if st.mixture is None else final.reshape(n, -1, D)
+
+    def _shard_scores(self, final, items, item_bias):
+        """(n, len(items)) scores of the final representations against the item rows given, with
+        the single-GPU scorer's arithmetic: the dot head's GEMM then += bias, or the mixture head."""
+        if self.state.mixture is None:
+            return self.backend.seq_dot_scores(final, items, item_bias)
+        return self.backend.mixture_scores(final, items, item_bias)
+
+    def _eval_blocks(self, inputs, targets, exclude_preceding, sequence_block):
+        """Collective: yields (first row, (3, n * k) int64 counts gt, eq, eq_before over all items) for
+        every block of ``sequence_block`` input sequences; ``targets`` (n_seq, k) holds each
+        sequence's targets in global item ids.
+
+        Per block: the final representations are built on the slices and all-gathered, each rank
+        scores them against its item range, pushes the block's input items inside the range to the
+        bottom (``exclude_preceding``) and reads the targets it owns (slb_shard_mask_targets); the
+        targets' scores, then the rank counts of every range, are all-reduced.  A rank that owns no
+        items scores nothing and joins every collective."""
+        st, be, group = self.state, self.backend, self.seq.group
+        k = targets.shape[1]
+        for lo in range(0, len(inputs), sequence_block):
+            blk = np.ascontiguousarray(inputs[lo:lo + sequence_block], dtype=np.int64)
+            n = len(blk)
+            final = self._final_representations(blk)
+            if st.ihi == st.ilo:
+                scores = final.new_empty((n, 0))
+            else:
+                if st.mixture is None:
+                    # the operand layout evaluation._score_sequences hands its GEMM (the last step of an
+                    # (n, S+1, D) representation), so that the library takes the same algorithm for it
+                    steps = final.new_empty((n, blk.shape[1] + 1, final.shape[1]))
+                    steps[:, -1] = final
+                    final = steps[:, -1]
+                scores = self._shard_scores(final, st.Wi, st.bi)
+            tg = targets[lo:lo + n].reshape(-1)
+            row_ptr = np.arange(n + 1) * k
+            target_scores = be.shard_mask_targets(scores, st.ilo, be.to_device(blk) if exclude_preceding else None,
+                                                  row_ptr, tg)
+            dist.all_reduce(target_scores, group=group)
+            counts = be.rank_counts(scores, st.ilo, row_ptr, tg, target_scores)
+            dist.all_reduce(counts, group=group)
+            yield lo, counts.cpu().numpy().astype(np.int64)
+
+    def predict(self, sequences, item_ids=None):
+        """Collective: scores of ``item_ids`` (all items when None) as the next item of one sequence,
+        a flat NumPy array on every rank -- ``ImplicitSequenceModel.predict``'s arguments and result.
+        Every rank calls it with the same arguments.  Each rank scores the requested items it owns,
+        from their rows gathered contiguously, against the sequence's final representation; the
+        zero-filled outputs are all-reduced.  ``fit()`` leaves every row current, so the model can be
+        scored as it stands."""
+        st, be = self.state, self.backend
+        seqs = np.atleast_2d(sequences).astype(np.int64).reshape(1, -1)
+        items = (np.arange(self._num_items, dtype=np.int64) if item_ids is None
+                 else np.asarray(item_ids).astype(np.int64).reshape(-1))
+        for ids in (items, seqs):                   # every rank raises before any collective
+            if ids.size and ids.max() >= self._num_items:
+                raise ValueError('Maximum item id greater than number of items in model.')
+            if ids.size and ids.min() < 0:
+                raise ValueError('Item ids must not be negative.')
+        final = self._final_representations(seqs)
+        own = np.nonzero((items >= st.ilo) & (items < st.ihi))[0]
+        out = torch.zeros(len(items), dtype=torch.float32, device=st.Wi.device)
+        if len(own):
+            rows, bias = be.gather(st.Wi, st.bi, be.to_device(items[own] - st.ilo))
+            out[be.to_device(own)] = self._shard_scores(final, rows, bias)[0]
+        dist.all_reduce(out, group=self.seq.group)
+        return out.cpu().numpy()
 
 
 class ShardedImplicitFactorizationModel(object):
@@ -1703,3 +1850,46 @@ def sharded_precision_recall_score(model, test, train=None, k=10, user_block=204
     precision = hits / np.minimum(ks, model._num_items).reshape(1, -1).astype(np.float64)
     recall = hits / n_test.reshape(-1, 1).astype(np.float64)
     return precision.squeeze(), recall.squeeze()
+
+
+def sharded_sequence_mrr_score(model, test, exclude_preceding=False, sequence_block=256):
+    """Collective ``evaluation.sequence_mrr_score`` of a :class:`ShardedImplicitSequenceModel`: every
+    rank calls it with the same arguments and gets the whole result.  Each rank ranks the last item
+    of every test sequence among its own item range (:meth:`ShardedImplicitSequenceModel._eval_blocks`);
+    the summed counts are those of the whole score row, so the result equals the single-GPU scorer's
+    on ``gathered_net()``, ties included, wherever the per-range scores reproduce the full row's."""
+    from spotlight_b200.evaluation import _check_items
+    from spotlight_b200.interactions import _to_host
+    test = _to_host(test)
+    _check_items(test.sequences.reshape(-1), model._num_items)
+    sequences = test.sequences[:, :-1]
+    out = np.empty(len(sequences), dtype=np.float64)
+    for lo, counts in model._eval_blocks(sequences, test.sequences[:, -1:].astype(np.int64), exclude_preceding,
+                                         sequence_block):
+        ranks, _ = _finalize_ranks(counts)
+        out[lo:lo + len(ranks)] = 1.0 / ranks
+    return out
+
+
+def sharded_sequence_precision_recall_score(model, test, k=10, exclude_preceding=False, sequence_block=256):
+    """Collective ``evaluation.sequence_precision_recall_score`` of a
+    :class:`ShardedImplicitSequenceModel` (see :func:`sharded_sequence_mrr_score`): hits count the
+    distinct targets among the last k items ranked in the top k; precision = hits / min(k,
+    num_items), recall = hits / k; ties across the k boundary ordered by ascending item id."""
+    from spotlight_b200.evaluation import _check_items, _hits_at
+    from spotlight_b200.interactions import _to_host
+    test = _to_host(test)
+    S = test.sequences.shape[1]
+    if not 0 < k < S:
+        raise ValueError('k = %d must be in [1, sequence length %d)' % (k, S))
+    _check_items(test.sequences.reshape(-1), model._num_items)
+    sequences = test.sequences[:, :-k]
+    targets = np.sort(test.sequences[:, -k:].astype(np.int64), axis=1)
+    unique = np.ones(targets.shape, dtype=bool)
+    unique[:, 1:] = targets[:, 1:] != targets[:, :-1]
+    hits = np.empty(len(sequences), dtype=np.int64)
+    for lo, counts in model._eval_blocks(sequences, targets, exclude_preceding, sequence_block):
+        _, pos = _finalize_ranks(counts)
+        n = len(pos) // k
+        hits[lo:lo + n] = _hits_at(pos, np.arange(n + 1) * k, [k], unique[lo:lo + n].reshape(-1))[:, 0]
+    return hits / float(min(k, model._num_items)), hits / float(k)
